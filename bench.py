@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- audio-seconds per second of ToneColorConverter.convert on B200 (BASELINE.json metric).
+"""bench.py -- audio-seconds per second of ToneColorConverter.convert on H100 (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch 32] [--secs 10] [--impl native|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch 32] [--secs 10] [--impl native|reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path over one batch of synthetic utterances.  The default
-workload is BASELINE.json configs[1]: batch 32 x 10 s clips at 22.05 kHz on one B200, in the
+workload is BASELINE.json configs[1]: batch 32 x 10 s clips at 22.05 kHz on one H100, in the
 default arithmetic mode (--precision f16x3: split-precision fp16 tensor-core convolutions, fp32-grade
 results -- stricter than the config's "fp16"; fp32 = CUDA cores only, f16 = single pass).  The
 other modes are timed briefly in the same run and reported under "modes_audio_s_per_s".  For N > 1 launch under torchrun: one rank per
@@ -20,10 +20,16 @@ One JSON line on stdout (rank 0):
              ToneColorConverter.convert_batch is timed beside it (`e2e_convert_batch`)
   roofline   generator ResBlock conv family (90 % of the FLOPs), timed live with CUDA events around every launch:
              ALGORITHMIC TFLOP/s (2*MAC of the reference's convs, no credit for the 3 split-precision passes) over
-             the measured dense fp16/bf16 tensor peak; pipe occupancy, HBM figures and a per-kernel table beside it
+             the dense fp16/bf16 tensor peak; pipe occupancy, HBM figures and a per-kernel table beside it
   cudnn_baseline  the reference's own torch graph (oracle port, F.conv1d -> cuDNN) on this GPU, TF32 on and off
   cpu_baseline  the oracle port of the reference's CPU path on this box's host cores (N=1 only)
 --impl reference times that CPU path alone (the reference arm).
+--dump-outputs DIR writes what the last timed step of the device-resident leg returned (o_hat.npy: the converted waveforms
+[B, T * hop] float32; frames.npy: the frame counts, float64), at most 64 MB in all.  When the waveforms are larger, a fixed
+sample (seed 0) of whole utterances is kept and their indices written to o_hat_rows.npy; when even one utterance is too
+large, a fixed sample of sample positions of every utterance is kept instead, indices in o_hat_cols.npy (float64).
+Inputs, checkpoint and noise seeds depend only on the arguments, so two builds run with the same arguments can be
+compared output for output.
 """
 import argparse
 import json
@@ -42,16 +48,39 @@ sys.path.insert(0, ROOT)
 SR = 22050
 HOP = 256
 GFLOP_PER_FRAME = 0.65766          # SURVEY.md section 8d: 657.66 MFLOP per spectrogram frame
-FFMA_PEAK_TFLOPS = 74.4            # nominal 148 SM x 128 lanes x 2 x 1.965 GHz (fallback)
+# H100 SXM data sheet (700 W card): dense fp32 FMA, dense fp16 / bf16 tensor and HBM3 peaks
+FFMA_PEAK_TFLOPS = 67.0
+TC_PEAK_TFLOPS = 989.0
+HBM_PEAK_GBS = 3350.0
 
 
 def ffma_peak():
-    """fp32 FMA peak of this pool's B200s as tools/ffma_bench.cu measured it (profiles/r02_ffma_peak.json), else nominal"""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "r02_ffma_peak.json")))
-        return float(d["ffma_peak_tflops"]), "measured (tools/ffma_bench.cu, profiles/r02_ffma_peak.json)"
-    except Exception:
-        return FFMA_PEAK_TFLOPS, "nominal 148 SM x 128 lanes x 2 x 1.965 GHz"
+    return FFMA_PEAK_TFLOPS, "H100 SXM data sheet, dense fp32"
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def dump_outputs(d, out, frames):
+    """out [B, N] float32 and frames [B] -> d/*.npy, at most DUMP_LIMIT bytes in all (seeded sample when larger)."""
+    import torch
+    os.makedirs(d, exist_ok=True)
+    B, N = out.shape
+    budget = DUMP_LIMIT - 16 * B - 4 * 4096        # frames + a row index, .npy headers
+    rng = np.random.default_rng(0)
+    arrays = {"frames": frames.cpu().numpy().astype(np.float64)}
+    if B * N * 4 <= budget:
+        arrays["o_hat"] = out.cpu().numpy()
+    elif N * 4 <= budget:
+        rows = np.sort(rng.choice(B, budget // (N * 4), replace=False))
+        arrays["o_hat"] = out[torch.from_numpy(rows).to(out.device)].cpu().numpy()
+        arrays["o_hat_rows"] = rows.astype(np.float64)
+    else:
+        cols = np.sort(rng.choice(N, budget // (4 * B + 8), replace=False))
+        arrays["o_hat"] = out[:, torch.from_numpy(cols).to(out.device)].cpu().numpy()
+        arrays["o_hat_cols"] = cols.astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), a.astype(np.float32 if name == "o_hat" else np.float64))
 
 
 def synth_wave(i, secs):
@@ -66,7 +95,7 @@ def synth_se(i, base):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -316,8 +345,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--precision", default=os.environ.get("OVC_PRECISION", "f16x3"), choices=["fp32", "f16x3", "f16"],
                     help="conv arithmetic: f16x3 = split-precision fp16 tensor cores (default, fp32-grade), "
-                         "fp32 = CUDA-core FFMA2, f16 = single-pass fp16 (11-bit operands, the reference's own GPU default class)")
-    ap.add_argument("--wide-variant", type=int, default=None, help="tiling of the 128-column tensor-core kernel (ovc_set_option)")
+                         "fp32 = CUDA-core FFMA, f16 = single-pass fp16 (11-bit operands, the reference's own GPU default class)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--no-config3", action="store_true", help="skip the BASELINE config-3 side measurement (V1 TTS + convert, batch 16)")
     ap.add_argument("--no-modes", action="store_true", help="skip the short side measurements of the other precisions")
     ap.add_argument("--no-cudnn", action="store_true", help="skip the reference-on-this-GPU (PyTorch / cuDNN) column")
@@ -357,8 +387,6 @@ def main():
             json.dump(hp, open(cfg, "w"))
             cv = ToneColorConverter(cfg, device=dev, enable_watermark=False, precision=args.precision)
         cv.model.load_state_dict(sd)
-        if args.wide_variant is not None:
-            cv.model.native.set_option("wide_variant", args.wide_variant)
         return cv
 
     conv = make_converter()
@@ -407,6 +435,9 @@ def main():
     barrier()
     ms_dev = max_over_ranks(e0.elapsed_time(e1)) / args.steps
     launches_per_call = native.last_launch_count
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        # what the caller of the timed path receives from its last step, before any later leg reuses the buffers
+        dump_outputs(args.dump_outputs, out_dev, frames_dev)
 
     # ---- per-kernel leg (roofline): the same steps again with CUDA events around every conv launch
     native.profile_enable(True)
@@ -523,13 +554,8 @@ def main():
             dist.destroy_process_group()
         return
 
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured" if "hbm_gbs" in peaks else "fallback"
+    hbm_peak = HBM_PEAK_GBS
+    peak_src = "H100 SXM data sheet"
     k_ms = prof["ms"] / max(1, prof["launches"])
     ach_gbs = prof["bytes"] / max(1e-9, prof["ms"] * 1e-3) / 1e9
     ach_tf = prof["flops"] / max(1e-9, prof["ms"] * 1e-3) / 1e12
@@ -539,46 +565,18 @@ def main():
     for name, ms, fl, by, f in detail:
         if not f:
             continue
-        key = {"T128": "tcconv_wide_kernel<1> / tcconv_kernel<128> (C >= 128)", "T64c": "tcconv_kernel<64> (C = 64)",
-               "T32c": "tcconv_kernel<32> (C = 32)", "P32k": "tcpair_kernel<32> (C = 32, fused k = 3 conv pairs; 2 convs per launch)",
-               "P64k": "tcpair_kernel<64> (C = 64, fused k = 3 conv pairs; 2 convs per launch)"
+        key = {"T128": "tcconv_kernel<128> (C >= 128)", "T64c": "tcconv_kernel<64> (C = 64)",
+               "T32c": "tcconv_kernel<32> (C = 32)", "P32k": "tcconv_kernel<32, pair> (C = 32, fused k = 3 conv pairs; 2 convs per launch)",
+               "P64k": "tcconv_kernel<64, pair> (C = 64, fused k = 3 conv pairs; 2 convs per launch)"
                }.get(name[:4], "conv1d_f32 (CUDA cores)")
         a = fam.setdefault(key, [0, 0.0, 0.0, 0.0])
         a[0] += 1; a[1] += ms; a[2] += fl; a[3] += by
 
-    def ncu_traffic(pattern):
-        """dram read + write bytes of one launch of the dominant kernel from the committed ncu --set full capture"""
-        import glob
-        for path in sorted(glob.glob(os.path.join(ROOT, "profiles", pattern))):
-            try:
-                cap = json.load(open(path))
-                cap = cap[0] if isinstance(cap, list) else cap
-                rd, wr = cap["dram__bytes_read.sum"].split(), cap["dram__bytes_write.sum"].split()
-                unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-                return ((float(rd[0]) * unit.get(rd[1], 1.0) + float(wr[0]) * unit.get(wr[1], 1.0)),
-                        f"{os.path.basename(path)}: {cap.get('what', 'ncu --set full, one launch')}")
-            except Exception:
-                continue
-        return None, None
-
-    def ncu_dram_pass():
-        """average DRAM bytes per ResBlock conv launch from the committed single-pass ncu run of THIS workload (batch 32 x 10 s,
-        f16x3: tools/gpu_ncu.sh -> tools/summarize_ncu.py dram); only valid for the default batch / length / precision"""
-        import glob
-        if (B, secs, args.precision) != (32, 10.0, "f16x3"):
-            return None, "no ncu DRAM pass for this batch / length / precision (committed one: batch 32 x 10 s, f16x3)"
-        paths = sorted(glob.glob(os.path.join(ROOT, "profiles", "r02*_ncu_dram_b32_f16x3.json")))
-        if not paths:
-            return None, None
-        cap = json.load(open(paths[-1]))
-        return cap["dram_bytes_per_launch_avg"], f"{os.path.basename(paths[-1])}: {cap['what']} (average over the 72 launches)"
-
     if args.precision == "fp32":
-        traffic, traffic_note = ncu_traffic("r0*_ncu_full_A_K11D1_ffma2.json")
         roofline = {
             "kernel": "conv1d_f32<EPI_LINEAR> (generator ResBlock1 convs, 72 launches per call)",
             "bound": "hbm", "achieved": ach_gbs, "peak": hbm_peak, "unit": "GB/s", "frac": ach_gbs / hbm_peak,
-            "traffic": traffic, "traffic_note": traffic_note, "peak_source": peak_src,
+            "peak_source": peak_src,
             "avg_launch_ms": k_ms, "launches": prof["launches"], "share_of_step": prof["ms"] / args.steps / ms_prof_step,
             "binding": "fp32 FFMA (dense contraction, SURVEY.md section 8d)",
             "ffma": {"achieved": ach_tf, "peak": ffma_peak()[0], "unit": "TFLOP/s", "frac": ach_tf / ffma_peak()[0],
@@ -588,17 +586,16 @@ def main():
         # tensor-core modes.  achieved = ALGORITHMIC FLOPs (2*MAC of the reference's convs) / CUDA-event time; the split
         # precision spends 3 tensor FLOPs per algorithmic FLOP, which shows up as pipe_occupancy, not as achieved work.
         passes = 3 if args.precision == "f16x3" else 1
-        tc_peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
-        traffic, traffic_note = ncu_dram_pass()
+        tc_peak = TC_PEAK_TFLOPS
         roofline = {
-            "kernel": "tcconv_kernel<128|64|32> + tcconv_wide_kernel<1> (C = 256, k >= 7) + tcpair_kernel<64|32> (fused k = 3 conv pairs): "
-                      f"the 72 generator ResBlock1 convs on tcgen05, {prof['launches'] // max(1, args.steps)} launches per call",
+            "kernel": "tcconv_kernel<128|64|32> + tcconv_kernel<64|32, pair> (fused conv pairs): "
+                      f"the 72 generator ResBlock1 convs on wgmma, {prof['launches'] // max(1, args.steps)} launches per call",
             "bound": "tensor", "achieved": ach_tf, "peak": tc_peak, "unit": "TFLOP/s", "frac": ach_tf / tc_peak,
-            "frac_note": "algorithmic FLOPs / time / measured dense 16-bit tensor peak; the fp32-grade split precision needs "
+            "frac_note": "algorithmic FLOPs / time / data-sheet dense 16-bit tensor peak; the fp32-grade split precision needs "
                          "3 MMA passes, so 1/3 is the ceiling of this mode",
             "mma_passes": passes, "pipe_occupancy": ach_tf * passes / tc_peak,
-            "traffic": traffic, "traffic_note": traffic_note, "algorithmic_bytes_per_launch": prof["bytes"] / max(1, prof["launches"]),
-            "peak_source": ("measured" if "bf16_tflops_sustained" in peaks else "fallback") + " dense bf16/fp16 sustained (MEASURED_PEAKS.json)",
+            "algorithmic_bytes_per_launch": prof["bytes"] / max(1, prof["launches"]),
+            "peak_source": "H100 SXM data sheet, dense bf16/fp16",
             "avg_launch_ms": k_ms, "launches": prof["launches"], "share_of_step": prof["ms"] / args.steps / ms_prof_step,
             "hbm": {"achieved": ach_gbs, "peak": hbm_peak, "unit": "GB/s", "frac": ach_gbs / hbm_peak, "peak_source": peak_src,
                     "note": "layer-granular algorithmic bytes (SURVEY 8d tier T2: in + out per conv) / time"},
@@ -611,11 +608,11 @@ def main():
     line = {
         "metric": "audio_seconds_per_second", "value": value, "unit": "audio-s/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms_dev, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": {"fp32": "f32", "f16x3": "f32 (3xFP16 split-precision tensor-core convs with fp32 accumulation, fp32 FFMA2 elsewhere)",
+        "dtype": {"fp32": "f32", "f16x3": "f32 (3xFP16 split-precision tensor-core convs with fp32 accumulation, fp32 FFMA elsewhere)",
                   "f16": "f16 operands, f32 accumulation (single-pass tensor-core convs, fp32 elsewhere)"}[args.precision],
         "data": "synthetic", "precision": args.precision, "modes_audio_s_per_s": modes,
         "config": dict(workload_config(B, secs, world),
-                       l2="activations per step (>3 GB) exceed the 126 MB L2; no explicit flush",
+                       l2="activations per step (>3 GB) exceed the 50 MB L2; no explicit flush",
                        parallelism=f"replicas x{world}" + (f", rank 0 pinned to {numa}" if numa else ""), e2e_api=e2e_api),
         "tflops_algorithmic": world * B * T * GFLOP_PER_FRAME / ms_dev,
         "e2e": {"value": e2e_val, "unit": "audio-s/s", "ms_per_step": ms_e2e,

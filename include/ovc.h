@@ -1,7 +1,7 @@
 /*
  * ovc.h -- C ABI of libovc_b200.so: the tone-colour-converter hot path of OpenVoice
  * (ToneColorConverter.convert -> SynthesizerTrn.voice_conversion) as hand-written
- * sm_100a CUDA kernels.
+ * sm_90a (H100) CUDA kernels.
  *
  * The reference has no FFI / plugin interface (it is pure Python; SURVEY.md section 8b).  The
  * boundary this library replaces is the Python seam
@@ -25,7 +25,8 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 2   /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR */
+#define OVC_ABI_VERSION 3   /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+                               * activation TMA, tune bits) removed */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -72,7 +73,7 @@ OVC_API int ovc_abi_version(void);
 OVC_API const char* ovc_last_error(void);
 
 /* Build a converter context on CUDA device `device` (replaces SynthesizerTrn construction,
- * openvoice/api.py:23-30).  Fails with OVC_ERR_CUDA when no usable sm_100 device exists. */
+ * openvoice/api.py:23-30).  Fails with OVC_ERR_CUDA when no usable sm_90 device exists. */
 OVC_API int ovc_create(const ovc_hparams* hp, int device, ovc_ctx** out);
 OVC_API void ovc_destroy(ovc_ctx* ctx);
 
@@ -167,8 +168,8 @@ OVC_API int ovc_tts_decode(ovc_ctx* ctx, const float* noise, uint64_t seed, floa
                            int ragged, float* o, float* z, float* z_p, void* stream);
 
 /* Arithmetic of the convolutions (generator ResBlocks = 90 % of the FLOPs, WaveNet stacks, upsamplers):
- *   0            fp32 FFMA2 on the CUDA cores
- *   1 (default of the Python surface)  split-precision "3xFP16" on the 5th-gen tensor cores (tcgen05 + TMEM):
+ *   0            fp32 FFMA on the CUDA cores
+ *   1 (default of the Python surface)  split-precision "3xFP16" on the Hopper tensor cores (wgmma):
  *                x = hi + lo / 2^11 with hi = fp16(x), lo = fp16((x - hi) * 2^11); every product is
  *                a_hi*b_hi + (a_lo*b_hi + a_hi*b_lo) / 2^11, fp32 accumulation, cross terms in their own
  *                accumulator -- fp32-grade error, same parity gate as mode 0.  Operands must be < 65504 in magnitude.
@@ -177,29 +178,19 @@ OVC_API int ovc_tts_decode(ovc_ctx* ctx, const float* noise, uint64_t seed, floa
 OVC_API int ovc_set_precision(ovc_ctx* ctx, int mode);
 
 /* Tuning / diagnostics switches (never change results beyond fp32 reordering):
- *   OVC_OPT_WIDE_VARIANT  kernel of the 128-column tensor-core layers: 0 the persistent kernel (one CTA per SM,
- *                         TMA-staged activations, overlapped epilogue); 1: one 256-step tile per CTA; 2: one 128-step
- *                         tile per CTA, two CTAs per SM; 3 (default): 2 for k >= 7 at Cin >= 256, else 0
  *   OVC_OPT_TTS_SIMPLE    1: one-thread-per-element text-side kernels (the CPU-checked element functions) instead of
  *                         the warp-cooperative LayerNorm / fused attention
- *   OVC_OPT_ACT_TMA       1 (default): the persistent conv kernel receives its activation tiles by tensor-map TMA;
- *                         0: its converter warps load them from global memory
  *   OVC_OPT_GRAPH         1 (default): replay the launch sequence of a repeated (shape, buffers) call from a CUDA graph
  *   OVC_OPT_PDL           programmatic stream serialization of the tensor-core conv launches (the prologue of kernel n+1 --
- *                         barriers, TMEM, weight TMA -- overlaps the drain of kernel n): 0 off, 1 all of them, 2 (default)
- *                         the WaveNet stacks only.  Measured on a B200: 2 saves 0.5-0.8 % at batch 32 and 2.4 % at batch 1;
- *                         1 costs 3 % at batch 32 */
-#define OVC_OPT_WIDE_VARIANT 1
+ *                         barriers, weight TMA -- overlaps the drain of kernel n): 0 off, 1 all of them, 2 (default)
+ *                         the WaveNet stacks only */
 #define OVC_OPT_TTS_SIMPLE 2
 #define OVC_OPT_GRAPH 3
-#define OVC_OPT_ACT_TMA 4
 #define OVC_OPT_PDL 5
-#define OVC_OPT_TUNE 6       /* A/B bits of the persistent conv kernel: 1 = L2 prefetch of the residual tile (default off),
-                              * 2 = two items per converter iteration (default on) */
 #define OVC_OPT_BRANCHES 7   /* 1 (default): latency-bound calls (B * Tmax <= 512 frames) run the three ResBlock branches of an
                               * MRF stage concurrently (three streams, a third of the SMs per kernel); results are bit-identical */
 #define OVC_OPT_PAIR 8       /* 1 (default): the HBM-bound ResBlock conv pairs (C <= 64, k = 3) run as ONE kernel each
-                              * (ovc_tcpair.cuh): the intermediate activation stays in shared memory; same bits as two launches */
+                              * (tcconv_kernel<C, true>): the intermediate activation stays in shared memory */
 OVC_API int ovc_set_option(ovc_ctx* ctx, int key, int value);
 
 /* Number of kernels the last ovc_voice_conversion / ovc_convert_waveform call launched. */

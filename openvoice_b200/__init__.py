@@ -1,4 +1,4 @@
-"""openvoice_b200 -- B200-native (sm_100a) tone-colour-converter hot path of OpenVoice.
+"""openvoice_b200 -- H100-native (sm_90a) tone-colour-converter hot path of OpenVoice.
 
 Drop-in surface of the reference's ``openvoice.api`` / ``openvoice.se_extractor`` for the
 ``ToneColorConverter.convert -> SynthesizerTrn.voice_conversion`` path; the arithmetic runs in

@@ -1,7 +1,7 @@
 """ctypes binding of libovc_b200.so (C ABI: include/ovc.h).
 
 PyTorch is used for device memory and streams only; every tensor crosses the boundary as a raw
-device pointer.  If the library is missing or no sm_100 GPU is present this module raises --
+device pointer.  If the library is missing or no sm_90 GPU is present this module raises --
 there is no fallback path of any kind.
 """
 from __future__ import annotations
@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -53,7 +53,7 @@ def load_library(path: Optional[str] = None):
     path = path or os.environ.get("OVC_B200_LIB", LIB_PATH)
     if not os.path.exists(path):
         raise OvcError(
-            f"{path} not found: build the sm_100a extension first "
+            f"{path} not found: build the sm_90a extension first "
             "(python -c 'import __graft_entry__ as g; g.build()' or make -C openvoice_b200/csrc). "
             "openvoice_b200 has no CPU / PyTorch fallback.")
     lib = C.CDLL(path)
@@ -153,10 +153,6 @@ class NativeConverter:
         self.handle = h
         self.device_index = int(device_index)
         self.finalized = False
-        if os.environ.get("OVC_WIDE_VARIANT"):      # tuning experiments: kernel of the 128-column tensor-core layers
-            self.set_option("wide_variant", int(os.environ["OVC_WIDE_VARIANT"]))
-        if os.environ.get("OVC_ACT_TMA"):
-            self.set_option("act_tma", int(os.environ["OVC_ACT_TMA"]))
 
     def close(self):
         if getattr(self, "handle", None):
@@ -191,14 +187,14 @@ class NativeConverter:
         self.finalized = True
 
     def set_precision(self, mode: str):
-        """'fp32' (CUDA-core FFMA2), 'f16x3' (split-precision fp16 tensor-core convs, fp32-grade) or 'f16' (single pass)."""
+        """'fp32' (CUDA-core FFMA), 'f16x3' (split-precision fp16 tensor-core convs, fp32-grade) or 'f16' (single pass)."""
         m = PRECISIONS[mode]
         _check(self.lib, self.lib.ovc_set_precision(self.handle, m), "ovc_set_precision")
         self.precision = mode
 
     def set_option(self, key: str, value: int):
-        """Tuning switches of include/ovc.h: 'wide_variant' (0..3), 'tts_simple', 'graph', 'act_tma', 'pdl' (0/1/2), 'tune' (bits), 'branches', 'pair' (0/1)."""
-        k = {"wide_variant": 1, "tts_simple": 2, "graph": 3, "act_tma": 4, "pdl": 5, "tune": 6, "branches": 7, "pair": 8}[key]
+        """Tuning switches of include/ovc.h: 'tts_simple', 'graph', 'pdl' (0/1/2), 'branches', 'pair' (0/1)."""
+        k = {"tts_simple": 2, "graph": 3, "pdl": 5, "branches": 7, "pair": 8}[key]
         _check(self.lib, self.lib.ovc_set_option(self.handle, k, int(value)), "ovc_set_option")
 
     # ---- hot path --------------------------------------------------------------------------

@@ -120,12 +120,12 @@ class NativeSynthesizer:
 
     def __init__(self, hps, device: str, precision: Optional[str] = None):
         """``precision``: arithmetic of the generator's ResBlock / upsampling convolutions --
-        ``"f16x3"`` (default; split-precision fp16 on the tcgen05 tensor cores, fp32-grade),
-        ``"fp32"`` (CUDA-core FFMA2 everywhere) or ``"f16"`` (single-pass fp16: the 11-bit operand precision the
+        ``"f16x3"`` (default; split-precision fp16 on the tensor cores (wgmma), fp32-grade),
+        ``"fp32"`` (CUDA-core FFMA everywhere) or ``"f16"`` (single-pass fp16: the 11-bit operand precision the
         reference itself gets on a GPU through cuDNN's allow_tf32 default; ~1e-2).  Env override: OVC_PRECISION."""
         dev = torch.device(device)
         if dev.type != "cuda":
-            raise RuntimeError("openvoice_b200 runs on CUDA (sm_100a) only; there is no CPU path")
+            raise RuntimeError("openvoice_b200 runs on CUDA (sm_90a) only; there is no CPU path")
         self.device = dev
         self.hps = hps
         self.zero_g = bool(getattr(hps.model, "zero_g", False))

@@ -16,7 +16,6 @@
 #include "../../include/ovc.h"
 #include "ovc_small.cuh"
 #include "ovc_tcconv.cuh"
-#include "ovc_tcpair.cuh"
 #include "ovc_tts.cuh"
 #include "ovc_refenc.cuh"
 #include "ovc_variants.h"
@@ -60,22 +59,6 @@ struct DeviceGuard {
       return fail(OVC_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e_), __FILE__, \
                   __LINE__);                                                                      \
   } while (0)
-
-// cuTensorMapEncodeTiled, resolved through the runtime (no link-time dependency on libcuda)
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-  static EncodeTiledFn fn = [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess)
-      p = nullptr;
-    cudaGetLastError();
-    return reinterpret_cast<EncodeTiledFn>(p);
-  }();
-  return fn;
-}
 
 static const VariantInfo kInfo[V_COUNT] = {
 #define X(name, K, D, WM, WN, CI, EPI, NG, XA)                                                    \
@@ -133,7 +116,7 @@ struct WNLayers {
 // V1 TTS front half (TextEncoder / DurationPredictor / StochasticDurationPredictor, models.py:16-180): dense convs
 // as tensor-core layers, small fp32 parameters as offsets into the fp32 arena.  Hyper-parameters are read off the
 // checkpoint shapes (the reference takes them from config.json: api.py:26-31, models.py:451-465).
-// k = 3 convs and the whole duration chain stay on the CUDA cores in plain fp32: the FFMA2 conv kernel on a [C][T]
+// k = 3 convs and the whole duration chain stay on the CUDA cores in plain fp32: the FFMA conv kernel on a [C][T]
 // copy when the shape fits a variant (k 3, N % 64 == 0: every released checkpoint), else the one-thread-per-output
 // kernel (sequential fmaf chain over w [K][Cin][N])
 struct Fp32Dense { size_t w = 0, b = 0; int Cin = 0, K = 0, N = 0; bool fast = false; ConvLayer cl; };
@@ -188,20 +171,16 @@ struct ovc_ctx {
   TcLayer tc_c1[12][3], tc_c2[12][3], tc_ups[4], tc_pre;
   float* d_tcw = nullptr;      // tensor-core weight arena (hi/lo split)
   std::vector<float> h_tcw;
-  int precision = 0;           // 0: fp32 FFMA everywhere; 1: 3xFP16 split-precision tcgen05 convs; 2: single-pass fp16
-  int wide_variant = 3;        // kernel of the 128-column tensor-core layers (see launch_tc); 3 = chosen per layer
-  bool act_tma = true;         // OVC_OPT_ACT_TMA
+  int precision = 0;           // 0: fp32 FFMA everywhere; 1: 3xFP16 split-precision wgmma convs; 2: single-pass fp16
   bool tts_simple = false;     // OVC_OPT_TTS_SIMPLE
   bool use_graph = true;       // OVC_OPT_GRAPH
   int use_pdl = 2;             // OVC_OPT_PDL: 0 off, 1 every tensor-core conv, 2 (default) the WaveNet stacks only -- short kernels
-                               // whose fill / drain dominates (measured: 2 gives -0.5 .. -0.8 % at batch 32 and -2.4 % at
-                               // batch 1; 1 gives +3 % at batch 32)
-  int tune = 2;                // OVC_OPT_TUNE (TcConvArgs.tune)
+                               // whose fill / drain dominates
   // small calls: the three ResBlock branches of an MRF stage run concurrently on three streams, each kernel on a third
-  // of the SMs (OVC_OPT_BRANCHES; taken when B * Tmax <= par_frames = 512 frames: measured -8 % at 258 frames, +2 % at 861)
+  // of the SMs (OVC_OPT_BRANCHES; taken when B * Tmax <= par_frames = 512 frames)
   bool use_branches = true;
   int par_frames = 512;
-  bool use_pair = true;        // OVC_OPT_PAIR: the HBM-bound ResBlock conv pairs (C <= 64, k = 3) as ONE kernel (ovc_tcpair.cuh)
+  bool use_pair = true;        // OVC_OPT_PAIR: the HBM-bound ResBlock conv pairs (C <= 64, k = 3) as ONE kernel (tcconv_kernel<C, true>)
   cudaStream_t br_stream[2] = {nullptr, nullptr};
   cudaEvent_t br_ev[4] = {nullptr, nullptr, nullptr, nullptr};
   size_t post_w_off = 0;
@@ -709,13 +688,11 @@ static int finalize(ovc_ctx* c) {
   CK(cudaMemcpy(c->d_tcw, c->h_tcw.data(), c->h_tcw.size() * sizeof(float), cudaMemcpyHostToDevice));
   c->h_tcw.clear();
   c->h_tcw.shrink_to_fit();
-  CK(cudaFuncSetAttribute(tcconv_wide_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcwCfg<1>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcconv_wide_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcwCfg<2>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcconv_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<128>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcconv_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<64>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcconv_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<32>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcpair_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcpCfg<32>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcpair_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcpCfg<64>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tcconv_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<128, false>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tcconv_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<64, false>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tcconv_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<32, false>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tcconv_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<64, true>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tcconv_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<32, true>::SMEM_BYTES));
   if (c->d_cond_wrow) cudaFree(c->d_cond_wrow);
   if (c->d_cond_sel) cudaFree(c->d_cond_sel);
   CK(cudaMalloc(&c->d_cond_wrow, wrow.size() * sizeof(int)));
@@ -936,54 +913,18 @@ static int launch_tc(Run& r, const TcLayer& T, const float* x, float* y, const f
   a.Cin = T.Cin; a.Ntot = T.Ntot; a.K = T.K; a.DIL = T.DIL;
   a.slope = slope; a.scale = scale; a.accumulate = accumulate;
   a.passes = r.c->precision == 2 ? 1 : 3;
-  a.tune = r.c->tune;
   if (T.TN == 0) return fail(OVC_ERR_INVALID, "conv %d -> %d (k %d, dilation %d) does not fit the tensor-core kernels", T.Cin, T.Ntot, T.K, T.DIL);
   if (!(slope >= 0.f && slope <= 1.f)) return fail(OVC_ERR_INVALID, "leaky_relu slope %g outside [0, 1]", (double)slope);
   TRY(prof_begin(r));
-  // 3 (default): the generator's first stage (k >= 7 at C = 256: few, long tiles) on the two-CTAs-per-SM kernel, whose
-  // second CTA fills the tensor pipe while the first waits on a barrier; everything else on the persistent kernel
-  int wv = r.c->wide_variant;
-  if (wv == 3) wv = (T.K >= 7 && T.Cin >= 256) ? 2 : 0;
-  if (T.TN == 128 && wv != 0) {
-    // A/B alternatives of the 128-column layers: 1 = 256-step tiles, one CTA per SM; 2 = 128-step tiles, two CTAs per SM
-    const int MT = wv == 1 ? 2 : 1;
-    dim3 grid((t_len + MT * 128 - 1) / (MT * 128), T.Ntot / 128, r.B);
-    const bool pdl = r.c->use_pdl == 1 || (r.c->use_pdl == 2 && ex.epi != 0);
-    if (wv == 1) CK(launch_ex(tcconv_wide_kernel<2>, grid, TcwCfg<2>::THREADS, TcwCfg<2>::SMEM_BYTES, r.st, pdl, a));
-    else CK(launch_ex(tcconv_wide_kernel<1>, grid, TcwCfg<1>::THREADS, TcwCfg<1>::SMEM_BYTES, r.st, pdl, a));
-  } else {
-    // persistent: one CTA per SM walks the (utterance, tile) list; column tiles (if any) on grid.y
-    const int MT = T.TN == 128 ? TcnCfg<128>::MT : TcnCfg<64>::MT;
-    const int steps = MT * 128;
-    const int n_tt = (t_len + steps - 1) / steps, total = n_tt * r.B;
-    // activation chunks by tensor-map TMA: the channels-last input as a [B][rows][Cin] fp32 tensor, one box = box_rows x 32
-    // channels (128 bytes, 128-byte swizzle); rows outside the tensor are zero-filled by the copy engine
-    CUtensorMap tmap;
-    memset(&tmap, 0, sizeof tmap);
-    a.act_tma = 0;
-    if (r.c->act_tma && encode_tiled_fn()) {
-      const int rows = tcn_rows(MT, (T.K - 1) / 2 * T.DIL);
-      a.n_box = rows > 256 ? 2 : 1;
-      a.box_rows = rows / a.n_box;
-      const cuuint64_t gdim[3] = {(cuuint64_t)T.Cin, (cuuint64_t)r.P * mul, (cuuint64_t)r.B};
-      const cuuint64_t gstr[2] = {(cuuint64_t)T.Cin * 4, (cuuint64_t)a.x_bs * 4};
-      const cuuint32_t box[3] = {32, (cuuint32_t)a.box_rows, 1};
-      const cuuint32_t estr[3] = {1, 1, 1};
-      const CUresult cr = encode_tiled_fn()(&tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), gdim, gstr, box, estr,
-                                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (cr != CUDA_SUCCESS) return fail(OVC_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) for a [%d][%d][%d] activation tensor", (int)cr,
-                                          r.B, r.P * mul, T.Cin);
-      a.act_tma = 1;
-    }
-    const int ncol = T.Ntot / T.TN;
-    const int per_col = std::max(1, r.c->sm_count / ncol / std::max(1, ex.grid_div));
-    dim3 pg((unsigned)std::min(total, per_col), ncol, 1);
-    const bool pdl = r.c->use_pdl == 1 || (r.c->use_pdl == 2 && ex.epi != 0);
-    if (T.TN == 128) CK(launch_ex(tcconv_kernel<128>, pg, TCN_THREADS, TcnCfg<128>::SMEM_BYTES, r.st, pdl, a, n_tt, total, tmap));
-    else if (T.TN == 64) CK(launch_ex(tcconv_kernel<64>, pg, TCN_THREADS, TcnCfg<64>::SMEM_BYTES, r.st, pdl, a, n_tt, total, tmap));
-    else CK(launch_ex(tcconv_kernel<32>, pg, TCN_THREADS, TcnCfg<32>::SMEM_BYTES, r.st, pdl, a, n_tt, total, tmap));
-  }
+  // persistent: one CTA per SM walks the (utterance, 128-step tile) list; column tiles (if any) on grid.y
+  const int n_tt = (t_len + 127) / 128, total = n_tt * r.B;
+  const int ncol = T.Ntot / T.TN;
+  const int per_col = std::max(1, r.c->sm_count / ncol / std::max(1, ex.grid_div));
+  dim3 pg((unsigned)std::min(total, per_col), ncol, 1);
+  const bool pdl = r.c->use_pdl == 1 || (r.c->use_pdl == 2 && ex.epi != 0);
+  if (T.TN == 128) CK(launch_ex(tcconv_kernel<128, false>, pg, TCN_THREADS, TcnCfg<128, false>::SMEM_BYTES, r.st, pdl, a, n_tt, total));
+  else if (T.TN == 64) CK(launch_ex(tcconv_kernel<64, false>, pg, TCN_THREADS, TcnCfg<64, false>::SMEM_BYTES, r.st, pdl, a, n_tt, total));
+  else CK(launch_ex(tcconv_kernel<32, false>, pg, TCN_THREADS, TcnCfg<32, false>::SMEM_BYTES, r.st, pdl, a, n_tt, total));
   CK(cudaGetLastError());
   r.c->launches++;
   const double units = (double)r.B * t_len;
@@ -993,47 +934,34 @@ static int launch_tc(Run& r, const TcLayer& T, const float* x, float* y, const f
   return OVC_OK;
 }
 
-// one ResBlock conv pair (c1 dilated, c2 dilation 1, residual = the pair's input) as ONE kernel: C = 64 / 32 stages
-// Only where BOTH convs' weights stay resident in shared memory next to the operand tiles, and only the HBM-bound pairs:
-// C = 32 and C = 64 at k <= 5 / k = 3.  Measured (C = 32, per pair, 32 x 10 s): k = 3 -25 %, k = 7 equal, k = 11 +8 % (those are
-// bound by shared-memory operand reads, not HBM, and pay for the 118 / 128 tile efficiency).
+// one ResBlock conv pair (c1 dilated, c2 dilation 1, residual = the pair's input) as ONE kernel: C = 64 / 32 stages.
+// Only where BOTH convs' weights stay resident in shared memory next to the operand tiles, and only the pairs whose
+// traffic is dominated by HBM (k <= 5): at larger k a tile's 128 - (k - 1) output steps waste more of the MMA work.
 static bool pair_fits(const TcLayer& T1, const TcLayer& T2) {
   if (!(T1.TN == 32 || T1.TN == 64)) return false;
-  const int ring = T1.TN == 32 ? TcpCfg<32>::RING : TcpCfg<64>::RING, hmax = T1.TN == 32 ? TcpCfg<32>::HMAX : TcpCfg<64>::HMAX;
+  const int ring = T1.TN == 32 ? TcnCfg<32, true>::RING : TcnCfg<64, true>::RING;
   return T1.Ntot == T1.TN && T1.Cin == T1.TN && T2.Ntot == T1.TN && T2.Cin == T1.TN && T2.TN == T1.TN && T2.K == T1.K &&
-         T2.DIL == 1 && (T1.K - 1) / 2 * T1.DIL <= hmax && 2 * (T1.Cin / 16) * T1.K <= ring && T1.K <= 5;
+         T2.DIL == 1 && (T1.K - 1) / 2 * T1.DIL <= TCN_HMAX && 2 * (T1.Cin / 16) * T1.K <= ring && T1.K <= 5;
 }
 static int launch_pair(Run& r, const TcLayer& T1, const TcLayer& T2, const float* x, float* y, int t_len, int mul, float slope,
                        float scale, int accumulate) {
-  TcPairArgs a{};
+  TcConvArgs a{};
   const int C = T1.TN;
   a.x = x; a.x_bs = (long long)C * r.P * mul;
-  a.w1 = reinterpret_cast<const uint16_t*>(r.c->d_tcw + T1.w_off);
+  a.w = reinterpret_cast<const uint16_t*>(r.c->d_tcw + T1.w_off);
   a.w2 = reinterpret_cast<const uint16_t*>(r.c->d_tcw + T2.w_off);
-  a.bias1 = r.c->d_tcw + T1.b_off; a.bias2 = r.c->d_tcw + T2.b_off;
-  a.y = y; a.y_bs = a.x_bs;
+  a.bias = r.c->d_tcw + T1.b_off; a.bias2 = r.c->d_tcw + T2.b_off;
+  a.y = y; a.y_bs = a.x_bs; a.y_ld = C;
   a.lens = r.glens; a.tmax = r.Tmax; a.mul = mul;
-  a.C = C; a.K = T1.K; a.DIL1 = T1.DIL;
+  a.Cin = C; a.Ntot = C; a.K = T1.K; a.DIL = T1.DIL;
   a.slope = slope; a.scale = scale; a.accumulate = accumulate;
   a.passes = r.c->precision == 2 ? 1 : 3;
-  if (!encode_tiled_fn()) return fail(OVC_ERR_CUDA, "cuTensorMapEncodeTiled is not available");
-  const int H1 = (T1.K - 1) / 2 * T1.DIL, H2 = (T1.K - 1) / 2;
-  const int R = 128 - 2 * H2, rows8 = (128 + 2 * H1 + 7) & ~7;
+  const int R = 128 - (T1.K - 1);   // output steps per tile
   const int n_tt = (t_len + R - 1) / R, total = n_tt * r.B;
-  CUtensorMap tmap;
-  memset(&tmap, 0, sizeof tmap);
-  const cuuint64_t gdim[3] = {(cuuint64_t)C, (cuuint64_t)r.P * mul, (cuuint64_t)r.B};
-  const cuuint64_t gstr[2] = {(cuuint64_t)C * 4, (cuuint64_t)a.x_bs * 4};
-  const cuuint32_t box[3] = {32, (cuuint32_t)rows8, 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  const CUresult cr = encode_tiled_fn()(&tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), gdim, gstr, box, estr,
-                                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) return fail(OVC_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) for a conv pair", (int)cr);
   TRY(prof_begin(r));
   dim3 pg((unsigned)std::min(total, r.c->sm_count), 1, 1);
-  if (C == 64) CK(launch_ex(tcpair_kernel<64>, pg, TCN_THREADS, TcpCfg<64>::SMEM_BYTES, r.st, false, a, n_tt, total, tmap));
-  else CK(launch_ex(tcpair_kernel<32>, pg, TCN_THREADS, TcpCfg<32>::SMEM_BYTES, r.st, false, a, n_tt, total, tmap));
+  if (C == 64) CK(launch_ex(tcconv_kernel<64, true>, pg, TCN_THREADS, TcnCfg<64, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
+  else CK(launch_ex(tcconv_kernel<32, true>, pg, TCN_THREADS, TcnCfg<32, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
   CK(cudaGetLastError());
   r.c->launches++;
   const double units = (double)r.B * t_len;
@@ -1212,7 +1140,7 @@ static int set_call_params(ovc_ctx* c, uint64_t seed, float tau, cudaStream_t st
   return OVC_OK;
 }
 static uintptr_t option_bits(const ovc_ctx* c) {
-  return (uintptr_t)c->precision | ((uintptr_t)c->wide_variant << 4) | ((uintptr_t)c->act_tma << 8) | ((uintptr_t)c->use_pdl << 15) | ((uintptr_t)c->tune << 10) | ((uintptr_t)c->use_branches << 14) | ((uintptr_t)c->use_pair << 17);
+  return (uintptr_t)c->precision | ((uintptr_t)c->use_pdl << 15) | ((uintptr_t)c->use_branches << 14) | ((uintptr_t)c->use_pair << 17);
 }
 
 static int ensure_ws(ovc_ctx* c, const WsLayout& W, int B, int Tmax, cudaStream_t st) {
@@ -1524,8 +1452,8 @@ int ovc_create(const ovc_hparams* hp, int device, ovc_ctx** out) {
   if (device < 0 || device >= n) return fail(OVC_ERR_INVALID, "device %d out of range (0..%d)", device, n - 1);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(OVC_ERR_CUDA, "device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(OVC_ERR_CUDA, "device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major, prop.minor);
   ovc_ctx* c = new ovc_ctx();
   c->hp = *hp;
   c->device = device;
@@ -1750,7 +1678,7 @@ int ovc_tts_decode(ovc_ctx* c, const float* noise, uint64_t seed, float noise_sc
 
 int ovc_set_precision(ovc_ctx* c, int mode) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
-  if (mode < 0 || mode > 2) return fail(OVC_ERR_INVALID, "precision mode must be 0 (fp32 FFMA2), 1 (3xTF32 tensor cores) or 2 (single-pass TF32)");
+  if (mode < 0 || mode > 2) return fail(OVC_ERR_INVALID, "precision mode must be 0 (fp32 FFMA), 1 (3xFP16 tensor cores) or 2 (single-pass fp16)");
   c->precision = mode;
   return OVC_OK;
 }
@@ -1758,18 +1686,12 @@ int ovc_set_precision(ovc_ctx* c, int mode) {
 int ovc_set_option(ovc_ctx* c, int key, int value) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   switch (key) {
-    case OVC_OPT_WIDE_VARIANT:
-      if (value < 0 || value > 3) return fail(OVC_ERR_INVALID, "wide variant must be 0, 1, 2 or 3");
-      c->wide_variant = value;
-      return OVC_OK;
     case OVC_OPT_TTS_SIMPLE: c->tts_simple = value != 0; return OVC_OK;
     case OVC_OPT_GRAPH: c->use_graph = value != 0; return OVC_OK;
-    case OVC_OPT_ACT_TMA: c->act_tma = value != 0; return OVC_OK;
     case OVC_OPT_PDL:
       if (value < 0 || value > 2) return fail(OVC_ERR_INVALID, "pdl must be 0, 1 or 2");
       c->use_pdl = value;
       return OVC_OK;
-    case OVC_OPT_TUNE: c->tune = value; return OVC_OK;
     case OVC_OPT_BRANCHES: c->use_branches = value != 0; return OVC_OK;
     case OVC_OPT_PAIR: c->use_pair = value != 0; return OVC_OK;
     default: return fail(OVC_ERR_INVALID, "unknown option %d", key);

@@ -4,23 +4,32 @@
 //
 // Channels-last fp32 activations X[b][t][C] (time-major rows).  Every operand is split x = hi + lo / 2^11 with
 // hi = fp16(x), lo = fp16((x - hi) * 2^11) (22 mantissa bits, ovc_tc.cuh) and every product is evaluated as
-// a_hi*b_hi + (a_lo*b_hi + a_hi*b_lo) / 2^11 by tcgen05.mma.kind::f16 with fp32 accumulation in TMEM: the hi*hi
+// a_hi*b_hi + (a_lo*b_hi + a_hi*b_lo) / 2^11 by wgmma (fp16 operands, fp32 accumulation in registers): the hi*hi
 // products in one accumulator, the two cross terms in a second one ("low-order accumulator"), joined in the
-// epilogue.  The two accumulators of a tile sit side by side in TMEM and a weight slot holds [b_hi ; b_lo] as ONE
-// 2*TN-row operand, so a_hi * [b_hi ; b_lo]^T is a single MMA of width 2*TN (both accumulators at once) and
-// a_lo * b_hi^T a second one of width TN: two A-operand reads per k-step instead of three (SS-mode MMAs of the
-// narrow layers are bound by shared-memory operand reads, 128 B/clk).  Besides carrying the 2^-11 scale, the second accumulator keeps the tensor core's truncating adds
-// (tools/tc_acc_test.cu) away from the long hi*hi sum.  Error ~1e-6 per conv, i.e. fp32-grade
-// (tools/tc_f16_test.cu); fp16 MMAs run at twice the TF32 rate on half the operand bytes.
+// epilogue.  A weight slot holds b_hi in rows [0, TN) and b_lo in rows [TN, 2 TN); the main and the low-order
+// accumulator are disjoint halves of one register array, and every k-step issues three MMAs of width TN: a_hi * b_hi^T
+// into the main one, a_hi * b_lo^T and a_lo * b_hi^T into the low-order one.  (A single 2*TN-wide MMA over both halves
+// followed by a TN-wide one into the upper half would save an A-operand read, but MMAs of different shapes on
+// overlapping accumulator registers make ptxas serialise the whole wgmma chain.)  Besides carrying the 2^-11 scale,
+// the second accumulator keeps the long hi*hi sum apart from the small cross terms.  Error ~1e-6 per conv, i.e.
+// fp32-grade.
 //
 // K-major, no-swizzle operand tiles (see ovc_tc.cuh): a convolution tap is a 16-byte-per-row shift of the A
-// descriptor's start address, so all taps (any dilation) read ONE staged halo tile.  Two kernels:
-//   tcconv_kernel<TN>        TN = 128 / 64 / 32 output columns, persistent: one CTA per SM walks the (utterance, tile)
-//                            list, activations staged by TMA, epilogue of tile i under the MMAs of tile i+1
-//   tcconv_wide_kernel<MT>   TN = 128, one tile set (MT x 128 steps) per CTA (kept as the A/B alternative)
+// descriptor's start address, so all taps (any dilation) read ONE staged halo tile.
+//
+// tcconv_kernel<TN, PAIR>: persistent, one CTA (three warpgroups) per SM walks the (utterance, 128-step tile) list.
+//   warp 0       weights by TMA bulk copies: resident in shared memory for the whole launch when they fit, else a ring
+//                streams them per tile
+//   warps 1-3    converters: global fp32 rows -> lrelu -> fp16 hi/lo split -> A operand layout, running ahead across
+//                tiles (two operand buffers); rows outside the utterance become zeros here (zero padding, x_mask and
+//                the ragged batch in one rule)
+//   warpgroups 1, 2  MMAs of 64 tile rows each (accumulators in registers), then the fused epilogue from registers
+// PAIR = true runs one ResBlock conv PAIR of the narrow generator stages in the same kernel:
+//   t = c1(lrelu(x)) (k taps, dilation d);  y = (c2(lrelu(t)) + x [+ y_old]) * scale (k taps, dilation 1)
+// The epilogue of conv 1 writes lrelu(t), split into hi/lo, straight into a shared-memory A operand of conv 2, so t
+// never leaves the SM.  A tile is 128 conv-1 steps; conv 2 needs (k-1)/2 steps of t on either side, so it yields
+// 128 - (k-1) output steps.
 #pragma once
-#include <cuda.h>   // CUtensorMap (the driver entry point that encodes it is resolved at run time, ovc_lib.cu)
-
 #include "ovc_conv.cuh"
 #include "ovc_tc.cuh"
 
@@ -41,28 +50,11 @@ struct TcConvArgs {
   int Cin; int Ntot; int K; int DIL;   // Ntot = output row width (C for a ResBlock conv, stride*Cout for a polyphase transposed conv)
   float slope; float scale; int accumulate;
   int passes;   // 3: split precision (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo); 1: single-pass fp16 (11-bit operands, like cuDNN's TF32 default)
-  int act_tma;  // persistent kernel: 1 = activation chunks arrive by tensor-map TMA (box_rows x 32 channels, n_box boxes per
-  int box_rows; //                    chunk), 0 = the converter warps load them from global memory themselves
-  int n_box;
-  int tune;     // A/B switches (OVC_OPT_TUNE): bit 0 = L2 prefetch of the residual tile, bit 1 = two items per converter iteration
+  const uint16_t* w2; const float* bias2;   // PAIR: conv 2 (Cin = Ntot = TN, dilation 1); x is also the residual
 };
 
-// one box of a [B][rows][Cin] fp32 tensor -> shared memory (128-byte swizzle), completion on an mbarrier
-__device__ __forceinline__ void tma_tensor3d_g2s(void* dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];" ::"r"(
-          smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar))
-      : "memory");
-}
-
-// ask the L2 for `bytes` (multiple of 16) starting at `p`: no destination, no completion -- the loads that follow hit L2
-__device__ __forceinline__ void l2_prefetch_bulk(const void* p, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
-}
-
 // Programmatic dependent launch (launch_tc sets the stream-serialization attribute): the NEXT kernel's CTAs may start
-// their prologue (barriers, TMEM, weight TMA) while this grid drains; a thread must pass pdl_wait() before it touches
+// their prologue (barriers, weight TMA) while this grid drains; a thread must pass pdl_wait() before it touches
 // anything the PREVIOUS kernel wrote (or overwrites anything it read).
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -74,131 +66,48 @@ __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
-// item i of a staged chunk -> (row, 8-channel column block): 8 consecutive lanes take 8 consecutive rows of one
-// column block, so the 16-byte operand stores of a quarter-warp are 128 contiguous bytes (conflict-free)
-template <int NKC>
-__device__ __forceinline__ void tc_item(int i, int& row, int& kc) {
-  kc = (i >> 3) % NKC;
-  row = (i / (8 * NKC)) * 8 + (i & 7);
-}
-
-// Epilogue of MMA tiles [mt_lo, mt_hi) x columns [c_lo, c_hi) of one CTA tile (MT x 128 steps x TN columns): TMEM ->
-// registers -> fused ops -> global.  Warp w may read TMEM lanes [32*(w%4), +32); tile mt owns columns [2*mt*TN, +TN)
-// (main accumulator) and the next TN (low-order accumulator).
-// TMEM is read in the accumulator-fragment layout (tc::tmem_ld16x256_x4_issue): one block = 16 steps x 32 columns,
-// four consecutive threads per 32-byte segment of an output row, so every global access of a warp is made of whole
-// sectors (the thread-per-row layout moved 16 bytes per sector and spilled).  Operands with DRAM latency -- the
-// residual of a ResBlock conv, the read-modify-write target of the WaveNet res/skip update -- are fetched one block
-// ahead, and those of the first block BEFORE the wait on the accumulator barrier `bar`: they arrive under the MMAs.
-template <int TN, int MT>
-__device__ __forceinline__ void tc_epilogue(const TcConvArgs& a, uint32_t acc, int b, int t0, int n0, int lim, int warp, int lane,
-                                            int mt_lo, int mt_hi, int c_lo, int c_hi, uint64_t* bar, uint32_t parity) {
-  const int lane_base = (warp & 3) * 32;
-  const int rsub = lane >> 2, csub = (lane & 3) * 2;
+// Epilogue of one thread's two rows (tile rows row_a and row_a + 8, output steps t0 + row) x TN columns, straight from
+// the accumulator fragment d (ovc_tc.cuh: columns [0, TN) main accumulator, [TN, 2 TN) low-order accumulator).  Four
+// consecutive threads cover 32 contiguous bytes of an output row, so every global access of a warp is whole sectors.
+template <int TN>
+__device__ __forceinline__ void tc_epilogue(const TcConvArgs& a, const float (&d)[TN], int b, int t0, int n0, int lim, int row_a) {
+  const int csub = (threadIdx.x & 3) * 2;
   float* yb = a.y + (size_t)b * a.y_bs;
   const float* rb = a.r ? a.r + (size_t)b * a.y_bs : nullptr;
   float* sb = a.s ? a.s + (size_t)b * a.s_bs : nullptr;
   const float* bias = a.bias + (size_t)b * a.bias_bs;
   const bool two = a.passes == 3;
-  const int ncb = (c_hi - c_lo) >> 5;
-  const int nblk = (mt_hi - mt_lo) * ncb * 2;
-
-  // block k -> (MMA tile, 32-column group, 16-row half); rows a = first row of this thread, b = a + 8
-  auto geom = [&](int k, int& mt, int& c0, int& row) {
-    const int h = k & 1, q = k >> 1;
-    mt = mt_lo + q / ncb;
-    c0 = c_lo + (q % ncb) * 32;
-    row = lane_base + 16 * h + rsub;
-  };
-  // where block k's read-modify-write / residual operand lives (nullptr: none)
-  auto operand = [&](int c0, bool& add) -> const float* {
-    add = true;
-    if (a.epi == 0) return rb ? rb + n0 + c0 + csub : nullptr;
-    if (a.epi == 2) {
-      const int col = n0 + c0;
-      const bool to_x = col < a.split;          // uniform per 32-column group (split is a multiple of 32)
-      add = to_x || !a.first;
-      return to_x ? yb + col + csub : sb + (col - a.split) + csub;
-    }
-    return nullptr;
-  };
-  auto prefetch = [&](int k, float2 (&q)[8]) {
-    int mt, c0, row;
-    geom(k, mt, c0, row);
-    bool add;
-    const float* src = operand(c0, add);
-    const int ta = t0 + mt * 128 + row, tb = ta + 8;
+  const int ta = t0 + row_a, tb = ta + 8;
+  const bool oka = ta < lim, okb = tb < lim;
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      q[2 * g] = make_float2(0.f, 0.f);
-      q[2 * g + 1] = make_float2(0.f, 0.f);
-      if (src && add) {
-        if (ta < lim) q[2 * g] = *reinterpret_cast<const float2*>(src + (size_t)ta * a.y_ld + 8 * g);
-        if (tb < lim) q[2 * g + 1] = *reinterpret_cast<const float2*>(src + (size_t)tb * a.y_ld + 8 * g);
-      }
-    }
-  };
-
-  float2 rq[8];
-  if (nblk > 0) prefetch(0, rq);
-  mbar_wait(bar, parity);
-  tc::fence_after();
-#pragma unroll 1
-  for (int k = 0; k < nblk; ++k) {
-    int mt, c0, row;
-    geom(k, mt, c0, row);
-    const int ta = t0 + mt * 128 + row, tb = ta + 8;
-    const bool oka = ta < lim, okb = tb < lim;
-    const uint32_t taddr = acc + ((uint32_t)(lane_base + 16 * (k & 1)) << 16) + 2 * mt * TN + c0;
-    uint32_t rm[16], rl[16];
-    tc::tmem_ld16x256_x4_issue(taddr, rm);
-    if (two) tc::tmem_ld16x256_x4_issue(taddr + TN, rl);
-    // under the TMEM read: the next block's operand, this block's bias (and previous output when accumulating)
-    float2 rn[8];
-    if (k + 1 < nblk) {
-      prefetch(k + 1, rn);
-    } else {
-#pragma unroll
-      for (int g = 0; g < 8; ++g) rn[g] = make_float2(0.f, 0.f);
-    }
-    float2 bq[4], ya[4], yc[4];
-#pragma unroll
-    for (int g = 0; g < 4; ++g) bq[g] = __ldg(reinterpret_cast<const float2*>(bias + n0 + c0 + 8 * g + csub));
-    const bool accum = a.epi == 0 && a.accumulate;
-    if (accum) {
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        ya[g] = make_float2(0.f, 0.f);
-        yc[g] = make_float2(0.f, 0.f);
-        if (oka) ya[g] = *reinterpret_cast<const float2*>(yb + (size_t)ta * a.y_ld + n0 + c0 + 8 * g + csub);
-        if (okb) yc[g] = *reinterpret_cast<const float2*>(yb + (size_t)tb * a.y_ld + n0 + c0 + 8 * g + csub);
-      }
-    }
+  for (int c0 = 0; c0 < TN; c0 += 32) {
     float v[16];
-    if (two) {
-      tc::tmem_ld_wait16x2(rm, rl);
 #pragma unroll
-      for (int i = 0; i < 16; ++i) v[i] = fmaf(__uint_as_float(rl[i]), tc::kLoInv, __uint_as_float(rm[i]));
-    } else {
-      tc::tmem_ld_wait16(rm);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(rm[i]);
-    }
+    for (int i = 0; i < 16; ++i) v[i] = two ? fmaf(d[TN / 2 + c0 / 2 + i], tc::kLoInv, d[c0 / 2 + i]) : d[c0 / 2 + i];
 #pragma unroll
     for (int g = 0; g < 4; ++g) {
-      v[4 * g] += bq[g].x; v[4 * g + 1] += bq[g].y; v[4 * g + 2] += bq[g].x; v[4 * g + 3] += bq[g].y;
+      const float2 bq = __ldg(reinterpret_cast<const float2*>(bias + n0 + c0 + 8 * g + csub));
+      v[4 * g] += bq.x; v[4 * g + 1] += bq.y; v[4 * g + 2] += bq.x; v[4 * g + 3] += bq.y;
     }
     if (a.epi == 0) {
       // ---- linear: bias, residual, MRF accumulate, scale
       float* ypa = yb + (size_t)ta * a.y_ld + n0 + c0 + csub;
       float* ypb = yb + (size_t)tb * a.y_ld + n0 + c0 + csub;
+      const float* rpa = rb ? rb + (size_t)ta * a.y_ld + n0 + c0 + csub : nullptr;
+      const float* rpb = rb ? rb + (size_t)tb * a.y_ld + n0 + c0 + csub : nullptr;
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
-        float2 oa = make_float2(v[4 * g] + rq[2 * g].x, v[4 * g + 1] + rq[2 * g].y);
-        float2 ob = make_float2(v[4 * g + 2] + rq[2 * g + 1].x, v[4 * g + 3] + rq[2 * g + 1].y);
-        if (accum) {
-          oa.x = ya[g].x + oa.x; oa.y = ya[g].y + oa.y;
-          ob.x = yc[g].x + ob.x; ob.y = yc[g].y + ob.y;
+        float2 oa = make_float2(v[4 * g], v[4 * g + 1]), ob = make_float2(v[4 * g + 2], v[4 * g + 3]);
+        if (rb) {
+          const float2 qa = oka ? *reinterpret_cast<const float2*>(rpa + 8 * g) : make_float2(0.f, 0.f);
+          const float2 qb = okb ? *reinterpret_cast<const float2*>(rpb + 8 * g) : make_float2(0.f, 0.f);
+          oa.x += qa.x; oa.y += qa.y; ob.x += qb.x; ob.y += qb.y;
+        }
+        if (a.accumulate) {
+          const float2 ya = oka ? *reinterpret_cast<const float2*>(ypa + 8 * g) : make_float2(0.f, 0.f);
+          const float2 yc = okb ? *reinterpret_cast<const float2*>(ypb + 8 * g) : make_float2(0.f, 0.f);
+          oa.x = ya.x + oa.x; oa.y = ya.y + oa.y;
+          ob.x = yc.x + ob.x; ob.y = yc.y + ob.y;
         }
         if (a.scale != 1.f) { oa.x *= a.scale; oa.y *= a.scale; ob.x *= a.scale; ob.y *= a.scale; }
         if (oka) *reinterpret_cast<float2*>(ypa + 8 * g) = oa;
@@ -220,492 +129,160 @@ __device__ __forceinline__ void tc_epilogue(const TcConvArgs& a, uint32_t acc, i
       }
     } else {
       // ---- WaveNet res/skip: columns < split update x in place (x += res), the rest go to the skip sum (= / +=)
-      bool add;
-      float* dst = const_cast<float*>(operand(c0, add));
+      const int col = n0 + c0;
+      const bool to_x = col < a.split;          // uniform per 32-column group (split is a multiple of 32)
+      const bool add = to_x || !a.first;
+      float* dst = (to_x ? yb + col : sb + (col - a.split)) + csub;
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
-        const float2 oa = make_float2(rq[2 * g].x + v[4 * g], rq[2 * g].y + v[4 * g + 1]);
-        const float2 ob = make_float2(rq[2 * g + 1].x + v[4 * g + 2], rq[2 * g + 1].y + v[4 * g + 3]);
+        float2 oa = make_float2(v[4 * g], v[4 * g + 1]), ob = make_float2(v[4 * g + 2], v[4 * g + 3]);
+        if (add) {
+          const float2 qa = oka ? *reinterpret_cast<const float2*>(dst + (size_t)ta * a.y_ld + 8 * g) : make_float2(0.f, 0.f);
+          const float2 qb = okb ? *reinterpret_cast<const float2*>(dst + (size_t)tb * a.y_ld + 8 * g) : make_float2(0.f, 0.f);
+          oa = make_float2(qa.x + oa.x, qa.y + oa.y);
+          ob = make_float2(qb.x + ob.x, qb.y + ob.y);
+        }
         if (oka) *reinterpret_cast<float2*>(dst + (size_t)ta * a.y_ld + 8 * g) = oa;
         if (okb) *reinterpret_cast<float2*>(dst + (size_t)tb * a.y_ld + 8 * g) = ob;
       }
     }
-#pragma unroll
-    for (int g = 0; g < 8; ++g) rq[g] = rn[g];
   }
 }
 
-// one thread issues the MMAs of MMA tiles [mt_lo, mt_hi) for one (k-step, tap) against weight slot b_slot = [b_hi ; b_lo]
-#define OVC_TC_ISSUE_MMAS(ACC)                                                                       \
-  _Pragma("unroll") for (int mt = mt_lo; mt < mt_hi; ++mt) {                                         \
-    const uint64_t ad_hi = a_cur + mt * 128, ad_lo = ad_hi + A_LO16;                                 \
-    const uint32_t d = (ACC) + 2 * mt * TN;                                                          \
-    if (three) {                                                                                     \
-      tc::mma_f16(d, ad_hi, b_slot, idesc2, !first);      /* [main | low] (+)= a_hi * [b_hi ; b_lo]^T */ \
-      tc::mma_f16(d + TN, ad_lo, b_slot, idesc1, true);   /* low += a_lo * b_hi^T */                 \
-    } else {                                                                                         \
-      tc::mma_f16(d, ad_hi, b_slot, idesc1, !first);                                                 \
-    }                                                                                                \
-  }
-
-// ---------------------------------------------------------------------------------------------------------
-// tcconv_wide_kernel: TN = 128 output columns, one tile set (MT x 128 steps) per CTA.
-//   MT = 1: 256 TMEM columns and ~109 KB of shared memory per CTA -> TWO CTAs per SM, so one CTA's prologue /
-//           epilogue overlaps the other's MMAs (the layer's weights are re-streamed per 128 steps).
-//   MT = 2: all 512 TMEM columns, one CTA per SM, weights streamed once per 256 steps, serial epilogue.
-// (A 2-CTA-cluster variant that multicast the weight stream was measured in round 2: no faster, and wrong results
-// whenever both CTAs of a cluster were active -- removed.)
-// Warp roles: warp 0 TMA weight producer; warp 1 (and 6 when MT >= 2) one MMA-issuing thread each; warps 2..5
-// A producers (cp.async raw rows RAWD chunks ahead -> lrelu -> hi/lo fp16 split -> operand layout), then epilogue.
-// ---------------------------------------------------------------------------------------------------------
-template <int MT_>
-struct TcwCfg {
-  static constexpr int TN = 128, MT = MT_;
-  static constexpr int KCH = 16, NKC = KCH / 8, KS = KCH / 16;    // channels per A stage
-  static constexpr int NISS = MT >= 2 ? 2 : 1;                    // MMA-issuing threads
-  static constexpr int THREADS = NISS == 2 ? 224 : 192;
-  static constexpr int ROWS = MT * 128 + 64;                      // staged rows per A buffer (tile + 2*25 halo, padded)
-  static constexpr int NABUF = 2;                                 // converted A stages
-  static constexpr int RAWD = 2, NST = RAWD + 1;                  // raw fp32 landing stages in flight ahead
-  static constexpr int SLOTS = MT == 1 ? 6 : 14;                  // weight ring depth
-  static constexpr int A_BUF_BYTES = 2 * NKC * ROWS * 16;         // [hi|lo][column block][row][8 halfs]
-  static constexpr int SLOT_BYTES = 2 * 2 * TN * 16;              // [column block][hi|lo][n][8 halfs]
-  static constexpr int RAW_BYTES = ROWS * KCH * 4;
-  static constexpr size_t SMEM_BYTES = 512 + NABUF * A_BUF_BYTES + SLOTS * SLOT_BYTES + NST * RAW_BYTES;
-  static constexpr uint32_t TMEM_COLS = 2 * MT * TN;              // main + low-order accumulators
-  static constexpr int MINB = MT == 1 ? 2 : 1;
-};
-
-template <int MT>
-__global__ void __launch_bounds__(TcwCfg<MT>::THREADS, TcwCfg<MT>::MINB) tcconv_wide_kernel(const TcConvArgs a) {
-  using Cfg = TcwCfg<MT>;
-  constexpr int TN = Cfg::TN, NABUF = Cfg::NABUF, SLOTS = Cfg::SLOTS, ROWS = Cfg::ROWS, NKC = Cfg::NKC, NISS = Cfg::NISS;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
-  uint64_t* a_full = bars, *a_empty = bars + NABUF, *b_full = bars + 2 * NABUF, *b_empty = b_full + SLOTS,
-            *acc_full = b_empty + SLOTS;
-  static_assert((2 * NABUF + 2 * SLOTS + 1) * 8 + 8 <= 512, "barrier area");
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
-  unsigned char* abuf = smem_raw + 512;
-  unsigned char* bring = abuf + NABUF * Cfg::A_BUF_BYTES;
-  unsigned char* raw = bring + SLOTS * Cfg::SLOT_BYTES;
-
-  const int b = blockIdx.z;
-  const int t0 = blockIdx.x * (MT * 128);
-  const int n0 = blockIdx.y * TN;
-  const int lim = (a.lens ? (int)min((long long)a.tmax, a.lens[b]) : a.tmax) * a.mul;
-  const int lim_x = a.has_lens_x ? (int)min((long long)a.tmax, a.lens_x[b]) * a.mul : lim;
-  if (t0 >= lim) return;   // the tile lies past the utterance
-
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: role code may use uniform registers
-  const int H = (a.K - 1) / 2 * a.DIL;
-  const int nq = a.Cin / Cfg::KCH;            // A chunks
-  const int n_slots = (a.Cin / 16) * a.K;
-
-  if (tid == 0) {
-    for (int i = 0; i < NABUF; ++i) { mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], NISS); }
-    for (int i = 0; i < SLOTS; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], NISS); }
-    mbar_init(acc_full, NISS);
-    fence_mbar_init();
-  }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc::fence_before();
-  __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem_d = *tmem_slot;
-  pdl_launch_dependents();
-  if (warp != 0) pdl_wait();   // warp 0 only streams the (constant) weights: it may run ahead of the previous kernel's end
-
-  if (warp == 0) {
-    // ------------------------------------------------------------ weight producer (TMA bulk)
-    if (lane == 0) {
-      const unsigned char* wp = reinterpret_cast<const unsigned char*>(a.w) + (size_t)blockIdx.y * n_slots * Cfg::SLOT_BYTES;
-      constexpr uint32_t BYTES = Cfg::SLOT_BYTES;
-      int slot = 0;
-      uint32_t phase = 1;   // the first pass over the ring finds every slot free
-      for (int it = 0; it < n_slots; ++it) {
-        mbar_wait(&b_empty[slot], phase);
-        mbar_expect_tx(&b_full[slot], BYTES);
-        tma_bulk_g2s(bring + slot * Cfg::SLOT_BYTES, wp, BYTES, &b_full[slot]);
-        wp += Cfg::SLOT_BYTES;
-        if (++slot == SLOTS) { slot = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1 || (NISS == 2 && warp == 6)) {
-    // ------------------------------------------------------------ MMA issuers (one elected thread per warp)
-    // The whole warp runs the loop converged and only the tcgen05 instructions are predicated on elect.sync: the
-    // descriptors then live in uniform registers and advance by plain adds (they differ only in their 14-bit
-    // start-address field).  [A divergent `if (lane == 0)` around the loop made ptxas wrap every MMA in an
-    // ELECT / R2UR / BRA.U.ANY replay sequence: ~60 dependent instructions per MMA pair, 35 % tensor-pipe activity.]
-    {
-      const int mt_lo = (warp == 1 ? 0 : MT / NISS), mt_hi = mt_lo + MT / NISS;
-      const uint32_t idesc1 = tc::make_idesc_f16(128, TN), idesc2 = tc::make_idesc_f16(128, 2 * TN);
-      constexpr uint32_t LBO_A = ROWS * 16, LBO_B = 2 * TN * 16, SBO = 128;
-      constexpr uint32_t A_LO16 = (NKC * ROWS * 16) >> 4;        // hi -> lo inside an A buffer, in 16-byte units
-      constexpr uint32_t SLOT16 = Cfg::SLOT_BYTES >> 4;
-      const uint64_t a_proto = tc::make_desc(0, LBO_A, SBO), b_proto = tc::make_desc(0, LBO_B, SBO);
-      const uint64_t b_ring = b_proto + (tc::smem_addr(bring) >> 4);
-      const uint32_t dil = (uint32_t)a.DIL;
-      const bool three = a.passes == 3;
-      int slot = 0;
-      uint32_t bphase = 0;
-      bool first = true;
-      for (int q = 0; q < nq; ++q) {
-        const int buf = q % NABUF;
-        mbar_wait(&a_full[buf], (q / NABUF) & 1);
-        tc::fence_after();
-        for (int j = 0; j < Cfg::KS; ++j) {
-          uint64_t a_cur = a_proto + ((tc::smem_addr(abuf + buf * Cfg::A_BUF_BYTES) + 2 * j * LBO_A) >> 4);
-          for (int tap = 0; tap < a.K; ++tap) {
-            mbar_wait(&b_full[slot], bphase);
-            tc::fence_after();
-            const uint64_t b_slot = b_ring + (uint32_t)slot * SLOT16;
-            // output step (t0 + mt*128 + i) reads staged row (mt*128 + i + tap*DIL): the halo tile starts at t0 - H
-            if (tc::elect_one()) {
-              OVC_TC_ISSUE_MMAS(tmem_d)
-              tc::mma_commit(&b_empty[slot]);       // slot reusable once these MMAs have read it
-            }
-            __syncwarp();
-            first = false;
-            a_cur += dil;
-            if (++slot == SLOTS) { slot = 0; bphase ^= 1; }
-          }
-        }
-        if (tc::elect_one()) tc::mma_commit(&a_empty[buf]);
-        __syncwarp();
-      }
-      if (tc::elect_one()) tc::mma_commit(acc_full);
-      __syncwarp();
-    }
-  } else if (warp >= 2 && warp <= 5) {
-    // ------------------------------------------------------------ A producers, then epilogue
-    const int pt = tid - 64;                                   // 0..127
-    const float* xb = a.x + (size_t)b * a.x_bs;
-    const int rows8 = (MT * 128 + 2 * H + 7) & ~7;
-    constexpr int NP = Cfg::KCH / 4;                           // 16-byte pieces per raw row
-    const int pieces = rows8 * NP, items = rows8 * NKC;
-    // raw fp32 rows land by cp.async (zero-filled outside [0, lim)), fully coalesced, RAWD chunks ahead; piece p of
-    // row r sits at 16-byte slot r*NP + (p ^ ((r >> 1) & 3)) so the conversion's row-strided reads are conflict-free
-    auto stage = [&](int q) {
-      unsigned char* dst = raw + (q % Cfg::NST) * Cfg::RAW_BYTES;
-      for (int i = pt; i < pieces; i += 128) {
-        const int row = i / NP, p = i % NP;
-        const int t = t0 - H + row;
-        const bool ok = (t >= 0 && t < lim_x);
-        const float* src = ok ? xb + (size_t)t * a.Cin + q * Cfg::KCH + p * 4 : xb;
-        cp_async16_zfill(dst + (row * NP + (p ^ ((row >> 1) & 3))) * 16, src, ok ? 16 : 0);
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-    for (int q = 0; q < Cfg::RAWD; ++q) {
-      if (q < nq) stage(q);
-      else asm volatile("cp.async.commit_group;" ::: "memory");
-    }
-    for (int q = 0; q < nq; ++q) {
-      asm volatile("cp.async.wait_group %0;" ::"n"(Cfg::RAWD - 1) : "memory");   // this thread's pieces of chunk q landed
-      named_bar_sync(1, 128);   // ... everybody's did, and everybody is done reading the stage refilled next
-      if (q + Cfg::RAWD < nq) stage(q + Cfg::RAWD);
-      else asm volatile("cp.async.commit_group;" ::: "memory");                   // keep the group count uniform
-      const int buf = q % NABUF;
-      mbar_wait(&a_empty[buf], ((q / NABUF) & 1) ^ 1);
-      unsigned char* ah = abuf + buf * Cfg::A_BUF_BYTES;
-      unsigned char* al = ah + NKC * ROWS * 16;
-      const unsigned char* src = raw + (q % Cfg::NST) * Cfg::RAW_BYTES;
-      for (int i = pt; i < items; i += 128) {
-        int row, kc;
-        tc_item<NKC>(i, row, kc);
-        const int sw = (row >> 1) & 3;
-        const float4 v0 = *reinterpret_cast<const float4*>(src + (row * NP + ((2 * kc) ^ sw)) * 16);
-        const float4 v1 = *reinterpret_cast<const float4*>(src + (row * NP + ((2 * kc + 1) ^ sw)) * 16);
-        uint4 hi, lo;
-        tc::split_f16x8(v0, v1, a.slope, hi, lo);
-        *reinterpret_cast<uint4*>(ah + (kc * ROWS + row) * 16) = hi;
-        *reinterpret_cast<uint4*>(al + (kc * ROWS + row) * 16) = lo;
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> tensor-core (async) proxy
-      mbar_arrive(&a_full[buf]);
-    }
-    // epilogue: warp w may read TMEM lanes [32*(w%4), +32)
-    tc_epilogue<TN, MT>(a, tmem_d, b, t0, n0, lim, warp, lane, 0, MT, 0, TN, acc_full, 0);
-  }
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_d, Cfg::TMEM_COLS);
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// tcconv_kernel<TN>: persistent split-precision conv, TN = 128 / 64 / 32 output columns per CTA.
-// One CTA per SM loops over tiles (TN = 128: 128 steps, else 256): barriers / TMEM live for the whole launch, the
-// layer's weights stay resident in shared memory when they fit (C = 32: <= 44 KB; C = 64, k = 3: 48 KB; otherwise a
-// ring streams them per tile), and every stage runs ahead across tile boundaries:
-//   warp 15     activation TMA (act_tma): a chunk of a halo tile = rows x 32 channels of the channels-last tensor is
-//               ONE tensor-map box (two when it has more than 256 rows): cp.async.bulk.tensor lands it in a raw fp32
-//               stage, 128-byte swizzled, NRAW chunks ahead, rows before the tensor's start zero-filled by the copy
-//               engine -- the copy engine, not registers, holds the bytes in flight (the narrow layers are HBM-bound:
-//               a whole tile must be in flight per SM to cover the latency).  [Measured: one 128-byte bulk copy per
-//               row instead costs ~55 cycles of TMA issue each and caps the kernel at 1.1 TB/s.]
-//   warps 3-6   (2-6 when TN = 128: its second MMA-issuer warp is free) converters: raw stage (or, act_tma = 0, global
-//               memory) -> lrelu -> fp16 hi/lo split -> operand
-//               layout; rows outside the utterance become zeros here (zero padding, x_mask and the ragged batch in
-//               one rule)
-//   warp 0      weight TMA; warps 1-2 one MMA-issuing thread each (TN = 128: one)
-//   warps 7-14  epilogue of tile i (second TMEM accumulator set) while the MMAs of tile i+1 run
-// The raw stage's 128-byte swizzle and the operand tiles' ROWS = 2 (mod 8) column-block pitch make both sides of
-// the conversion shared-memory bank-conflict free.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int TCN_THREADS = 512;
-
+// one k-step x tap of a warpgroup's 64 rows: main (+)= a_hi * b_hi^T, low (+)= a_hi * b_lo^T + a_lo * b_hi^T
 template <int TN>
+__device__ __forceinline__ void tc_mma_step(float (&d)[TN], uint64_t a_hi, uint64_t a_lo, uint64_t b, bool three, bool first) {
+  float (&lo)[TN / 2] = *reinterpret_cast<float(*)[TN / 2]>(&d[TN / 2]);
+  float (&hi)[TN / 2] = *reinterpret_cast<float(*)[TN / 2]>(&d[0]);
+  tc::Wgmma<TN>::mma(hi, a_hi, b, first ? 0 : 1);
+  if (three) {
+    tc::Wgmma<TN>::mma(lo, a_hi, b + TN, first ? 0 : 1);   // b_lo: rows [TN, 2 TN) of the slot, TN * 16 bytes on
+    tc::Wgmma<TN>::mma(lo, a_lo, b, 1);
+  }
+}
+
+constexpr int TCN_THREADS = 384;   // warpgroup 0: producers; warpgroups 1, 2: MMAs + epilogue
+constexpr int TCN_NCT = 96;        // converter threads (warps 1-3)
+constexpr int TCN_HMAX = 25;       // largest conv-1 halo (k = 11, dilation 5)
+
+template <int TN, bool PAIR>
 struct TcnCfg {
-  static constexpr int MT = TN == 128 ? 1 : 2;                    // 2 sets x MT x (main + low-order) x TN <= 512 TMEM columns
-  static constexpr int NISS = MT >= 2 ? 2 : 1;
-  static constexpr int CONV_W0 = 1 + NISS;                        // first converter warp: with one MMA issuer (TN = 128) warp 2
-  static constexpr int NCT = (7 - CONV_W0) * 32;                  // joins the converters (5 warps instead of 4)
-  static constexpr int KCH = 32, NKC = KCH / 8, KS = KCH / 16;
-  static constexpr int ROWS = MT * 128 + 66;                      // = 2 (mod 8)
-  static constexpr int RAW_ROWS = MT == 1 ? 184 : 320;            // tile + 2 * 25 halo, rounded up to 8 (16 when two boxes)
+  static_assert(!PAIR || TN == 32 || TN == 64, "conv pairs: C = 32 or 64");
+  static constexpr int KCH = 32, NKC = KCH / 8;                   // channels per converted A chunk
+  static constexpr int ROWS = 194;                                // A pitch in rows: >= 128 + 2 * TCN_HMAX, = 2 (mod 8)
+  static constexpr int ROWS2 = 146;                               // PAIR: conv-2 A pitch: 128 + 2 * H2 rows, H2 <= 9
   static constexpr int NABUF = 2;
-  static constexpr int NRAW = TN == 128 ? 3 : 2;                  // raw fp32 chunk stages
-  static constexpr int RAW_STAGE_BYTES = RAW_ROWS * 128;          // multiple of 1024: every stage keeps the swizzle phase
-  static constexpr int RING = TN == 32 ? 22 : (TN == 64 ? 12 : 13);   // weight slots: 44 KB / 48 KB / 104 KB
-  static constexpr int A_BUF_BYTES = 2 * NKC * ROWS * 16;
+  // weight slots (16 channels x 1 tap): TN = 32 holds k = 11 resident, TN = 64 k = 3; pairs hold both convs
+  static constexpr int RING = PAIR ? (TN == 32 ? 44 : 24) : (TN == 32 ? 22 : 12);
   static constexpr int SLOT_BYTES = 2 * 2 * TN * 16;
-  static constexpr size_t SMEM_BYTES = 1024 + NABUF * A_BUF_BYTES + RING * SLOT_BYTES + 1024 + NRAW * RAW_STAGE_BYTES;
-  static constexpr uint32_t TMEM_COLS = 2 * 2 * MT * TN;          // 512 (TN 128, 64) / 256 (TN 32)
+  static constexpr int A_BUF_BYTES = 2 * NKC * ROWS * 16;         // [hi|lo][column block][row][8 halfs]
+  static constexpr int A2_BYTES = PAIR ? 2 * (TN / 8) * ROWS2 * 16 : 0;
+  static constexpr size_t SMEM_BYTES = 1024 + NABUF * A_BUF_BYTES + A2_BYTES + RING * SLOT_BYTES;
+  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+  static_assert((2 * NABUF + 2 * RING) * 8 <= 1024, "barrier area");
 };
 
-// rows staged per chunk: the tile plus its halo, rounded so that one box (<= 256 rows) or two equal boxes of a
-// multiple of 8 rows cover it
-__host__ __device__ inline int tcn_rows(int mt, int H) {
-  const int r = mt * 128 + 2 * H;
-  return r <= 256 ? (r + 7) & ~7 : (r + 15) & ~15;
-}
+// registers per thread after the producers hand theirs to the MMA warpgroups (128 x 56 + 256 x 224 = 64 K)
+constexpr int TCN_PROD_REGS = 56, TCN_MMA_REGS = 224;
 
-template <int TN>
-__global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs a, int n_tt, int total,
-                                                                const __grid_constant__ CUtensorMap tmap) {
-  using Cfg = TcnCfg<TN>;
-  constexpr int MT = Cfg::MT, ROWS = Cfg::ROWS, NABUF = Cfg::NABUF, RING = Cfg::RING, NKC = Cfg::NKC, NRAW = Cfg::NRAW,
-                NISS = Cfg::NISS, NCT = Cfg::NCT;
-  constexpr uint32_t SET_COLS = 2 * MT * TN;
+template <int TN, bool PAIR>
+__global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs a, int n_tt, int total) {
+  using Cfg = TcnCfg<TN, PAIR>;
+  constexpr int ROWS = Cfg::ROWS, ROWS2 = Cfg::ROWS2, NABUF = Cfg::NABUF, RING = Cfg::RING, NKC = Cfg::NKC;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
-  uint64_t* a_full = bars, *a_empty = bars + NABUF, *b_full = bars + 2 * NABUF, *b_empty = b_full + RING,
-            *acc_full = b_empty + RING, *acc_empty = acc_full + 2, *raw_full = acc_empty + 2, *raw_empty = raw_full + NRAW;
-  static_assert((2 * NABUF + 2 * RING + 4 + 2 * NRAW) * 8 + 8 <= 1024, "barrier area");
-  static_assert(Cfg::SMEM_BYTES <= 232448, "shared memory budget");
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(raw_empty + NRAW);
+  uint64_t *a_full = bars, *a_empty = bars + NABUF, *b_full = a_empty + NABUF, *b_empty = b_full + RING;
   unsigned char* abuf = smem_raw + 1024;
-  unsigned char* bring = abuf + NABUF * Cfg::A_BUF_BYTES;
-  // raw stages: 1024-byte aligned in the shared window (the 128-byte swizzle is a function of address bits 4..9)
-  unsigned char* raw = bring + RING * Cfg::SLOT_BYTES;
-  raw += (1024u - (smem_u32(raw) & 1023u)) & 1023u;
+  unsigned char* a2buf = abuf + NABUF * Cfg::A_BUF_BYTES;
+  unsigned char* bring = a2buf + Cfg::A2_BYTES;
 
   const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform: role code may use uniform registers
-  const int n0 = blockIdx.y * TN;
-  const int H = (a.K - 1) / 2 * a.DIL;
-  const int rows8 = tcn_rows(MT, H);
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform
+  const int H1 = (a.K - 1) / 2 * a.DIL;
+  const int H2 = PAIR ? (a.K - 1) / 2 : 0;
+  const int R = 128 - 2 * H2;                  // output steps per tile
+  const int rows8 = (128 + 2 * H1 + 7) & ~7;   // staged input rows per chunk
   const int nq = a.Cin / Cfg::KCH;
-  const int n_slots = (a.Cin / 16) * a.K;
-  const bool resident = n_slots <= RING;
-  const bool act_tma = a.act_tma != 0;
+  const int n_slots = (a.Cin / 16) * a.K;      // weight slots per conv
+  const int n_w = PAIR ? 2 * n_slots : n_slots;
+  const bool resident = n_w <= RING;
+  if (H1 > TCN_HMAX || (PAIR && (!resident || 128 + 2 * H2 > ROWS2))) __trap();   // host: pack_tc / pair_fits
   constexpr uint32_t BYTES = Cfg::SLOT_BYTES;
 
   if (tid == 0) {
-    for (int i = 0; i < NABUF; ++i) { mbar_init(&a_full[i], NCT); mbar_init(&a_empty[i], NISS); }
-    for (int i = 0; i < RING; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], NISS); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], NISS); mbar_init(&acc_empty[i], 8); }
-    for (int i = 0; i < NRAW; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], NCT); }
+    for (int i = 0; i < NABUF; ++i) { mbar_init(&a_full[i], TCN_NCT); mbar_init(&a_empty[i], 2); }
+    for (int i = 0; i < RING; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 2); }
     fence_mbar_init();
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc::fence_before();
+  if (PAIR) {
+    // rows of the conv-2 operand that conv 1 never produces (the taps of the discarded last output rows read them)
+    for (int i = tid; i < Cfg::A2_BYTES / 16; i += TCN_THREADS) reinterpret_cast<uint4*>(a2buf)[i] = make_uint4(0u, 0u, 0u, 0u);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
   __syncthreads();
-  tc::fence_after();
-  const uint32_t tmem_d = *tmem_slot;
   pdl_launch_dependents();
   if (warp != 0) pdl_wait();   // warp 0 only streams the (constant) weights: it may run ahead of the previous kernel's end
 
   // every role walks the same tile sequence
 #define TCN_FOR_TILES                                                                                   \
   for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {                                        \
-    const int b = tile / n_tt, t0 = (tile % n_tt) * (MT * 128);                                         \
+    const int b = tile / n_tt, t0 = (tile % n_tt) * R;                                                  \
     const int lim = (a.lens ? (int)min((long long)a.tmax, a.lens[b]) : a.tmax) * a.mul;                 \
     const int lim_x = a.has_lens_x ? (int)min((long long)a.tmax, a.lens_x[b]) * a.mul : lim;            \
     (void)lim_x;                                                                                        \
     if (t0 >= lim) continue;
 
-  if (warp == 0) {
-    // ------------------------------------------------------------ weights
-    if (lane == 0) {
-      const unsigned char* wt = reinterpret_cast<const unsigned char*>(a.w) + (size_t)blockIdx.y * n_slots * Cfg::SLOT_BYTES;
-      if (resident) {
-        for (int it = 0; it < n_slots; ++it) {
-          mbar_expect_tx(&b_full[it], BYTES);
-          tma_bulk_g2s(bring + it * Cfg::SLOT_BYTES, wt + (size_t)it * Cfg::SLOT_BYTES, BYTES, &b_full[it]);
-        }
-        // a CTA whose tiles all lie past their utterances never waits on these copies: they must have landed before the
-        // CTA can exit (its shared memory may be handed to the next kernel's CTA)
-        for (int it = 0; it < n_slots; ++it) mbar_wait(&b_full[it], 0u);
-      } else {
-        int slot = 0;
-        uint32_t phase = 1;
-        TCN_FOR_TILES
-          (void)b; (void)lim;
-          for (int it = 0; it < n_slots; ++it) {
-            mbar_wait(&b_empty[slot], phase);
-            mbar_expect_tx(&b_full[slot], BYTES);
-            tma_bulk_g2s(bring + slot * Cfg::SLOT_BYTES, wt + (size_t)it * Cfg::SLOT_BYTES, BYTES, &b_full[slot]);
-            if (++slot == RING) { slot = 0; phase ^= 1; }
+  if (warp < 4) {
+    tc::regs_dealloc<TCN_PROD_REGS>();
+    if (warp == 0) {
+      // ------------------------------------------------------------ weights
+      if (lane == 0) {
+        const unsigned char* wt = reinterpret_cast<const unsigned char*>(a.w) + (size_t)blockIdx.y * n_slots * BYTES;
+        if (resident) {
+          for (int it = 0; it < n_w; ++it) {
+            const unsigned char* src = it < n_slots ? wt + (size_t)it * BYTES
+                                                    : reinterpret_cast<const unsigned char*>(a.w2) + (size_t)(it - n_slots) * BYTES;
+            mbar_expect_tx(&b_full[it], BYTES);
+            tma_bulk_g2s(bring + it * BYTES, src, BYTES, &b_full[it]);
           }
-        }
-      }
-    }
-  } else if (warp == 15) {
-    // ------------------------------------------------------------ activation chunks by tensor-map TMA
-    if (lane == 0 && act_tma) {
-      int st = 0;
-      uint32_t phase = 1;   // the first pass finds every raw stage free
-      const uint32_t box_bytes = (uint32_t)a.box_rows * 128u;
-      // the epilogue reads the residual (and the previous output when accumulating) of this tile long after its
-      // activations were requested: when the tile is contiguous in memory (one column tile: Ntot == TN == y_ld), pull it
-      // into L2 now, so that those loads -- few bytes in flight per warp -- pay L2 latency, not DRAM latency
-      const bool pf = (a.tune & 1) && a.epi == 0 && a.Ntot == TN && a.y_ld == TN && (a.r != nullptr || a.accumulate);
-      TCN_FOR_TILES
-        if (pf) {
-          const int rows = min(MT * 128, lim - t0);
-          const size_t off = ((size_t)b * a.y_bs + (size_t)t0 * TN) * sizeof(float);
-          const uint32_t bytes = (uint32_t)rows * TN * 4u;
-          for (uint32_t o = 0; o < bytes; o += 16384u) {
-            const uint32_t n = min(16384u, bytes - o);
-            if (a.r) l2_prefetch_bulk(reinterpret_cast<const char*>(a.r) + off + o, n);
-            if (a.accumulate) l2_prefetch_bulk(reinterpret_cast<const char*>(a.y) + off + o, n);
-          }
-        }
-        for (int q = 0; q < nq; ++q) {
-          mbar_wait(&raw_empty[st], phase);
-          mbar_expect_tx(&raw_full[st], box_bytes * (uint32_t)a.n_box);
-          unsigned char* dst = raw + st * Cfg::RAW_STAGE_BYTES;
-          for (int i = 0; i < a.n_box; ++i)   // coordinates: channel, row (may be negative: zero-filled), utterance
-            tma_tensor3d_g2s(dst + i * box_bytes, &tmap, q * Cfg::KCH, t0 - H + i * a.box_rows, b, &raw_full[st]);
-          if (++st == NRAW) { st = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1 || (NISS == 2 && warp == 2)) {
-    // ------------------------------------------------------------ MMA issuers (one elected thread per warp, converged loop)
-    {
-      const int mt_lo = (warp - 1) * (MT / NISS), mt_hi = mt_lo + MT / NISS;
-      const uint32_t idesc1 = tc::make_idesc_f16(128, TN), idesc2 = tc::make_idesc_f16(128, 2 * TN);
-      constexpr uint32_t LBO_A = ROWS * 16, LBO_B = 2 * TN * 16, SBO = 128;
-      constexpr uint32_t A_LO16 = (NKC * ROWS * 16) >> 4, SLOT16 = Cfg::SLOT_BYTES >> 4;
-      const uint64_t a_proto = tc::make_desc(0, LBO_A, SBO), b_proto = tc::make_desc(0, LBO_B, SBO);
-      const uint64_t b_ring = b_proto + (tc::smem_addr(bring) >> 4);
-      const uint32_t dil = (uint32_t)a.DIL;
-      const bool three = a.passes == 3;
-      int slot = 0, buf = 0, n = 0;
-      uint32_t bphase = 0, aphase = 0;
-      TCN_FOR_TILES
-        (void)b; (void)lim;
-        const int set = n & 1;
-        mbar_wait(&acc_empty[set], ((n >> 1) & 1) ^ 1);   // the epilogue has drained this accumulator set
-        tc::fence_after();
-        const uint32_t acc = tmem_d + set * SET_COLS;
-        bool first = true;
-        if (resident) slot = 0;
-        for (int q = 0; q < nq; ++q) {
-          mbar_wait(&a_full[buf], aphase);
-          tc::fence_after();
-          for (int j = 0; j < Cfg::KS; ++j) {
-            uint64_t a_cur = a_proto + ((tc::smem_addr(abuf + buf * Cfg::A_BUF_BYTES) + 2 * j * LBO_A) >> 4);
-            for (int tap = 0; tap < a.K; ++tap) {
-              if (!resident || n == 0) {
-                mbar_wait(&b_full[slot], resident ? 0u : bphase);
-                tc::fence_after();
-              }
-              const uint64_t b_slot = b_ring + (uint32_t)slot * SLOT16;
-              if (tc::elect_one()) {
-                OVC_TC_ISSUE_MMAS(acc)
-                if (!resident) tc::mma_commit(&b_empty[slot]);
-              }
-              __syncwarp();
-              first = false;
-              a_cur += dil;
-              if (++slot == RING) { slot = 0; bphase ^= 1; }
-            }
-          }
-          if (tc::elect_one()) tc::mma_commit(&a_empty[buf]);
-          __syncwarp();
-          if (++buf == NABUF) { buf = 0; aphase ^= 1; }
-        }
-        if (tc::elect_one()) tc::mma_commit(&acc_full[set]);
-        __syncwarp();
-        ++n;
-      }
-    }
-  } else if (warp >= Cfg::CONV_W0 && warp <= 6) {
-    // ------------------------------------------------------------ converters (run ahead across tiles)
-    const int pt = tid - 32 * Cfg::CONV_W0;
-    const int items = rows8 * NKC;            // item i = (row i / 4, column block i % 4): 32 bytes of one row
-    int buf = 0, st = 0;
-    uint32_t ephase = 1, rphase = 0;
-    TCN_FOR_TILES
-      const float* xb = a.x + (size_t)b * a.x_bs;
-      for (int q = 0; q < nq; ++q) {
-        if (act_tma) mbar_wait(&raw_full[st], rphase);
-        mbar_wait(&a_empty[buf], ephase);
-        unsigned char* ah = abuf + buf * Cfg::A_BUF_BYTES;
-        unsigned char* al = ah + NKC * ROWS * 16;
-        if (act_tma) {
-          // raw stage, 128-byte swizzle: 16-byte chunk c of row r sits at r * 128 + ((c ^ (r & 7)) << 4).
-          // Two items per iteration: both pairs of shared-memory loads are in flight before the first conversion
-          // (one item at a time left the LDS latency exposed: a single warp per scheduler runs this role).
-          const unsigned char* rsrc = raw + st * Cfg::RAW_STAGE_BYTES;
-          auto fetch = [&](int i, float4& v0, float4& v1) {
-            const int row = i >> 2, kc = i & 3;
-            const int t = t0 - H + row;
-            v0 = make_float4(0.f, 0.f, 0.f, 0.f);
-            v1 = v0;
-            if (i < items && t >= 0 && t < lim_x) {
-              const unsigned char* rr = rsrc + row * 128;
-              v0 = *reinterpret_cast<const float4*>(rr + (((2 * kc) ^ (row & 7)) << 4));
-              v1 = *reinterpret_cast<const float4*>(rr + (((2 * kc + 1) ^ (row & 7)) << 4));
-            }
-          };
-          auto emit = [&](int i, const float4& v0, const float4& v1) {
-            if (i >= items) return;
-            const int row = i >> 2, kc = i & 3;
-            uint4 hi, lo;
-            tc::split_f16x8(v0, v1, a.slope, hi, lo);
-            *reinterpret_cast<uint4*>(ah + (kc * ROWS + row) * 16) = hi;
-            *reinterpret_cast<uint4*>(al + (kc * ROWS + row) * 16) = lo;
-          };
-          if (a.tune & 2) {
-            for (int i = pt; i < items; i += 2 * NCT) {
-              float4 a0, a1, b0, b1;
-              fetch(i, a0, a1);
-              fetch(i + NCT, b0, b1);
-              emit(i, a0, a1);
-              emit(i + NCT, b0, b1);
-            }
-          } else {
-            for (int i = pt; i < items; i += NCT) {
-              float4 a0, a1;
-              fetch(i, a0, a1);
-              emit(i, a0, a1);
-            }
-          }
+          // a CTA whose tiles all lie past their utterances never waits on these copies: they must have landed before
+          // the CTA can exit (its shared memory may be handed to the next kernel's CTA)
+          for (int it = 0; it < n_w; ++it) mbar_wait(&b_full[it], 0u);
         } else {
-          constexpr int PB = 5;   // items (32 bytes each) in flight per thread
-          for (int i0 = pt; i0 < items; i0 += NCT * PB) {
+          int slot = 0;
+          uint32_t phase = 1;   // the first pass over the ring finds every slot free
+          TCN_FOR_TILES
+            (void)b;
+            for (int it = 0; it < n_slots; ++it) {
+              mbar_wait(&b_empty[slot], phase);
+              mbar_expect_tx(&b_full[slot], BYTES);
+              tma_bulk_g2s(bring + slot * BYTES, wt + (size_t)it * BYTES, BYTES, &b_full[slot]);
+              if (++slot == RING) { slot = 0; phase ^= 1; }
+            }
+          }
+        }
+      }
+    } else {
+      // ------------------------------------------------------------ converters (run ahead across tiles)
+      const int pt = tid - 32;
+      const int items = rows8 * NKC;            // item i = (row i / 4, column block i % 4): 32 bytes of one row
+      int buf = 0;
+      uint32_t ephase = 1;
+      TCN_FOR_TILES
+        const float* xb = a.x + (size_t)b * a.x_bs;
+        const int r0 = t0 - H2 - H1;            // input step of staged row 0
+        for (int q = 0; q < nq; ++q) {
+          mbar_wait(&a_empty[buf], ephase);
+          unsigned char* ah = abuf + buf * Cfg::A_BUF_BYTES;
+          unsigned char* al = ah + NKC * ROWS * 16;
+          constexpr int PB = 2;   // items (32 bytes each) in flight per thread
+          for (int i0 = pt; i0 < items; i0 += TCN_NCT * PB) {
             float4 v0[PB], v1[PB];
 #pragma unroll
             for (int u = 0; u < PB; ++u) {
-              const int i = i0 + NCT * u;
+              const int i = i0 + TCN_NCT * u;
               const int row = i >> 2, kc = i & 3;
-              const int t = t0 - H + row;
+              const int t = r0 + row;
               v0[u] = make_float4(0.f, 0.f, 0.f, 0.f);
               v1[u] = v0[u];
               if (i < items && t >= 0 && t < lim_x) {
@@ -716,7 +293,7 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
             }
 #pragma unroll
             for (int u = 0; u < PB; ++u) {
-              const int i = i0 + NCT * u;
+              const int i = i0 + TCN_NCT * u;
               if (i >= items) break;
               const int row = i >> 2, kc = i & 3;
               uint4 hi, lo;
@@ -725,40 +302,122 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
               *reinterpret_cast<uint4*>(al + (kc * ROWS + row) * 16) = lo;
             }
           }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbar_arrive(&a_full[buf]);
-        if (++buf == NABUF) { buf = 0; ephase ^= 1; }
-        if (act_tma) {
-          mbar_arrive(&raw_empty[st]);          // this thread has read everything it needs from the raw stage
-          if (++st == NRAW) { st = 0; rphase ^= 1; }
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> tensor-core (async) proxy
+          mbar_arrive(&a_full[buf]);
+          if (++buf == NABUF) { buf = 0; ephase ^= 1; }
         }
       }
     }
-  } else if (warp >= 7 && warp <= 14) {
-    // ------------------------------------------------------------ epilogue (overlaps the next tile's MMAs)
-    // each warp covers the TMEM lane quadrant warp % 4; warps 7..10 / 11..14 split the MMA tiles (MT = 2) or the
-    // columns (MT = 1) of the CTA tile between them
-    const int half = (warp - 7) >> 2;
-    const int mt_lo = MT == 2 ? half : 0, mt_hi = MT == 2 ? half + 1 : 1;
-    const int c_lo = MT == 2 ? 0 : half * (TN / 2), c_hi = MT == 2 ? TN : c_lo + TN / 2;
-    int n = 0;
+  } else {
+    // ------------------------------------------------------------ MMA warpgroups: rows [64 wg, +64) of every tile
+    tc::regs_alloc<TCN_MMA_REGS>();
+    const int wg = (warp >> 2) - 1;
+    const bool leader = (tid & 127) == 0;
+    const int row_a = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // this thread's first accumulator row
+    constexpr uint32_t LBO_A = ROWS * 16, LBO_A2 = ROWS2 * 16, LBO_B = 2 * TN * 16, SBO = 128;
+    constexpr uint32_t A_LO16 = (NKC * ROWS * 16) >> 4, A2_LO16 = ((TN / 8) * ROWS2 * 16) >> 4, SLOT16 = BYTES >> 4;
+    const uint64_t a_proto = tc::make_desc(0, LBO_A, SBO), b_proto = tc::make_desc(0, LBO_B, SBO);
+    const uint64_t b_ring = b_proto + (tc::smem_addr(bring) >> 4);
+    const bool three = a.passes == 3;
+    float d[TN];
+#pragma unroll
+    for (int i = 0; i < TN; ++i) d[i] = 0.f;
+    if (resident)
+      for (int it = 0; it < n_w; ++it) mbar_wait(&b_full[it], 0u);   // resident weights: waited on once
+    int slot = 0, buf = 0;
+    uint32_t bphase = 0, aphase = 0;
     TCN_FOR_TILES
-      const int set = n & 1;
-      tc_epilogue<TN, MT>(a, tmem_d + set * SET_COLS, b, t0, n0, lim, warp, lane, mt_lo, mt_hi, c_lo, c_hi, &acc_full[set],
-                          (n >> 1) & 1);
-      tc::fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[set]);
-      ++n;
+      (void)lim_x;
+      // ---- conv (conv 1 of a pair)
+      bool first = true;
+      if (resident) slot = 0;
+      for (int q = 0; q < nq; ++q) {
+        mbar_wait(&a_full[buf], aphase);
+        tc::fence_regs(d);
+        tc::wgmma_fence();
+        int prev = -1;
+        for (int j = 0; j < 2; ++j) {
+          uint64_t a_cur = a_proto + ((tc::smem_addr(abuf + buf * Cfg::A_BUF_BYTES) + 64 * wg * 16 + 2 * j * LBO_A) >> 4);
+          for (int tap = 0; tap < a.K; ++tap) {
+            if (!resident) mbar_wait(&b_full[slot], bphase);
+            // output row i reads staged row i + tap * DIL: the staged tile starts at the first output step - H
+            tc_mma_step<TN>(d, a_cur, a_cur + A_LO16, b_ring + (uint32_t)slot * SLOT16, three, first);
+            tc::wgmma_commit();
+            if (!resident) {
+              tc::wgmma_wait<1>();                              // the previous step's MMAs have read their slot
+              if (leader && prev >= 0) mbar_arrive(&b_empty[prev]);
+              prev = slot;
+            }
+            first = false;
+            a_cur += a.DIL;
+            if (++slot == RING) { slot = 0; bphase ^= 1; }
+          }
+        }
+        tc::wgmma_wait<0>();
+        tc::fence_regs(d);
+        if (leader) {
+          if (prev >= 0) mbar_arrive(&b_empty[prev]);
+          mbar_arrive(&a_empty[buf]);
+        }
+        if (++buf == NABUF) { buf = 0; aphase ^= 1; }
+      }
+      if constexpr (!PAIR) {
+        tc_epilogue<TN>(a, d, b, t0, blockIdx.y * TN, lim, row_a);
+      } else {
+        // ---- conv-1 epilogue: bias, leaky-relu, hi/lo split -> conv-2 A operand (rows = steps t0 - H2 + row)
+        named_bar_sync(1, 256);   // both warpgroups are done reading the conv-2 operand of the previous tile
+        unsigned char* a2h = a2buf;
+        unsigned char* a2l = a2buf + (TN / 8) * ROWS2 * 16;
+        const int ta = t0 - H2 + row_a, tb = ta + 8;
+        // t lives on steps [0, lim): outside them conv 2 sees zero padding, not conv 1 evaluated on padding
+        const bool oka = ta >= 0 && ta < lim, okb = tb >= 0 && tb < lim;
+        const int csub = (lane & 3) * 2;
+#pragma unroll
+        for (int g = 0; g < TN / 8; ++g) {
+          const float2 bq = __ldg(reinterpret_cast<const float2*>(a.bias + 8 * g + csub));
+          float x[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) x[i] = (three ? fmaf(d[TN / 2 + 4 * g + i], tc::kLoInv, d[4 * g + i]) : d[4 * g + i]) + ((i & 1) ? bq.y : bq.x);
+          x[0] = oka ? fmaxf(x[0], x[0] * a.slope) : 0.f;
+          x[1] = oka ? fmaxf(x[1], x[1] * a.slope) : 0.f;
+          x[2] = okb ? fmaxf(x[2], x[2] * a.slope) : 0.f;
+          x[3] = okb ? fmaxf(x[3], x[3] * a.slope) : 0.f;
+          const __half2 ha = __floats2half2_rn(x[0], x[1]), hb = __floats2half2_rn(x[2], x[3]);
+          const float2 fa = __half22float2(ha), fb = __half22float2(hb);
+          const __half2 la = __floats2half2_rn((x[0] - fa.x) * tc::kLoScale, (x[1] - fa.y) * tc::kLoScale);
+          const __half2 lb = __floats2half2_rn((x[2] - fb.x) * tc::kLoScale, (x[3] - fb.y) * tc::kLoScale);
+          const int oa = (g * ROWS2 + row_a) * 16 + (lane & 3) * 4, ob = oa + 8 * 16;
+          *reinterpret_cast<__half2*>(a2h + oa) = ha;
+          *reinterpret_cast<__half2*>(a2h + ob) = hb;
+          *reinterpret_cast<__half2*>(a2l + oa) = la;
+          *reinterpret_cast<__half2*>(a2l + ob) = lb;
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> tensor-core (async) proxy
+        named_bar_sync(2, 256);   // every row of the conv-2 operand is written
+        // ---- conv 2 (dilation 1, weights in the resident slots after conv 1's)
+        const uint64_t a2_proto = tc::make_desc(0, LBO_A2, SBO);
+        tc::fence_regs(d);
+        tc::wgmma_fence();
+        bool first2 = true;
+        for (int kk = 0; kk < TN / 16; ++kk) {
+          uint64_t a_cur = a2_proto + ((tc::smem_addr(a2buf) + 64 * wg * 16 + 2 * kk * LBO_A2) >> 4);
+          for (int tap = 0; tap < a.K; ++tap) {
+            tc_mma_step<TN>(d, a_cur, a_cur + A2_LO16, b_ring + (uint32_t)(n_slots + kk * a.K + tap) * SLOT16, three, first2);
+            first2 = false;
+            a_cur += 1;
+          }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::fence_regs(d);
+        TcConvArgs e = a;
+        e.y_ld = TN; e.r = a.x; e.bias = a.bias2; e.bias_bs = 0; e.epi = 0;
+        tc_epilogue<TN>(e, d, b, t0, 0, min(lim, t0 + R), row_a);
+      }
     }
   }
 #undef TCN_FOR_TILES
-  tc::fence_before();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem_d, Cfg::TMEM_COLS);
 }
-#undef OVC_TC_ISSUE_MMAS
 
 // conv_post on channels-last input: y[b, t] = tanh(sum_{k<7, ci<C} w[ci, k] * lrelu_0.01(x[b, t+k-3, ci]))
 // (models.py:287-289).  HBM-bound (132 B per sample): a CTA stages 256+6 rows with coalesced 16-byte loads into a

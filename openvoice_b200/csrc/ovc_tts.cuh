@@ -195,7 +195,7 @@ __global__ void tts_dense_kernel(const float* x, const long long* lens, const fl
   out[((size_t)b * T + t) * N + n] = ovc_tts::dense_at(x + (size_t)b * T * Cin, w, bias, Cin, K, N, t, n, len, relu_in);
 }
 
-// channels-last rows -> the [C][P] layout of the FFMA2 conv kernels (ovc_conv.cuh) and back; P = T rounded up to 4.
+// channels-last rows -> the [C][P] layout of the FFMA conv kernels (ovc_conv.cuh) and back; P = T rounded up to 4.
 // grid (ceil(P/32), ceil(C/32), B), block (32, 8): 32x32 tiles through shared memory, both sides coalesced
 __global__ void tts_to_ct_kernel(const float* x, const long long* lens, int T, int C, int P, float* out) {
   __shared__ float tile[32][33];

@@ -104,8 +104,8 @@ OVC_HD float attn_out(const float* scores_row, const float* qkv_b, int ld, int H
 
 // ---- dense 'same' conv, one output element, plain fp32 FMA chain               attentions.py:439-448, models.py:90-96
 // The k = 3 convs of the FFN and the DurationPredictor contract over up to 3 * 768 terms; on the tensor cores the
-// TMEM accumulator's truncation costs ~3e-5 of the row there (DESIGN.md), which the spline inverses of the SDP amplify
-// into duration flips -- so these four layers stay on the CUDA cores.  w is stored [K][Cin][N] (n contiguous: a
+// accumulator's truncating adds over that many terms cost far more than fp32 rounding, which the spline inverses of the
+// SDP amplify into duration flips -- so these four layers stay on the CUDA cores.  w is stored [K][Cin][N] (n contiguous: a
 // warp of consecutive n reads coalesced weights and one broadcast activation).  relu_in: relu on the input rows.
 OVC_HD float dense_at(const float* x_b, const float* w, const float* bias, int Cin, int K, int N, int t, int n, int len,
                       int relu_in) {

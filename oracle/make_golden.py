@@ -1,7 +1,8 @@
-"""Generate tests/golden/*.npz by running the REAL reference from /root/reference.
+"""Generate tests/golden/*.npz by running the REAL reference (a checkout of myshell-ai/OpenVoice).
 
-Run in the build container only (``python oracle/make_golden.py``): /root/reference does not
-exist on the GPU box.  The reference ships no tests or golden vectors (SURVEY.md section 8c),
+Run on a machine that has the reference checked out:
+``OPENVOICE_REFERENCE=<path to the checkout> python oracle/make_golden.py``.  The tests only read the
+committed vectors, so nothing else in the project needs the reference.  The reference ships no tests or golden vectors (SURVEY.md section 8c),
 so parity is pinned on outputs of the reference's own code -- ``SynthesizerTrn.voice_conversion``
 (openvoice/models.py:492-499), ``ToneColorConverter.convert`` (openvoice/api.py:141-160),
 ``spectrogram_torch`` (openvoice/mel_processing.py:40-75) and ``ReferenceEncoder``
@@ -31,7 +32,10 @@ import vc_oracle as O  # noqa: E402
 
 
 def import_reference():
-    sys.path.insert(0, "/root/reference")
+    ref = os.environ.get("OPENVOICE_REFERENCE")
+    if not ref or not os.path.isdir(ref):
+        raise SystemExit("set OPENVOICE_REFERENCE to a checkout of myshell-ai/OpenVoice")
+    sys.path.insert(0, ref)
     lib = types.ModuleType("librosa")
     lib.filters = types.ModuleType("librosa.filters")
     lib.filters.mel = lambda *a, **k: None

@@ -5,11 +5,11 @@ restatement (torch CPU, fp32 or fp64) of what the reference computes on
 ``ToneColorConverter.convert -> SynthesizerTrn.voice_conversion``.  Only
 ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s cpu_baseline /
 ``--impl reference`` leg may import it.  The product (``openvoice_b200``) never
-does: its only compute path is the sm_100a CUDA library and it fails loudly
+does: its only compute path is the sm_90a CUDA library and it fails loudly
 without it.
 
-Parity pinning: ``oracle/make_golden.py`` imports the real reference from
-``/root/reference`` (in the build container only), drives the reference's own
+Parity pinning: ``oracle/make_golden.py`` imports the real reference from the
+checkout named by ``OPENVOICE_REFERENCE``, drives the reference's own
 ``SynthesizerTrn.voice_conversion`` / ``ToneColorConverter.convert`` /
 ``spectrogram_torch`` / ``ReferenceEncoder`` on the seeded synthetic checkpoint
 below and commits the results under ``tests/golden/``;
@@ -17,7 +17,7 @@ below and commits the results under ``tests/golden/``;
 reference ships no tests / golden vectors of its own -- SURVEY.md section 8c).
 
 Every function cites the reference lines it follows (paths relative to
-``/root/reference``).  Tensors are ``[B, C, T]`` like the reference.
+the reference repository's root).  Tensors are ``[B, C, T]`` like the reference.
 """
 from __future__ import annotations
 

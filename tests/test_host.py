@@ -31,11 +31,11 @@ def test_library_exports_every_declared_symbol():
     assert lib.ovc_abi_version() == _native.ABI_VERSION
 
 
-def test_library_contains_sm100a_tma_code():
-    """The shipped cubin is sm_100a and stages weights with TMA bulk copies (UBLKCP)."""
+def test_library_contains_sm90a_tma_code():
+    """The shipped cubin is sm_90a and stages weights with TMA bulk copies (UBLKCP)."""
     lib = os.path.join(ROOT, "openvoice_b200", "libovc_b200.so")
     out = subprocess.run(["cuobjdump", "-lelf", lib], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     sass = subprocess.run(["bash", "-c", f"cuobjdump -sass -fun '_ZN3ovc10conv1d_f32INS_7ConvCfgILi1ELi1ELi2ELi2ELi8ELi2ELi1ELi16EEEEEvNS_8ConvArgsE' {lib} | grep -c -E 'UBLKCP|SYNCS'"],
                           capture_output=True, text=True).stdout.strip()
     assert int(sass or 0) > 0

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """One small conversion that exercises every tensor-core kernel for compute-sanitizer: the sequential schedule (fused conv
-pairs, tcpair_kernel) and the concurrent-branch schedule of small calls, checked against the oracle."""
+pairs, tcconv_kernel<C, true>) and the concurrent-branch schedule of small calls, checked against the oracle."""
 import os
 import sys
 

@@ -58,7 +58,7 @@ def main():
                      "graph_replays": int(conv.model.native.graph_replays)})
         print(f"B={B:4d} x {secs:5.1f} s: {ms:9.2f} ms  {rows[-1]['audio_s_per_s']:9.1f} audio-s/s", flush=True)
     res = {"what": f"ToneColorConverter.convert_batch, host numpy in / out, max_batch {args.max_batch}, {args.precision}, "
-                   "median wall time, one B200", "points": rows}
+                   "median wall time, one H100", "points": rows}
     if args.json:
         json.dump(res, open(args.json, "w"), indent=1)
 

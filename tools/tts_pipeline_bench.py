@@ -1,4 +1,4 @@
-"""BASELINE.json config 3: V1 full pipeline BaseSpeakerTTS.tts + ToneColorConverter.convert, batch 16, one B200.
+"""BASELINE.json config 3: V1 full pipeline BaseSpeakerTTS.tts + ToneColorConverter.convert, batch 16, one H100.
 
 Synthetic checkpoints (no network), token sequences of the length SURVEY.md section 8 measured for a sentence
 (T_text = 121 incl. blanks).  Timed with CUDA events after warm-up:
