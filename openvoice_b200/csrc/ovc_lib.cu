@@ -102,10 +102,9 @@ struct ConvLayer {
 };
 
 // one ResBlock conv as the tensor-core kernel sees it (pre-split hi/lo weights in operand layout)
-struct TcLayer {
+struct TcLayer : TcGeom {
   size_t w_off = 0;   // float offsets into the tc weight arena
   size_t b_off = 0;
-  int Cin = 0, Ntot = 0, K = 0, DIL = 1, TN = 0;
 };
 
 struct WNLayers {
@@ -389,32 +388,16 @@ static int pack_wn(ovc_ctx* c, const std::string& prefix, int n_layers, WNLayers
 }
 
 // tensor-core copy of a conv: fp16 [n_tile][Cin/16][K][column block][hi|lo][TN][8]: hi = fp16(w), lo = fp16((w - hi) * 2^11)
-// (ovc_tc.cuh), laid out exactly as the kernel's shared-memory operand slots (one TMA bulk copy per slot)
+// (ovc_tcpack.h), laid out exactly as the kernel's shared-memory operand slots (one TMA bulk copy per slot)
 template <class WF, class BF>
 static TcLayer pack_tc(ovc_ctx* c, int Ntot, int Cin, int K, int DIL, WF wfun, BF bfun) {
   TcLayer T;
   T.Cin = Cin; T.Ntot = Ntot; T.K = K; T.DIL = DIL;
-  T.TN = Ntot % 128 == 0 ? 128 : (Ntot % 64 == 0 ? 64 : 32);   // widest column tile that divides the row
-  // the kernels stage 32 input channels at a time (128-byte rows for the activation TMA); halo tile = 2 * 25 rows at most
-  if (Ntot % 32 || Cin % 32 || (K - 1) / 2 * DIL > 25) { T.TN = 0; return T; }
+  T.TN = tc_tile_n(Ntot, Cin, K, DIL);
+  if (!T.TN) return T;
   T.w_off = round_up(c->h_tcw.size(), 64);
-  const int slot = 16 * T.TN;   // floats: 2 (hi|lo) x 2 (column blocks) x TN x 8 halfs
-  c->h_tcw.resize(T.w_off + (size_t)(Ntot / T.TN) * (Cin / 16) * K * slot, 0.f);
-  uint16_t* dst = reinterpret_cast<uint16_t*>(c->h_tcw.data() + T.w_off);
-  for (int nt = 0; nt < Ntot / T.TN; ++nt)
-    for (int k16 = 0; k16 < Cin / 16; ++k16)
-      for (int tap = 0; tap < K; ++tap) {
-        uint16_t* sl = dst + (((size_t)nt * (Cin / 16) + k16) * K + tap) * (2 * slot);
-        for (int kc = 0; kc < 2; ++kc)
-          for (int n = 0; n < T.TN; ++n)
-            for (int e = 0; e < 8; ++e) {
-              const float w = wfun(nt * T.TN + n, k16 * 16 + kc * 8 + e, tap);
-              const __half hi = __float2half_rn(w);
-              const __half lo = __float2half_rn((w - __half2float(hi)) * 2048.f);
-              sl[((kc * 2 + 0) * T.TN + n) * 8 + e] = __half_as_ushort(hi);   // rows [0, TN) of the 2*TN-row operand
-              sl[((kc * 2 + 1) * T.TN + n) * 8 + e] = __half_as_ushort(lo);   // rows [TN, 2*TN)
-            }
-      }
+  c->h_tcw.resize(T.w_off + tc_packed_halfs(Ntot, Cin, K, T.TN) / 2, 0.f);
+  tc_pack_weights(reinterpret_cast<uint16_t*>(c->h_tcw.data() + T.w_off), Ntot, Cin, K, T.TN, wfun);
   T.b_off = round_up(c->h_tcw.size(), 64);
   c->h_tcw.resize(T.b_off + Ntot, 0.f);
   for (int n = 0; n < Ntot; ++n) c->h_tcw[T.b_off + n] = bfun(n);
@@ -534,13 +517,9 @@ static int finalize(ovc_ctx* c) {
         [&](int co) { return b->data[co]; }, cout, 2, cout);
     c->dec_ups[i].out_mul = s;
     // tensor-core form: channels-last, row = ph * cout + co, so input step n yields the s output rows s*n .. s*n+s-1
+    auto raw = [&](int ci, int co, int k) { return w.data[((size_t)ci * cout + co) * kk + k]; };
     c->tc_ups[i] = pack_tc(
-        c, s * cout, cin, 3, 1,
-        [&](int row, int ci, int tap) {
-          const int ph = row / cout, co = row % cout;
-          const int kidx = s * (1 - tap) + ph + pad;
-          return (kidx >= 0 && kidx < kk) ? w.data[((size_t)ci * cout + co) * kk + kidx] : 0.f;
-        },
+        c, s * cout, cin, 3, 1, [&](int row, int ci, int tap) { return tc_ups_weight(raw, s, kk, cout, row, ci, tap); },
         [&](int row) { return b->data[row % cout]; });
     ch = cout;
     for (int j = 0; j < 3; ++j) {
@@ -917,10 +896,9 @@ static int launch_tc(Run& r, const TcLayer& T, const float* x, float* y, const f
   if (!(slope >= 0.f && slope <= 1.f)) return fail(OVC_ERR_INVALID, "leaky_relu slope %g outside [0, 1]", (double)slope);
   TRY(prof_begin(r));
   // persistent: one CTA per SM walks the (utterance, 128-step tile) list; column tiles (if any) on grid.y
-  const int n_tt = (t_len + 127) / 128, total = n_tt * r.B;
-  const int ncol = T.Ntot / T.TN;
-  const int per_col = std::max(1, r.c->sm_count / ncol / std::max(1, ex.grid_div));
-  dim3 pg((unsigned)std::min(total, per_col), ncol, 1);
+  const TcGrid g = tc_grid(t_len, r.B, T.Ntot, T.TN, r.c->sm_count, ex.grid_div);
+  const int n_tt = g.n_tt, total = g.total;
+  dim3 pg((unsigned)g.grid_x, g.ncol, 1);
   const bool pdl = r.c->use_pdl == 1 || (r.c->use_pdl == 2 && ex.epi != 0);
   if (T.TN == 128) CK(launch_ex(tcconv_kernel<128, false>, pg, TCN_THREADS, TcnCfg<128, false>::SMEM_BYTES, r.st, pdl, a, n_tt, total));
   else if (T.TN == 64) CK(launch_ex(tcconv_kernel<64, false>, pg, TCN_THREADS, TcnCfg<64, false>::SMEM_BYTES, r.st, pdl, a, n_tt, total));
@@ -934,15 +912,8 @@ static int launch_tc(Run& r, const TcLayer& T, const float* x, float* y, const f
   return OVC_OK;
 }
 
-// one ResBlock conv pair (c1 dilated, c2 dilation 1, residual = the pair's input) as ONE kernel: C = 64 / 32 stages.
-// Only where BOTH convs' weights stay resident in shared memory next to the operand tiles, and only the pairs whose
-// traffic is dominated by HBM (k <= 5): at larger k a tile's 128 - (k - 1) output steps waste more of the MMA work.
-static bool pair_fits(const TcLayer& T1, const TcLayer& T2) {
-  if (!(T1.TN == 32 || T1.TN == 64)) return false;
-  const int ring = T1.TN == 32 ? TcnCfg<32, true>::RING : TcnCfg<64, true>::RING;
-  return T1.Ntot == T1.TN && T1.Cin == T1.TN && T2.Ntot == T1.TN && T2.Cin == T1.TN && T2.TN == T1.TN && T2.K == T1.K &&
-         T2.DIL == 1 && (T1.K - 1) / 2 * T1.DIL <= TCN_HMAX && 2 * (T1.Cin / 16) * T1.K <= ring && T1.K <= 5;
-}
+// one ResBlock conv pair (c1 dilated, c2 dilation 1, residual = the pair's input) as ONE kernel: C = 64 / 32 stages,
+// where tc_pair_fits (ovc_tcpack.h) accepts the pair
 static int launch_pair(Run& r, const TcLayer& T1, const TcLayer& T2, const float* x, float* y, int t_len, int mul, float slope,
                        float scale, int accumulate) {
   TcConvArgs a{};
@@ -956,10 +927,10 @@ static int launch_pair(Run& r, const TcLayer& T1, const TcLayer& T2, const float
   a.Cin = C; a.Ntot = C; a.K = T1.K; a.DIL = T1.DIL;
   a.slope = slope; a.scale = scale; a.accumulate = accumulate;
   a.passes = r.c->precision == 2 ? 1 : 3;
-  const int R = 128 - (T1.K - 1);   // output steps per tile
-  const int n_tt = (t_len + R - 1) / R, total = n_tt * r.B;
+  const TcGrid g = tc_pair_grid(t_len, r.B, T1.K, r.c->sm_count);
+  const int n_tt = g.n_tt, total = g.total;
   TRY(prof_begin(r));
-  dim3 pg((unsigned)std::min(total, r.c->sm_count), 1, 1);
+  dim3 pg((unsigned)g.grid_x, 1, 1);
   if (C == 64) CK(launch_ex(tcconv_kernel<64, true>, pg, TCN_THREADS, TcnCfg<64, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
   else CK(launch_ex(tcconv_kernel<32, true>, pg, TCN_THREADS, TcnCfg<32, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
   CK(cudaGetLastError());
@@ -1231,7 +1202,7 @@ static int run_dec(Run& r, const WsLayout& W, float* ws, const float* cond, cons
       if (!par) {
         for (int j = 0; j < 3; ++j) {
           bool fused = c->use_pair;
-          for (int d = 0; d < 3; ++d) fused = fused && pair_fits(c->tc_c1[i * 3 + j][d], c->tc_c2[i * 3 + j][d]);
+          for (int d = 0; d < 3; ++d) fused = fused && tc_pair_fits(c->tc_c1[i * 3 + j][d], c->tc_c2[i * 3 + j][d]);
           if (fused) {
             // one kernel per conv pair; a pair never runs in place (its tiles read x with a halo), so the running
             // activation ping-pongs bufA -> bufB -> bufC -> bufD (bufC is free: the intermediate stays on chip)

@@ -82,7 +82,10 @@ template <int R> __device__ __forceinline__ void regs_alloc() { asm volatile("se
 
 // ---- split precision on fp16 operands ("3xFP16"):  x = hi + lo / 2^11 (+ 2^-23 |x|), hi = fp16(x),
 // lo = fp16((x - hi) * 2^11).  The remainder is scaled back into fp16's normal range, so the pair carries 22
-// mantissa bits for any |x| < 65504 (absolute floor 2^-36); a*b ~ ah*bh + (al*bh + ah*bl) / 2^11, the two cross
+// mantissa bits for 2^-14 <= |x| < 65520 and an absolute error of at most 2^-36 below (the hi and lo parts are then
+// fp16 subnormals, which the wgmma keeps: measured on an H100, tests/test_gpu_kernels.py).  At |x| >= 65520 hi rounds
+// to infinity: every output that reads such an operand is inf or NaN, never a finite wrong number.  Activations and
+// weights must therefore stay below 65520 in magnitude.  a*b ~ ah*bh + (al*bh + ah*bl) / 2^11, the two cross
 // terms accumulate in their own accumulator and the epilogue adds them with the 2^-11 factor.  fp16 MMAs run
 // at twice the TF32 rate and move half the operand bytes, at the same 11-bit-per-part precision as 3xTF32.
 constexpr float kLoScale = 2048.f, kLoInv = 1.f / 2048.f;

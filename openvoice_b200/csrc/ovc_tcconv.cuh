@@ -11,8 +11,9 @@
 // into the main one, a_hi * b_lo^T and a_lo * b_hi^T into the low-order one.  (A single 2*TN-wide MMA over both halves
 // followed by a TN-wide one into the upper half would save an A-operand read, but MMAs of different shapes on
 // overlapping accumulator registers make ptxas serialise the whole wgmma chain.)  Besides carrying the 2^-11 scale,
-// the second accumulator keeps the long hi*hi sum apart from the small cross terms.  Error ~1e-6 per conv, i.e.
-// fp32-grade.
+// the second accumulator keeps the long hi*hi sum apart from the small cross terms.  Measured per conv on an H100
+// (tests/test_gpu_kernels.py, DESIGN.md section 4.1): |y - y_fp64| <= 2^-18 * (sum |w||a| + |bias| + |res| + |y_old|)
+// elementwise, max |y - y_fp64| <= 3e-5 * rms(y); the single pass (passes = 1): 2^-10 and 4e-3.
 //
 // K-major, no-swizzle operand tiles (see ovc_tc.cuh): a convolution tap is a 16-byte-per-row shift of the A
 // descriptor's start address, so all taps (any dilation) read ONE staged halo tile.
@@ -32,6 +33,7 @@
 #pragma once
 #include "ovc_conv.cuh"
 #include "ovc_tc.cuh"
+#include "ovc_tcpack.h"
 
 namespace ovc {
 
@@ -163,7 +165,6 @@ __device__ __forceinline__ void tc_mma_step(float (&d)[TN], uint64_t a_hi, uint6
 
 constexpr int TCN_THREADS = 384;   // warpgroup 0: producers; warpgroups 1, 2: MMAs + epilogue
 constexpr int TCN_NCT = 96;        // converter threads (warps 1-3)
-constexpr int TCN_HMAX = 25;       // largest conv-1 halo (k = 11, dilation 5)
 
 template <int TN, bool PAIR>
 struct TcnCfg {
@@ -172,8 +173,7 @@ struct TcnCfg {
   static constexpr int ROWS = 194;                                // A pitch in rows: >= 128 + 2 * TCN_HMAX, = 2 (mod 8)
   static constexpr int ROWS2 = 146;                               // PAIR: conv-2 A pitch: 128 + 2 * H2 rows, H2 <= 9
   static constexpr int NABUF = 2;
-  // weight slots (16 channels x 1 tap): TN = 32 holds k = 11 resident, TN = 64 k = 3; pairs hold both convs
-  static constexpr int RING = PAIR ? (TN == 32 ? 44 : 24) : (TN == 32 ? 22 : 12);
+  static constexpr int RING = tc_ring_slots(TN, PAIR);            // weight slots (ovc_tcpack.h)
   static constexpr int SLOT_BYTES = 2 * 2 * TN * 16;
   static constexpr int A_BUF_BYTES = 2 * NKC * ROWS * 16;         // [hi|lo][column block][row][8 halfs]
   static constexpr int A2_BYTES = PAIR ? 2 * (TN / 8) * ROWS2 * 16 : 0;
@@ -206,7 +206,7 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
   const int n_slots = (a.Cin / 16) * a.K;      // weight slots per conv
   const int n_w = PAIR ? 2 * n_slots : n_slots;
   const bool resident = n_w <= RING;
-  if (H1 > TCN_HMAX || (PAIR && (!resident || 128 + 2 * H2 > ROWS2))) __trap();   // host: pack_tc / pair_fits
+  if (H1 > TCN_HMAX || (PAIR && (!resident || 128 + 2 * H2 > ROWS2))) __trap();   // host: tc_tile_n / tc_pair_fits (ovc_tcpack.h)
   constexpr uint32_t BYTES = Cfg::SLOT_BYTES;
 
   if (tid == 0) {
