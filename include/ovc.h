@@ -84,8 +84,10 @@ OVC_API void ovc_destroy(ovc_ctx* ctx);
 OVC_API int ovc_load_tensor(ovc_ctx* ctx, const char* key, const float* data, const int64_t* shape, int ndim);
 
 /* Fold weight-norm (g*v/||v||, per dim-0 slice), absorb the channel Flips of the flow into the
- * coupling weights, repack every conv for the kernels and upload.  OVC_ERR_MISSING names the
- * first missing key. */
+ * coupling weights, repack every conv for the kernels and upload.  Every tensor read is checked
+ * against the shape the model's hyper-parameters give it: OVC_ERR_MISSING names the first missing
+ * key, OVC_ERR_INVALID the first mis-shaped one (with its shape and the expected shape).  On
+ * failure the loaded tensors are kept, so the caller can replace the offending one and retry. */
 OVC_API int ovc_finalize_weights(ovc_ctx* ctx);
 
 /* Number of floats of device workspace a call with (B, Tmax) needs (informational; the arena

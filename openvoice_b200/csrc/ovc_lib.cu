@@ -60,6 +60,12 @@ struct DeviceGuard {
                   __LINE__);                                                                      \
   } while (0)
 
+#define TRY(expr)                   \
+  do {                              \
+    int rc_ = (expr);               \
+    if (rc_ != OVC_OK) return rc_;  \
+  } while (0)
+
 static const VariantInfo kInfo[V_COUNT] = {
 #define X(name, K, D, WM, WN, CI, EPI, NG, XA)                                                    \
   {#name, K, D, 32 * WM, 64 * WN, CI, EPI, 32 * WM * WN, ConvCfg<K, D, WM, WN, CI, EPI, NG, XA>::SMEM_BYTES},
@@ -255,28 +261,58 @@ static const HostTensor* find(const ovc_ctx* c, const std::string& k) {
   return it == c->sd.end() ? nullptr : &it->second;
 }
 
-// effective weight of a (possibly weight-normed) conv: g * v / ||v|| over dims != 0
-// (torch.nn.utils.weight_norm dim=0; modules.py:160,172,182, models.py:247)
-static int effective_weight(const ovc_ctx* c, const std::string& prefix, HostTensor* out, std::string* missing) {
-  if (const HostTensor* w = find(c, prefix + ".weight")) {
-    *out = *w;
-    return 0;
+static std::string shape_str(const std::vector<int64_t>& shape) {
+  std::string s = "[";
+  for (size_t i = 0; i < shape.size(); ++i) s += (i ? ", " : "") + (shape[i] < 0 ? std::string("*") : std::to_string(shape[i]));
+  return s + "]";
+}
+
+// checkpoint tensor `key` of the given shape (-1: any size, a dim the caller reads a hyper-parameter from).  Every
+// tensor the packing code indexes comes through here or conv_weight, so no index can run past a tensor's end.
+static int tensor(const ovc_ctx* c, const std::string& key, const std::vector<int64_t>& shape, const HostTensor** out) {
+  const HostTensor* t = find(c, key);
+  if (!t) return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing", key.c_str());
+  bool ok = t->shape.size() == shape.size();
+  for (size_t i = 0; ok && i < shape.size(); ++i) ok = shape[i] < 0 || t->shape[i] == shape[i];
+  if (!ok)
+    return fail(OVC_ERR_INVALID, "checkpoint tensor '%s' has shape %s, expected %s", key.c_str(), shape_str(t->shape).c_str(),
+                shape_str(shape).c_str());
+  *out = t;
+  return OVC_OK;
+}
+
+// effective weight of a (possibly weight-normed) conv: `.weight`, or g * v / ||v|| over dims != 0 with one g per
+// slice of v's dim 0 (torch.nn.utils.weight_norm dim=0; modules.py:160,172,182, models.py:247)
+static int conv_weight(const ovc_ctx* c, const std::string& prefix, const std::vector<int64_t>& shape, HostTensor* out) {
+  const HostTensor *v, *g;
+  if (find(c, prefix + ".weight")) {
+    TRY(tensor(c, prefix + ".weight", shape, &v));
+    *out = *v;
+    return OVC_OK;
   }
-  const HostTensor* v = find(c, prefix + ".weight_v");
-  const HostTensor* g = find(c, prefix + ".weight_g");
-  if (!v) { *missing = prefix + ".weight_v"; return -1; }
-  if (!g) { *missing = prefix + ".weight_g"; return -1; }
-  *out = *v;
+  TRY(tensor(c, prefix + ".weight_v", shape, &v));
   const int64_t d0 = v->shape[0];
   const int64_t inner = v->numel() / d0;
-  if (g->numel() != d0) { *missing = prefix + ".weight_g(shape)"; return -1; }
+  if (!(g = find(c, prefix + ".weight_g"))) return fail(OVC_ERR_MISSING, "checkpoint tensor '%s.weight_g' is missing", prefix.c_str());
+  if (g->numel() != d0)
+    return fail(OVC_ERR_INVALID, "checkpoint tensor '%s.weight_g' has shape %s, expected %lld elements", prefix.c_str(),
+                shape_str(g->shape).c_str(), (long long)d0);
+  *out = *v;
   for (int64_t i = 0; i < d0; ++i) {
     double ss = 0;
     for (int64_t j = 0; j < inner; ++j) { const double q = v->data[i * inner + j]; ss += q * q; }
     const float scale = g->data[i] / (float)std::sqrt(ss);
     for (int64_t j = 0; j < inner; ++j) out->data[i * inner + j] = v->data[i * inner + j] * scale;
   }
-  return 0;
+  return OVC_OK;
+}
+
+// append a plain fp32 blob to a weight arena; returns its (256-byte aligned) float offset
+static size_t append(std::vector<float>& arena, const std::vector<float>& v) {
+  const size_t o = round_up(arena.size(), 64);
+  arena.resize(o + v.size());
+  std::copy(v.begin(), v.end(), arena.begin() + o);
+  return o;
 }
 
 // append a packed conv to the staging arena.  wfun(row_packed, ci, k) -> weight; bfun(row) -> bias
@@ -361,32 +397,6 @@ static bool key_is_hot(const std::string& k) {
          k.rfind("enc_p.", 0) == 0 || k.rfind("dp.", 0) == 0 || k.rfind("sdp.", 0) == 0 || k.rfind("emb_g.", 0) == 0;
 }
 
-static int pack_wn(ovc_ctx* c, const std::string& prefix, int n_layers, WNLayers* out, std::string* missing) {
-  const int H = 192;
-  for (int i = 0; i < n_layers; ++i) {
-    HostTensor w;
-    const std::string pin = prefix + ".in_layers." + std::to_string(i);
-    if (effective_weight(c, pin, &w, missing)) return -1;
-    if (w.shape.size() != 3 || w.shape[0] != 2 * H || w.shape[1] != H || w.shape[2] != 5) { *missing = pin + "(shape)"; return -1; }
-    // bias of the in_layer is folded into the per-batch conditioning vector (cond kernel)
-    out->in.push_back(pack_conv(
-        c, V_WN_IN, 2 * H, H,
-        [&](int p, int ci, int k) { return w.data[((size_t)paired_row(p, H) * H + ci) * 5 + k]; },
-        [&](int) { return 0.f; }, 0, 5, 2 * H));
-    const std::string prs = prefix + ".res_skip_layers." + std::to_string(i);
-    HostTensor r;
-    if (effective_weight(c, prs, &r, missing)) return -1;
-    const HostTensor* rb = find(c, prs + ".bias");
-    if (!rb) { *missing = prs + ".bias"; return -1; }
-    const int rows = (i < n_layers - 1) ? 2 * H : H;
-    if (r.shape[0] != rows || r.shape[1] != H) { *missing = prs + "(shape)"; return -1; }
-    out->rs.push_back(pack_conv(
-        c, V_WN_RS, rows, H, [&](int p, int ci, int) { return r.data[(size_t)p * H + ci]; },
-        [&](int p) { return rb->data[p]; }, rows, 1, rows));
-  }
-  return 0;
-}
-
 // tensor-core copy of a conv: fp16 [n_tile][Cin/16][K][column block][hi|lo][TN][8]: hi = fp16(w), lo = fp16((w - hi) * 2^11)
 // (ovc_tcpack.h), laid out exactly as the kernel's shared-memory operand slots (one TMA bulk copy per slot)
 template <class WF, class BF>
@@ -404,26 +414,34 @@ static TcLayer pack_tc(ovc_ctx* c, int Ntot, int Cin, int K, int DIL, WF wfun, B
   return T;
 }
 
-static int pack_wn_tc(ovc_ctx* c, const std::string& prefix, int n_layers, WNLayers* out, std::string* missing) {
+// WN stack (modules.py:133-183): every layer folded once, packed for the FFMA kernels into h_w and for the
+// tensor-core kernels into h_tcw.  The in_layer biases reach the kernels through the conditioning vector.
+static int pack_wn(ovc_ctx* c, const std::string& prefix, int n_layers, WNLayers* out) {
   const int H = 192;
+  *out = WNLayers();
   for (int i = 0; i < n_layers; ++i) {
-    HostTensor w;
-    const std::string pin = prefix + ".in_layers." + std::to_string(i);
-    if (effective_weight(c, pin, &w, missing)) return -1;
+    HostTensor w, r;
+    const HostTensor* rb;
+    const std::string prs = prefix + ".res_skip_layers." + std::to_string(i);
+    const int rows = (i < n_layers - 1) ? 2 * H : H;
+    TRY(conv_weight(c, prefix + ".in_layers." + std::to_string(i), {2 * H, H, 5}, &w));
+    TRY(conv_weight(c, prs, {rows, H, 1}, &r));
+    TRY(tensor(c, prs + ".bias", {rows}, &rb));
+    out->in.push_back(pack_conv(
+        c, V_WN_IN, 2 * H, H,
+        [&](int p, int ci, int k) { return w.data[((size_t)paired_row(p, H) * H + ci) * 5 + k]; },
+        [&](int) { return 0.f; }, 0, 5, 2 * H));
+    out->rs.push_back(pack_conv(
+        c, V_WN_RS, rows, H, [&](int p, int ci, int) { return r.data[(size_t)p * H + ci]; },
+        [&](int p) { return rb->data[p]; }, rows, 1, rows));
     out->tc_in.push_back(pack_tc(
         c, 2 * H, H, 5, 1, [&](int p, int ci, int k) { return w.data[((size_t)paired_row32(p, H) * H + ci) * 5 + k]; },
-        [&](int) { return 0.f; }));   // bias comes per utterance from the cond kernel
-    const std::string prs = prefix + ".res_skip_layers." + std::to_string(i);
-    HostTensor r;
-    if (effective_weight(c, prs, &r, missing)) return -1;
-    const HostTensor* rb = find(c, prs + ".bias");
-    if (!rb) { *missing = prs + ".bias"; return -1; }
-    const int rows = (i < n_layers - 1) ? 2 * H : H;
+        [&](int) { return 0.f; }));
     out->tc_rs.push_back(pack_tc(
         c, rows, H, 1, 1, [&](int p, int ci, int) { return r.data[(size_t)p * H + ci]; },
         [&](int p) { return rb->data[p]; }));
   }
-  return 0;
+  return OVC_OK;
 }
 
 #include "ovc_tts_pack.inc"   // pack_tts(): V1 TTS front-half weights (text encoder, duration predictors, emb_g)
@@ -431,32 +449,22 @@ static int pack_wn_tc(ovc_ctx* c, const std::string& prefix, int n_layers, WNLay
 static int finalize(ovc_ctx* c) {
   const ovc_hparams& hp = c->hp;
   const int H = 192, S = hp.spec_channels, G = hp.gin_channels;
-  std::string miss;
   drop_graphs(c);               // captured launches point at the old weight arenas
   c->h_w.clear();
   c->h_tcw.clear();
-#define NEED(ptr, key)                                                                     \
-  const HostTensor* ptr = find(c, key);                                                    \
-  if (!ptr) return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing", std::string(key).c_str())
-#define WEFF(var, prefix)                                                                  \
-  HostTensor var;                                                                          \
-  if (effective_weight(c, prefix, &var, &miss)) return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing or mis-shaped", miss.c_str())
 
   // ---- posterior encoder (models.py:182-221)
   {
-    NEED(w, "enc_q.pre.weight");
-    NEED(b, "enc_q.pre.bias");
-    if (w->shape.size() != 3 || w->shape[0] != H || w->shape[1] != S) return fail(OVC_ERR_INVALID, "enc_q.pre.weight has the wrong shape");
+    const HostTensor *w, *b, *pw, *pb;
+    TRY(tensor(c, "enc_q.pre.weight", {H, S, 1}, &w));
+    TRY(tensor(c, "enc_q.pre.bias", {H}, &b));
     c->enc_pre = pack_conv(c, V_ENC_PRE, H, S, [&](int p, int ci, int) { return w->data[(size_t)p * S + ci]; },
                            [&](int p) { return b->data[p]; }, H, 1, H);
     c->enc_pre16 = c->enc_pre;            // same packing, 16-byte cp.async when the spectrogram pitch allows it
     c->enc_pre16.variant = V_FLOW_PRE;
-    c->enc_wn = WNLayers();
-    if (pack_wn(c, "enc_q.enc", 16, &c->enc_wn, &miss) || pack_wn_tc(c, "enc_q.enc", 16, &c->enc_wn, &miss))
-      return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing or mis-shaped", miss.c_str());
-    NEED(pw, "enc_q.proj.weight");
-    NEED(pb, "enc_q.proj.bias");
-    if (pw->shape[0] != 2 * H || pw->shape[1] != H) return fail(OVC_ERR_INVALID, "enc_q.proj.weight has the wrong shape");
+    TRY(pack_wn(c, "enc_q.enc", 16, &c->enc_wn));
+    TRY(tensor(c, "enc_q.proj.weight", {2 * H, H, 1}, &pw));
+    TRY(tensor(c, "enc_q.proj.bias", {2 * H}, &pb));
     c->enc_proj = pack_conv(c, V_ENC_PROJ, 2 * H, H,
                             [&](int p, int ci, int) { return pw->data[(size_t)paired_row(p, H) * H + ci]; },
                             [&](int p) { return pb->data[paired_row(p, H)]; }, 2 * H, 1, 2 * H);
@@ -467,29 +475,25 @@ static int finalize(ovc_ctx* c) {
   for (int f = 0; f < 4; ++f) {
     const std::string p = "flow.flows." + std::to_string(2 * f);
     const bool flipped = f & 1;
-    NEED(w, p + ".pre.weight");
-    NEED(b, p + ".pre.bias");
-    if (w->shape[0] != H || w->shape[1] != 96) return fail(OVC_ERR_INVALID, "%s.pre.weight has the wrong shape", p.c_str());
+    const HostTensor *w, *b, *pw, *pb;
+    TRY(tensor(c, p + ".pre.weight", {H, 96, 1}, &w));
+    TRY(tensor(c, p + ".pre.bias", {H}, &b));
     c->flow_pre[f] = pack_conv(
         c, V_FLOW_PRE, H, 96,
         [&](int r, int ci, int) { return w->data[(size_t)r * 96 + (flipped ? 95 - ci : ci)]; },
         [&](int r) { return b->data[r]; }, H, 1, H);
-    c->flow_wn[f] = WNLayers();
-    if (pack_wn(c, p + ".enc", 4, &c->flow_wn[f], &miss) || pack_wn_tc(c, p + ".enc", 4, &c->flow_wn[f], &miss))
-      return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing or mis-shaped", miss.c_str());
-    NEED(pw, p + ".post.weight");
-    NEED(pb, p + ".post.bias");
-    if (pw->shape[0] != 96 || pw->shape[1] != H) return fail(OVC_ERR_INVALID, "%s.post.weight has the wrong shape (mean_only couplings only)", p.c_str());
+    TRY(pack_wn(c, p + ".enc", 4, &c->flow_wn[f]));
+    TRY(tensor(c, p + ".post.weight", {96, H, 1}, &pw));   // mean_only couplings only
+    TRY(tensor(c, p + ".post.bias", {96}, &pb));
     c->flow_post[f] = pack_conv(
         c, V_FLOW_POST, 96, H,
         [&](int r, int ci, int) { return pw->data[(size_t)(flipped ? 95 - r : r) * H + ci]; },
         [&](int r) { return pb->data[flipped ? 95 - r : r]; }, 96, 1, 96);
   }
   // ---- generator (models.py:224-291)
-  NEED(cpb, "dec.conv_pre.bias");
   {
-    NEED(w, "dec.conv_pre.weight");
-    if (w->shape[0] != 512 || w->shape[1] != H || w->shape[2] != 7) return fail(OVC_ERR_INVALID, "dec.conv_pre.weight has the wrong shape");
+    const HostTensor* w;
+    TRY(tensor(c, "dec.conv_pre.weight", {512, H, 7}, &w));
     // bias comes per batch item from the cond kernel (conv_pre.bias + cond(g))
     c->dec_pre = pack_conv(c, V_A_K7D1, 512, H, [&](int r, int ci, int k) { return w->data[((size_t)r * H + ci) * 7 + k]; },
                            [&](int) { return 0.f; }, 0, 7, 512);
@@ -501,9 +505,10 @@ static int finalize(ovc_ctx* c) {
     const int s = hp.upsample_rates[i], kk = hp.upsample_kernel_sizes[i], pad = (kk - s) / 2;
     const int cin = ch, cout = ch / 2;
     const std::string p = "dec.ups." + std::to_string(i);
-    WEFF(w, p);   // [cin][cout][kk], weight-norm over dim 0 = cin (SURVEY appendix C.12)
-    NEED(b, p + ".bias");
-    if (w.shape[0] != cin || w.shape[1] != cout || w.shape[2] != kk) return fail(OVC_ERR_INVALID, "%s weight has the wrong shape", p.c_str());
+    HostTensor w;   // [cin][cout][kk], weight-norm over dim 0 = cin (SURVEY appendix C.12)
+    const HostTensor* b;
+    TRY(conv_weight(c, p, {cin, cout, kk}, &w));
+    TRY(tensor(c, p + ".bias", {cout}, &b));
     const int variant = s == 8 ? V_UPS8_A : (cout * s >= 128 ? V_UPS2_A : V_UPS2_B);
     // polyphase: out[co, s*n+ph] = sum_ci sum_m x[ci, n-m] * W[ci, co, s*m + ph + pad];
     // packed row = co*s + ph, tap 0/1/2 <-> x[n-1], x[n], x[n+1] <-> m = 1, 0, -1
@@ -528,9 +533,10 @@ static int finalize(ovc_ctx* c) {
       for (int d = 0; d < 3; ++d) {
         for (int which = 0; which < 2; ++which) {
           const std::string q = "dec.resblocks." + std::to_string(rbi) + (which ? ".convs2." : ".convs1.") + std::to_string(d);
-          WEFF(rw, q);
-          NEED(rbias, q + ".bias");
-          if (rw.shape[0] != ch || rw.shape[1] != ch || rw.shape[2] != K) return fail(OVC_ERR_INVALID, "%s weight has the wrong shape", q.c_str());
+          HostTensor rw;
+          const HostTensor* rbias;
+          TRY(conv_weight(c, q, {ch, ch, K}, &rw));
+          TRY(tensor(c, q + ".bias", {ch}, &rbias));
           const int dil = which ? 1 : hp.resblock_dilations[j][d];
           ConvLayer L = pack_conv(c, dec_variant(ch, K, dil), ch, ch,
                                   [&](int r, int ci, int k) { return rw.data[((size_t)r * ch + ci) * K + k]; },
@@ -544,61 +550,51 @@ static int finalize(ovc_ctx* c) {
     }
   }
   {
-    NEED(w, "dec.conv_post.weight");
-    if (w->shape[0] != 1 || w->shape[1] != 32 || w->shape[2] != 7) return fail(OVC_ERR_INVALID, "dec.conv_post.weight has the wrong shape");
-    c->post_w_off = round_up(c->h_w.size(), 64);
-    c->h_w.resize(c->post_w_off + 32 * 7);
-    std::copy(w->data.begin(), w->data.end(), c->h_w.begin() + c->post_w_off);
+    const HostTensor* w;
+    TRY(tensor(c, "dec.conv_post.weight", {1, 32, 7}, &w));
+    c->post_w_off = append(c->h_w, w->data);
   }
   // ---- speaker conditioning mat-vec: stack cond_layer of enc_q, of the 4 couplings and dec.cond
   std::vector<int> wrow, sel;
   std::vector<float> cbias;
   {
     std::vector<float> cw;
-    auto add_wn = [&](const std::string& prefix, int n_layers, int first_row, int selv, bool add_matrix, bool tc_order = false) -> int {
+    struct WnCond { int first_row; const HostTensor* b; std::vector<const HostTensor*> in_b; };
+    WnCond wc[5];   // 0: enc_q, 1..4: the couplings
+    for (int s = 0; s < 5; ++s) {
+      const std::string p = s ? "flow.flows." + std::to_string(2 * s - 2) + ".enc" : std::string("enc_q.enc");
+      const int n_layers = s ? 4 : 16;
       HostTensor w;
-      if (effective_weight(c, prefix + ".cond_layer", &w, &miss)) return -1;
-      const HostTensor* cb = find(c, prefix + ".cond_layer.bias");
-      if (!cb) { miss = prefix + ".cond_layer.bias"; return -1; }
-      if (w.shape[0] != 2 * H * n_layers || w.shape[1] != G) { miss = prefix + ".cond_layer(shape)"; return -1; }
-      if (add_matrix) cw.insert(cw.end(), w.data.begin(), w.data.end());
-      for (int l = 0; l < n_layers; ++l) {
-        const HostTensor* ib = find(c, prefix + ".in_layers." + std::to_string(l) + ".bias");
-        if (!ib) { miss = prefix + ".in_layers." + std::to_string(l) + ".bias"; return -1; }
-        for (int p = 0; p < 2 * H; ++p) {
-          const int o = tc_order ? paired_row32(p, H) : paired_row(p, H);
-          wrow.push_back(first_row + l * 2 * H + o);
-          sel.push_back(selv);
-          cbias.push_back(cb->data[l * 2 * H + o] + ib->data[o]);
-        }
+      TRY(conv_weight(c, p + ".cond_layer", {2 * H * n_layers, G, 1}, &w));
+      TRY(tensor(c, p + ".cond_layer.bias", {2 * H * n_layers}, &wc[s].b));
+      wc[s].in_b.resize(n_layers);
+      for (int l = 0; l < n_layers; ++l) TRY(tensor(c, p + ".in_layers." + std::to_string(l) + ".bias", {2 * H}, &wc[s].in_b[l]));
+      wc[s].first_row = (int)(cw.size() / G);
+      cw.insert(cw.end(), w.data.begin(), w.data.end());
+    }
+    // sections enc_q, couplings on the source speaker, couplings on the target speaker; then the same three in the
+    // tensor-core kernel's column order
+    int (*const order[2])(int, int) = {paired_row, paired_row32};
+    int* const off[2][3] = {{&c->cond_off_enc, &c->cond_off_fsrc, &c->cond_off_ftgt},
+                            {&c->cond_off_enc_tc, &c->cond_off_fsrc_tc, &c->cond_off_ftgt_tc}};
+    const int selv[3] = {hp.zero_g ? 0 : 1, 1, 2};
+    for (int o = 0; o < 2; ++o)
+      for (int sec = 0; sec < 3; ++sec) {
+        *off[o][sec] = (int)wrow.size();
+        for (int s = sec ? 1 : 0; s < (sec ? 5 : 1); ++s)
+          for (int l = 0; l < (int)wc[s].in_b.size(); ++l)
+            for (int p = 0; p < 2 * H; ++p) {
+              const int r = order[o](p, H);
+              wrow.push_back(wc[s].first_row + l * 2 * H + r);
+              sel.push_back(selv[sec]);
+              cbias.push_back(wc[s].b->data[l * 2 * H + r] + wc[s].in_b[l]->data[r]);
+            }
       }
-      return 0;
-    };
-    c->cond_off_enc = 0;
-    if (add_wn("enc_q.enc", 16, 0, hp.zero_g ? 0 : 1, true)) return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing or mis-shaped", miss.c_str());
-    c->cond_off_fsrc = (int)wrow.size();
-    for (int f = 0; f < 4; ++f)
-      if (add_wn("flow.flows." + std::to_string(2 * f) + ".enc", 4, 16 * 2 * H + f * 4 * 2 * H, 1, true))
-        return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing or mis-shaped", miss.c_str());
-    c->cond_off_ftgt = (int)wrow.size();
-    for (int f = 0; f < 4; ++f)
-      if (add_wn("flow.flows." + std::to_string(2 * f) + ".enc", 4, 16 * 2 * H + f * 4 * 2 * H, 2, false))
-        return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing or mis-shaped", miss.c_str());
-    // the same conditioning vectors once more in the tensor-core kernel's column order
-    c->cond_off_enc_tc = (int)wrow.size();
-    if (add_wn("enc_q.enc", 16, 0, hp.zero_g ? 0 : 1, false, true)) return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing or mis-shaped", miss.c_str());
-    c->cond_off_fsrc_tc = (int)wrow.size();
-    for (int f = 0; f < 4; ++f)
-      if (add_wn("flow.flows." + std::to_string(2 * f) + ".enc", 4, 16 * 2 * H + f * 4 * 2 * H, 1, false, true))
-        return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing or mis-shaped", miss.c_str());
-    c->cond_off_ftgt_tc = (int)wrow.size();
-    for (int f = 0; f < 4; ++f)
-      if (add_wn("flow.flows." + std::to_string(2 * f) + ".enc", 4, 16 * 2 * H + f * 4 * 2 * H, 2, false, true))
-        return fail(OVC_ERR_MISSING, "checkpoint tensor '%s' is missing or mis-shaped", miss.c_str());
+    const HostTensor *dw, *db, *cpb;
+    TRY(tensor(c, "dec.cond.weight", {512, G, 1}, &dw));
+    TRY(tensor(c, "dec.cond.bias", {512}, &db));
+    TRY(tensor(c, "dec.conv_pre.bias", {512}, &cpb));
     c->cond_off_dec = (int)wrow.size();
-    NEED(dw, "dec.cond.weight");
-    NEED(db, "dec.cond.bias");
-    if (dw->shape[0] != 512 || dw->shape[1] != G) return fail(OVC_ERR_INVALID, "dec.cond.weight has the wrong shape");
     const int dec_first = (int)(cw.size() / G);
     cw.insert(cw.end(), dw->data.begin(), dw->data.end());
     for (int r = 0; r < 512; ++r) {
@@ -607,55 +603,40 @@ static int finalize(ovc_ctx* c) {
       cbias.push_back(db->data[r] + cpb->data[r]);
     }
     c->cond_rows_out = (int)wrow.size();
-    c->cond_w_off = round_up(c->h_w.size(), 64);
-    c->h_w.resize(c->cond_w_off + cw.size());
-    std::copy(cw.begin(), cw.end(), c->h_w.begin() + c->cond_w_off);
-    c->cond_b_off = round_up(c->h_w.size(), 64);
-    c->h_w.resize(c->cond_b_off + cbias.size());
-    std::copy(cbias.begin(), cbias.end(), c->h_w.begin() + c->cond_b_off);
+    c->cond_w_off = append(c->h_w, cw);
+    c->cond_b_off = append(c->h_w, cbias);
   }
   // ---- ReferenceEncoder (optional: only extract_se needs it; models.py:301-338)
   c->has_refenc = false;
   if (find(c, "ref_enc.proj.weight")) {
-    auto put = [&](const std::vector<float>& v) { size_t o = round_up(c->h_w.size(), 64); c->h_w.resize(o + v.size()); std::copy(v.begin(), v.end(), c->h_w.begin() + o); return o; };
     static const int filt[7] = {1, 32, 32, 64, 64, 128, 128};
     for (int i = 0; i < 6; ++i) {
       const std::string q = "ref_enc.convs." + std::to_string(i);
-      WEFF(cw, q);
-      NEED(cb, q + ".bias");
-      if (cw.shape.size() != 4 || cw.shape[0] != filt[i + 1] || cw.shape[1] != filt[i] || cw.shape[2] != 3 || cw.shape[3] != 3)
-        return fail(OVC_ERR_INVALID, "%s weight has the wrong shape", q.c_str());
-      c->re_conv_w[i] = put(cw.data);
-      c->re_conv_b[i] = put(cb->data);
+      HostTensor w;
+      const HostTensor* b;
+      TRY(conv_weight(c, q, {filt[i + 1], filt[i], 3, 3}, &w));
+      TRY(tensor(c, q + ".bias", {filt[i + 1]}, &b));
+      c->re_conv_w[i] = append(c->h_w, w.data);
+      c->re_conv_b[i] = append(c->h_w, b->data);
     }
-    NEED(wih, "ref_enc.gru.weight_ih_l0"); NEED(whh, "ref_enc.gru.weight_hh_l0");
-    NEED(bih, "ref_enc.gru.bias_ih_l0"); NEED(bhh, "ref_enc.gru.bias_hh_l0");
-    NEED(rpw, "ref_enc.proj.weight"); NEED(rpb, "ref_enc.proj.bias");
-    NEED(lng, "ref_enc.layernorm.weight"); NEED(lnb, "ref_enc.layernorm.bias");
-    if (wih->shape[0] != 384 || whh->shape[0] != 384 || whh->shape[1] != 128 || rpw->shape[0] != G || rpw->shape[1] != 128 ||
-        lng->shape[0] != S)
-      return fail(OVC_ERR_INVALID, "ref_enc.* tensors have the wrong shape");
-    {
-      int w6 = S;   // width after the six stride-2 convs (models.py:330-337)
-      for (int i = 0; i < 6; ++i) w6 = (w6 - 1) / 2 + 1;
-      if (wih->shape.size() != 2 || wih->shape[1] != 128 * w6 || bih->numel() != 384 || bhh->numel() != 384 ||
-          lnb->numel() != S || rpb->numel() != G)
-        return fail(OVC_ERR_INVALID, "ref_enc.gru / layernorm / proj tensors do not match spec_channels %d (GRU input %d expected)",
-                    S, 128 * w6);
-      c->re_gru_in = 128 * w6;
+    int w6 = S;   // width after the six stride-2 convs (models.py:330-337)
+    for (int i = 0; i < 6; ++i) w6 = (w6 - 1) / 2 + 1;
+    c->re_gru_in = 128 * w6;
+    const struct { const char* key; std::vector<int64_t> shape; size_t* off; } re[8] = {
+        {"ref_enc.gru.weight_ih_l0", {384, c->re_gru_in}, &c->re_wih}, {"ref_enc.gru.weight_hh_l0", {384, 128}, &c->re_whh},
+        {"ref_enc.gru.bias_ih_l0", {384}, &c->re_bih},                 {"ref_enc.gru.bias_hh_l0", {384}, &c->re_bhh},
+        {"ref_enc.proj.weight", {G, 128}, &c->re_pw},                  {"ref_enc.proj.bias", {G}, &c->re_pb},
+        {"ref_enc.layernorm.weight", {S}, &c->re_lng},                 {"ref_enc.layernorm.bias", {S}, &c->re_lnb}};
+    for (const auto& e : re) {
+      const HostTensor* t;
+      TRY(tensor(c, e.key, e.shape, &t));
+      *e.off = append(c->h_w, t->data);
     }
-    c->re_wih = put(wih->data); c->re_whh = put(whh->data); c->re_bih = put(bih->data); c->re_bhh = put(bhh->data);
-    c->re_pw = put(rpw->data); c->re_pb = put(rpb->data); c->re_lng = put(lng->data); c->re_lnb = put(lnb->data);
     c->has_refenc = true;
   }
   // ---- V1 TTS front half (optional: base-speaker checkpoints only, models.py:451-465)
   c->tts = TtsLayers();
-  if (find(c, "enc_p.emb.weight")) {
-    const int rc = pack_tts(c);
-    if (rc != OVC_OK) return rc;
-  }
-#undef NEED
-#undef WEFF
+  if (find(c, "enc_p.emb.weight")) TRY(pack_tts(c));
   // ---- upload
   ON_DEVICE(c);
   if (c->d_w) { cudaFree(c->d_w); c->d_w = nullptr; }
@@ -736,12 +717,6 @@ static WsLayout ws_layout(const ovc_ctx* c, int B, int Tmax) {
   L.total = o;
   return L;
 }
-
-#define TRY(expr)                   \
-  do {                              \
-    int rc_ = (expr);               \
-    if (rc_ != OVC_OK) return rc_;  \
-  } while (0)
 
 struct Run {
   ovc_ctx* c;
