@@ -25,8 +25,8 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 3   /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
-                               * activation TMA, tune bits) removed */
+#define OVC_ABI_VERSION 4   /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+                               * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -141,6 +141,18 @@ OVC_API int ovc_convert_waveform(ovc_ctx* ctx, const float* wav, const int64_t* 
  *   spec  [N, spec_channels, T] magnitude spectrogram as written by ovc_spectrogram (all N items T frames)
  *   out   [N, gin]                                                                                          */
 OVC_API int ovc_reference_encoder(ovc_ctx* ctx, const float* spec, int N, int T, float* out, void* stream);
+
+/* ovc_reference_encoder on a ragged batch, as extract_se needs for reference clips of different lengths.
+ *   spec     [N, spec_channels, Tmax]; item n's frames past lengths[n] are padding and are never read (NaN is fine)
+ *   lengths  [N] int64 (device): frames per item, 1 <= len <= Tmax; every item is encoded at its own length,
+ *            so row n equals ovc_reference_encoder on spec[n, :, :lengths[n]] alone, bit for bit.  A value outside
+ *            [1, Tmax] is clamped into it on the device (never an out-of-bounds read); the ovc_spectrogram `frames`
+ *            output can be passed as is.
+ *   out      [N, gin]
+ * Padding to a common length and calling ovc_reference_encoder is NOT equivalent: the reference's ReferenceEncoder
+ * ignores its mask, so its stride-2 convs and GRU read the padded frames. */
+OVC_API int ovc_reference_encoder_ragged(ovc_ctx* ctx, const float* spec, const int64_t* lengths,
+                                         int N, int Tmax, float* out, void* stream);
 
 /* ---- V1 base-speaker TTS front half: SynthesizerTrn.infer (openvoice/models.py:467-490), SURVEY.md section 8 row f3 ----
  * Available when the checkpoint passed through ovc_load_tensor holds enc_p.* / dp.* / sdp.* / emb_g.* (a V1 base

@@ -13,13 +13,14 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
     "ovc_profile_enable", "ovc_profile_read", "ovc_profile_detail", "ovc_debug_enable", "ovc_debug_fetch",
     "ovc_spectrogram", "ovc_convert_waveform", "ovc_set_precision", "ovc_reference_encoder",
     "ovc_tts_info", "ovc_tts_encode", "ovc_tts_decode", "ovc_set_option", "ovc_graph_replays",
+    "ovc_reference_encoder_ragged",
 )
 
 
@@ -75,6 +76,8 @@ def load_library(path: Optional[str] = None):
     lib.ovc_set_precision.argtypes = [C.c_void_p, C.c_int]
     lib.ovc_set_option.argtypes = [C.c_void_p, C.c_int, C.c_int]
     lib.ovc_reference_encoder.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib.ovc_reference_encoder_ragged.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                                 C.c_void_p]
     lib.ovc_profile_enable.argtypes = [C.c_void_p, C.c_int]
     lib.ovc_profile_read.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64),
                                      C.POINTER(C.c_double), C.POINTER(C.c_double)]
@@ -278,19 +281,30 @@ class NativeConverter:
         _check(self.lib, rc, "ovc_convert_waveform")
         return o, frames
 
-    def reference_encoder(self, spec, stream=None):
+    def reference_encoder(self, spec, lengths=None, stream=None):
         """spec [N, S, T] f32 cuda (ovc_spectrogram layout) -> tone-colour embedding [N, gin]
-        (ReferenceEncoder.forward, openvoice/models.py:339-359)."""
+        (ReferenceEncoder.forward, openvoice/models.py:339-359).  ``lengths`` ([N] int64 cuda, frames, or None): every
+        item is encoded at its own length and row n equals a call on ``spec[n:n+1, :, :lengths[n]]`` bit for bit; the
+        frames past it are never read.  The ``frames`` output of ``spectrogram`` can be passed as is (no host sync)."""
         import torch
         assert spec.is_cuda and spec.dtype == torch.float32 and spec.is_contiguous() and spec.dim() == 3
         N, S, T = spec.shape
         if S != self.hp.spec_channels:
             raise ValueError(f"reference_encoder: spec has {S} channels, the model has spec_channels {self.hp.spec_channels}")
+        if lengths is not None:
+            assert lengths.is_cuda and lengths.dtype == torch.int64 and lengths.is_contiguous()
+            if tuple(lengths.shape) != (N,):
+                raise ValueError(f"reference_encoder: lengths has shape {tuple(lengths.shape)}, expected ({N},)")
         out = torch.empty(N, self.hp.gin_channels, device=spec.device, dtype=torch.float32)
         st = stream if stream is not None else torch.cuda.current_stream(spec.device)
-        rc = self.lib.ovc_reference_encoder(self.handle, C.c_void_p(spec.data_ptr()), N, T, C.c_void_p(out.data_ptr()),
-                                            C.c_void_p(st.cuda_stream))
-        _check(self.lib, rc, "ovc_reference_encoder")
+        if lengths is None:
+            rc = self.lib.ovc_reference_encoder(self.handle, C.c_void_p(spec.data_ptr()), N, T, C.c_void_p(out.data_ptr()),
+                                                C.c_void_p(st.cuda_stream))
+            _check(self.lib, rc, "ovc_reference_encoder")
+        else:
+            rc = self.lib.ovc_reference_encoder_ragged(self.handle, C.c_void_p(spec.data_ptr()), C.c_void_p(lengths.data_ptr()),
+                                                       N, T, C.c_void_p(out.data_ptr()), C.c_void_p(st.cuda_stream))
+            _check(self.lib, rc, "ovc_reference_encoder_ragged")
         return out
 
     # ---- V1 TTS front half (SynthesizerTrn.infer, openvoice/models.py:467-490) ----------------

@@ -68,6 +68,28 @@ def _write_audio(path: str, audio: np.ndarray, sr: int) -> None:
         wavfile.write(path, sr, audio.astype(np.float32))
 
 
+# Padded-frame budget of one batched reference-encoder pass in extract_se / extract_se_batch.  The encoder's device
+# workspace (ovc_reference_encoder) is two copies of its largest activation -- conv layer 1: 32 channels x ceil(T/2)
+# rows x 257 columns, ~4.1 k floats per padded input frame -- plus the GRU inputs (384 floats per 64 frames):
+# 32 768 padded frames (~6 min of audio at 22.05 kHz, hop 256) take 2 * 4112 * 32768 * 4 B ~= 1.1 GB, which the
+# context keeps for reuse.  A pass of that size already gives its first conv ~1.3e8 output threads.
+SE_CHUNK_FRAMES = 32768
+
+
+def plan_se_chunks(frames: Sequence[int], budget: int = SE_CHUNK_FRAMES) -> List[List[int]]:
+    """Group clips of ``frames[i]`` spectrogram frames into batches of one reference-encoder pass each.  Clips are
+    taken longest first; a chunk is closed when one more clip would take (clips x longest) over ``budget`` padded
+    frames, so a clip longer than the budget runs alone.  Returns lists of clip indices covering every clip once."""
+    order = sorted(range(len(frames)), key=lambda i: -int(frames[i]))
+    chunks: List[List[int]] = []
+    for i in order:
+        if chunks and (len(chunks[-1]) + 1) * int(frames[chunks[-1][0]]) <= budget:
+            chunks[-1].append(i)
+        else:
+            chunks.append([i])
+    return chunks
+
+
 _POOL = None
 
 
@@ -359,24 +381,84 @@ class ToneColorConverter(OpenVoiceBaseClass):
 
     # ------------------------------------------------------------------ speaker embedding
     def extract_se(self, ref_wav_list, se_save_path=None):
-        """openvoice/api.py:114-139: mean ReferenceEncoder embedding over the given clips,
-        shape [1, gin, 1]."""
+        """openvoice/api.py:114-139: mean ReferenceEncoder embedding over the given clips, shape [1, gin, 1].
+
+        Every clip is encoded at its own length, exactly as the reference's per-clip loop does, but the clips share
+        batched ("ragged") passes: sorted by length and grouped under ``SE_CHUNK_FRAMES`` padded frames, one upload,
+        one ``ovc_spectrogram`` and one ``ovc_reference_encoder_ragged`` per group.  A clip's frames past its own
+        length are never read, so its embedding does not depend on which clips it is grouped with: the result is
+        bit-identical to encoding the clips one at a time.  The mean is taken over the clips in the caller's order.
+        A clip shorter than one hop, or not longer than the STFT reflect padding (384 samples), raises ValueError
+        naming it before anything is launched."""
         if isinstance(ref_wav_list, (str, np.ndarray)):
             ref_wav_list = [ref_wav_list]
-        hps = self.hps
-        gs = []
-        for fname in ref_wav_list:
-            audio_ref = _load_audio(fname, hps.data.sampling_rate)
-            y = torch.from_numpy(audio_ref).to(self.device).unsqueeze(0).contiguous()
-            n = torch.tensor([y.shape[1]], dtype=torch.int64, device=self.device)
-            y, _ = self.model.native.spectrogram(y, n)          # = spectrogram_torch (api.py:126-128)
-            g = self.model.native.reference_encoder(y).unsqueeze(-1)   # = model.ref_enc(y.transpose(1, 2)) (api.py:130)
-            gs.append(g.detach())
-        gs = torch.stack(gs).mean(0)
-        if se_save_path is not None:
-            os.makedirs(os.path.dirname(se_save_path), exist_ok=True)
-            torch.save(gs.cpu(), se_save_path)
+        waves = [_load_audio(f, self.hps.data.sampling_rate) for f in ref_wav_list]
+        gs = torch.stack(self._se_rows(waves)).mean(0)
+        self._save_se(gs, se_save_path)
         return gs
+
+    def extract_se_batch(self, speakers, se_save_paths=None) -> List[torch.Tensor]:
+        """Enrol many voices at once: ``speakers`` is a sequence whose items are each a list of reference clips or a
+        single clip (path or waveform).  Returns one [1, gin, 1] embedding per speaker, each bit-identical to
+        ``extract_se(speakers[i])``; the clips of all speakers share the same batched passes (see ``extract_se``).
+        ``se_save_paths``: one path (or None) per speaker, written like ``extract_se``'s ``se_save_path``."""
+        groups = [[s] if isinstance(s, (str, np.ndarray)) else list(s) for s in speakers]
+        if se_save_paths is not None and len(se_save_paths) != len(groups):
+            raise ValueError(f"{len(se_save_paths)} save paths for {len(groups)} speakers")
+        for i, g in enumerate(groups):
+            if not g:
+                raise ValueError(f"speaker {i} has no reference clips")
+        sr = self.hps.data.sampling_rate
+        rows = self._se_rows([_load_audio(f, sr) for g in groups for f in g])
+        out, k = [], 0
+        for i, g in enumerate(groups):
+            se = torch.stack(rows[k: k + len(g)]).mean(0)
+            k += len(g)
+            self._save_se(se, None if se_save_paths is None else se_save_paths[i])
+            out.append(se)
+        return out
+
+    @staticmethod
+    def _save_se(se, path):
+        if path is not None:
+            if os.path.dirname(path):
+                os.makedirs(os.path.dirname(path), exist_ok=True)
+            torch.save(se.cpu(), path)
+
+    @torch.no_grad()
+    def _se_rows(self, waves) -> List[torch.Tensor]:
+        """ReferenceEncoder embedding [1, gin, 1] of every waveform, in order; see ``extract_se``."""
+        hop = self.hps.data.hop_length
+        pad = (self.hps.data.filter_length - hop) // 2
+        for i, w in enumerate(waves):          # what _enqueue_chunk refuses, checked before any launch
+            if len(w) < hop or len(w) <= pad:
+                raise ValueError(f"reference clip {i} has {len(w)} samples: needs at least one hop ({hop}) and more "
+                                 f"than the STFT reflect padding ({pad})")
+        dev, nat = self.device, self.model.native
+        rows: List[Optional[torch.Tensor]] = [None] * len(waves)
+        for idx in plan_se_chunks([len(w) // hop for w in waves], SE_CHUNK_FRAMES):
+            k, Lmax = len(idx), max(len(waves[i]) for i in idx)
+            ev = self.__dict__.get("_se_h2d_done")
+            if ev is not None:
+                ev.synchronize()               # the previous chunk's upload has left the staging buffer
+            stage = self._pinned("se_in", k * Lmax).view(k, Lmax)
+            stage_np = stage.numpy()
+
+            def put(b):
+                w = waves[idx[b]]
+                stage_np[b, : len(w)] = w
+                stage_np[b, len(w):] = 0.0
+            _parallel(put, k)
+            wav = stage.to(dev, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(dev))
+            self._se_h2d_done = ev
+            wlen = torch.tensor([len(waves[i]) for i in idx], dtype=torch.int64).to(dev)
+            spec, frames = nat.spectrogram(wav, wlen)                     # = spectrogram_torch (api.py:126-128)
+            g = nat.reference_encoder(spec, frames)                        # = model.ref_enc per clip (api.py:130)
+            for j, i in enumerate(idx):
+                rows[i] = g[j: j + 1].unsqueeze(-1)
+        return rows  # type: ignore[return-value]
 
     # ------------------------------------------------------------------ conversion
     def convert(self, audio_src_path, src_se, tgt_se, output_path=None, tau=0.3, message="default",

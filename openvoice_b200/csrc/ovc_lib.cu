@@ -1528,7 +1528,8 @@ int ovc_convert_waveform(ovc_ctx* c, const float* wav, const int64_t* wav_length
   });
 }
 
-int ovc_reference_encoder(ovc_ctx* c, const float* spec, int N, int T, float* out, void* stream) {
+// ovc_reference_encoder (lengths == nullptr: every item T frames) and ovc_reference_encoder_ragged
+static int run_refenc(ovc_ctx* c, const float* spec, const long long* lengths, int N, int T, float* out, void* stream) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
   if (!c->has_refenc) return fail(OVC_ERR_MISSING, "the checkpoint had no ref_enc.* tensors");
@@ -1560,26 +1561,39 @@ int ovc_reference_encoder(ovc_ctx* c, const float* spec, int N, int T, float* ou
   float* gi = a1 + round_up(maxact, 64);
   {
     const int warps = N * T;
-    refenc_layernorm_kernel<<<(warps * 32 + 255) / 256, 256, 0, st>>>(spec, c->d_w + c->re_lng, c->d_w + c->re_lnb, a0, N, F, T);
+    refenc_layernorm_kernel<<<(warps * 32 + 255) / 256, 256, 0, st>>>(spec, c->d_w + c->re_lng, c->d_w + c->re_lnb, a0, N, F, T,
+                                                                      (const int64_t*)lengths);
     CK(cudaGetLastError());
   }
   float* cur = a0; float* nxt = a1;
   for (int i = 0; i < 6; ++i) {
     const long long total = (long long)N * filt[i + 1] * H[i + 1] * W[i + 1];
     refenc_conv_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(cur, c->d_w + c->re_conv_w[i], c->d_w + c->re_conv_b[i], nxt, N,
-                                                                        filt[i], H[i], W[i], filt[i + 1], H[i + 1], W[i + 1]);
+                                                                        filt[i], H[i], W[i], filt[i + 1], H[i + 1], W[i + 1],
+                                                                        (const int64_t*)lengths, T, i);
     CK(cudaGetLastError());
     std::swap(cur, nxt);
   }
   {
     const long long warps = (long long)N * H[6] * 384;
     refenc_gru_in_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(cur, c->d_w + c->re_wih, c->d_w + c->re_bih, gi, N, 128,
-                                                                              H[6], W[6], 384);
+                                                                              H[6], W[6], 384, (const int64_t*)lengths, T);
     CK(cudaGetLastError());
-    refenc_gru_kernel<<<N, 128, 0, st>>>(gi, c->d_w + c->re_whh, c->d_w + c->re_bhh, c->d_w + c->re_pw, c->d_w + c->re_pb, out, H[6], G);
+    refenc_gru_kernel<<<N, 128, 0, st>>>(gi, c->d_w + c->re_whh, c->d_w + c->re_bhh, c->d_w + c->re_pw, c->d_w + c->re_pb, out, H[6], G,
+                                         (const int64_t*)lengths, T);
     CK(cudaGetLastError());
   }
   return OVC_OK;
+}
+
+int ovc_reference_encoder(ovc_ctx* c, const float* spec, int N, int T, float* out, void* stream) {
+  return run_refenc(c, spec, nullptr, N, T, out, stream);
+}
+
+int ovc_reference_encoder_ragged(ovc_ctx* c, const float* spec, const int64_t* lengths, int N, int Tmax, float* out,
+                                 void* stream) {
+  if (!lengths) return fail(OVC_ERR_INVALID, "null lengths in ovc_reference_encoder_ragged");
+  return run_refenc(c, spec, (const long long*)lengths, N, Tmax, out, stream);
 }
 
 int ovc_tts_info(const ovc_ctx* c, int32_t* out8) {
