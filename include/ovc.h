@@ -25,8 +25,9 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 4   /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
-                               * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged */
+#define OVC_ABI_VERSION 5   /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+                               * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
+                               * 5: ovc_resample, ovc_resample_span */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -153,6 +154,29 @@ OVC_API int ovc_reference_encoder(ovc_ctx* ctx, const float* spec, int N, int T,
  * ignores its mask, so its stride-2 convs and GRU read the padded frames. */
 OVC_API int ovc_reference_encoder_ragged(ovc_ctx* ctx, const float* spec, const int64_t* lengths,
                                          int N, int Tmax, float* out, void* stream);
+
+/* Sample-rate conversion on the device, for waveforms that do not arrive at the model's rate (the reference resamples
+ * every input on the host: librosa.load(path, sr=hps.data.sampling_rate), openvoice/api.py:123,144).  The arithmetic is
+ * scipy.signal.resample_poly(x, up, down) at its defaults (Kaiser beta 5 window, 20 max(up, down) + 1 taps, constant
+ * padding), up / down = sr_out / sr_in reduced; fp64 taps and accumulation, one rounding to fp32 -- within one ulp of
+ * float32(resample_poly(float64(x))).  A rate that is not positive, or a reduced max(up, down) above 2048, is
+ * OVC_ERR_INVALID (every common rate from 8 kHz to 192 kHz is accepted).  The context builds each pair's filter bank on
+ * first use and keeps it: that first call uploads the bank on `stream` and waits for the stream to finish the copy.
+ *   in          [B, in_pitch] fp32 (device): row b holds input samples [in_start, in_start + in_pitch) of item b
+ *   in_lengths  [B] int64 (device): samples of item b's whole input; INT64_MAX = a stream that has not ended.  Samples
+ *               outside [0, len) and outside the row read as 0
+ *   out         [B, out_pitch] fp32 (device): row b receives y_b[out_start, out_start + out_pitch); outputs at or past
+ *               n_out(len) = ceil(len * up / down) are written as 0
+ * A whole-clip call has in_start = out_start = 0.  A windowed call gives the whole-clip samples bit for bit when its
+ * rows hold every input sample the requested outputs read: ovc_resample_span says which.  Only enqueues on `stream`. */
+OVC_API int ovc_resample(ovc_ctx* ctx, int sr_in, int sr_out, const float* in, const int64_t* in_lengths, int B,
+                         int64_t in_pitch, int64_t in_start, float* out, int64_t out_pitch, int64_t out_start, void* stream);
+
+/* Host-side geometry of ovc_resample for sr_in -> sr_out (no context, no device):
+ *   out4[0] = n_out(n_in), output samples of a clip of n_in input samples
+ *   out4[1] = outputs whose input support lies inside the first n_in samples (what a stream can emit before it ends)
+ *   out4[2], out4[3] = input samples [lo, hi) read by outputs [m0, m1) (m1 > m0; lo may be negative) */
+OVC_API int ovc_resample_span(int sr_in, int sr_out, int64_t n_in, int64_t m0, int64_t m1, int64_t* out4);
 
 /* ---- V1 base-speaker TTS front half: SynthesizerTrn.infer (openvoice/models.py:467-490), SURVEY.md section 8 row f3 ----
  * Available when the checkpoint passed through ovc_load_tensor holds enc_p.* / dp.* / sdp.* / emb_g.* (a V1 base

@@ -13,15 +13,17 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
     "ovc_profile_enable", "ovc_profile_read", "ovc_profile_detail", "ovc_debug_enable", "ovc_debug_fetch",
     "ovc_spectrogram", "ovc_convert_waveform", "ovc_set_precision", "ovc_reference_encoder",
     "ovc_tts_info", "ovc_tts_encode", "ovc_tts_decode", "ovc_set_option", "ovc_graph_replays",
-    "ovc_reference_encoder_ragged",
+    "ovc_reference_encoder_ragged", "ovc_resample", "ovc_resample_span",
 )
+
+STREAM_OPEN = 2 ** 63 - 1   # ovc_resample input length of a stream that has not ended
 
 
 class OvcHParams(C.Structure):
@@ -94,6 +96,9 @@ def load_library(path: Optional[str] = None):
                                    C.c_float, C.c_float, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.ovc_tts_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_float, C.c_int, C.c_int, C.c_int, C.c_int,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.ovc_resample.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64,
+                                 C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
+    lib.ovc_resample_span.argtypes = [C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.POINTER(C.c_int64)]
     if lib.ovc_abi_version() != ABI_VERSION:
         raise OvcError(f"ABI mismatch: library {lib.ovc_abi_version()} vs binding {ABI_VERSION}")
     _lib = lib
@@ -143,6 +148,16 @@ def hparams_struct(hps) -> OvcHParams:
     s.zero_g = 1 if get(model, "zero_g", False) else 0
     s.hop_length = int(get(data, "hop_length"))
     return s
+
+
+def resample_span(sr_in: int, sr_out: int, n_in: int = 0, m0: int = 0, m1: int = 1) -> Tuple[int, int, int, int]:
+    """Geometry of ``NativeConverter.resample`` (include/ovc.h: ovc_resample_span), computed on the host:
+    (n_out(n_in), outputs a stream of n_in samples can emit, and the input samples [lo, hi) outputs [m0, m1) read).
+    Raises ValueError naming both rates for a pair the resampler refuses."""
+    lib = load_library()
+    out = (C.c_int64 * 4)()
+    _check(lib, lib.ovc_resample_span(int(sr_in), int(sr_out), int(n_in), int(m0), int(m1), out), "ovc_resample_span")
+    return int(out[0]), int(out[1]), int(out[2]), int(out[3])
 
 
 class NativeConverter:
@@ -305,6 +320,34 @@ class NativeConverter:
             rc = self.lib.ovc_reference_encoder_ragged(self.handle, C.c_void_p(spec.data_ptr()), C.c_void_p(lengths.data_ptr()),
                                                        N, T, C.c_void_p(out.data_ptr()), C.c_void_p(st.cuda_stream))
             _check(self.lib, rc, "ovc_reference_encoder_ragged")
+        return out
+
+    def resample(self, x, in_lengths, sr_in: int, sr_out: int, out=None, out_pitch: Optional[int] = None,
+                 in_start: int = 0, out_start: int = 0, stream=None):
+        """Polyphase resampling on the device (scipy.signal.resample_poly arithmetic, include/ovc.h: ovc_resample).
+        x [B, in_pitch] f32 cuda: row b holds samples [in_start, in_start + in_pitch) of item b; in_lengths [B] int64
+        cuda: each item's whole input length (STREAM_OPEN: not ended).  Returns out [B, out_pitch] with
+        y_b[out_start, out_start + out_pitch), zero past each item's n_out; out_pitch defaults to
+        n_out(in_start + in_pitch) - out_start, computed on the host.  Asynchronous on `stream`."""
+        import torch
+        assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 2
+        assert in_lengths.is_cuda and in_lengths.dtype == torch.int64 and in_lengths.is_contiguous()
+        B, pitch = x.shape
+        if tuple(in_lengths.shape) != (B,):
+            raise ValueError(f"resample: in_lengths has shape {tuple(in_lengths.shape)}, expected ({B},)")
+        if out_pitch is None:
+            out_pitch = (out.shape[1] if out is not None else
+                         max(0, resample_span(sr_in, sr_out, in_start + pitch)[0] - out_start))
+        if out is None:
+            out = torch.empty(B, out_pitch, device=x.device, dtype=torch.float32)
+        assert out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (B, out_pitch)
+        if out_pitch == 0:
+            return out
+        st = stream if stream is not None else torch.cuda.current_stream(x.device)
+        rc = self.lib.ovc_resample(self.handle, int(sr_in), int(sr_out), C.c_void_p(x.data_ptr()),
+                                   C.c_void_p(in_lengths.data_ptr()), B, pitch, int(in_start), C.c_void_p(out.data_ptr()),
+                                   int(out_pitch), int(out_start), C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_resample")
         return out
 
     # ---- V1 TTS front half (SynthesizerTrn.infer, openvoice/models.py:467-490) ----------------

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from . import utils
-from ._native import NativeConverter
+from ._native import NativeConverter, resample_span
 from .ref_enc import ReferenceEncoder
 from .schema import hot_path_keys, ref_enc_keys, tts_keys
 
@@ -380,7 +380,7 @@ class ToneColorConverter(OpenVoiceBaseClass):
         self.version = getattr(self.hps, "_version_", "v1")
 
     # ------------------------------------------------------------------ speaker embedding
-    def extract_se(self, ref_wav_list, se_save_path=None):
+    def extract_se(self, ref_wav_list, se_save_path=None, sr: Optional[int] = None):
         """openvoice/api.py:114-139: mean ReferenceEncoder embedding over the given clips, shape [1, gin, 1].
 
         Every clip is encoded at its own length, exactly as the reference's per-clip loop does, but the clips share
@@ -389,27 +389,31 @@ class ToneColorConverter(OpenVoiceBaseClass):
         length are never read, so its embedding does not depend on which clips it is grouped with: the result is
         bit-identical to encoding the clips one at a time.  The mean is taken over the clips in the caller's order.
         A clip shorter than one hop, or not longer than the STFT reflect padding (384 samples), raises ValueError
-        naming it before anything is launched."""
+        naming it before anything is launched.  ``sr``: rate of NumPy waveform clips when it is not the model's; they
+        are resampled on the device (see ``convert_batch``) and the length checks apply to the resampled clips."""
         if isinstance(ref_wav_list, (str, np.ndarray)):
             ref_wav_list = [ref_wav_list]
+        rate = self._input_rate(ref_wav_list, sr)
         waves = [_load_audio(f, self.hps.data.sampling_rate) for f in ref_wav_list]
-        gs = torch.stack(self._se_rows(waves)).mean(0)
+        gs = torch.stack(self._se_rows(waves, rate)).mean(0)
         self._save_se(gs, se_save_path)
         return gs
 
-    def extract_se_batch(self, speakers, se_save_paths=None) -> List[torch.Tensor]:
+    def extract_se_batch(self, speakers, se_save_paths=None, sr: Optional[int] = None) -> List[torch.Tensor]:
         """Enrol many voices at once: ``speakers`` is a sequence whose items are each a list of reference clips or a
         single clip (path or waveform).  Returns one [1, gin, 1] embedding per speaker, each bit-identical to
         ``extract_se(speakers[i])``; the clips of all speakers share the same batched passes (see ``extract_se``).
-        ``se_save_paths``: one path (or None) per speaker, written like ``extract_se``'s ``se_save_path``."""
+        ``se_save_paths``: one path (or None) per speaker, written like ``extract_se``'s ``se_save_path``; ``sr`` as in
+        ``extract_se``."""
         groups = [[s] if isinstance(s, (str, np.ndarray)) else list(s) for s in speakers]
         if se_save_paths is not None and len(se_save_paths) != len(groups):
             raise ValueError(f"{len(se_save_paths)} save paths for {len(groups)} speakers")
         for i, g in enumerate(groups):
             if not g:
                 raise ValueError(f"speaker {i} has no reference clips")
-        sr = self.hps.data.sampling_rate
-        rows = self._se_rows([_load_audio(f, sr) for g in groups for f in g])
+        clips = [f for g in groups for f in g]
+        rate = self._input_rate(clips, sr)
+        rows = self._se_rows([_load_audio(f, self.hps.data.sampling_rate) for f in clips], rate)
         out, k = [], 0
         for i, g in enumerate(groups):
             se = torch.stack(rows[k: k + len(g)]).mean(0)
@@ -426,17 +430,20 @@ class ToneColorConverter(OpenVoiceBaseClass):
             torch.save(se.cpu(), path)
 
     @torch.no_grad()
-    def _se_rows(self, waves) -> List[torch.Tensor]:
-        """ReferenceEncoder embedding [1, gin, 1] of every waveform, in order; see ``extract_se``."""
+    def _se_rows(self, waves, sr: Optional[int] = None) -> List[torch.Tensor]:
+        """ReferenceEncoder embedding [1, gin, 1] of every waveform, in order; see ``extract_se``.  ``sr``: the
+        waveforms' rate when it is not the model's (``_input_rate``): each group is uploaded raw and resampled on the
+        device."""
         hop = self.hps.data.hop_length
         pad = (self.hps.data.filter_length - hop) // 2
-        for i, w in enumerate(waves):          # what _enqueue_chunk refuses, checked before any launch
-            if len(w) < hop or len(w) <= pad:
-                raise ValueError(f"reference clip {i} has {len(w)} samples: needs at least one hop ({hop}) and more "
-                                 f"than the STFT reflect padding ({pad})")
+        lens = [self._resampled_len(len(w), sr) for w in waves]
+        for i, n in enumerate(lens):           # what _enqueue_chunk refuses, checked before any launch
+            if n < hop or n <= pad:
+                raise ValueError(f"reference clip {i} has {n} samples{'' if sr is None else ' after resampling'}: needs "
+                                 f"at least one hop ({hop}) and more than the STFT reflect padding ({pad})")
         dev, nat = self.device, self.model.native
         rows: List[Optional[torch.Tensor]] = [None] * len(waves)
-        for idx in plan_se_chunks([len(w) // hop for w in waves], SE_CHUNK_FRAMES):
+        for idx in plan_se_chunks([n // hop for n in lens], SE_CHUNK_FRAMES):
             k, Lmax = len(idx), max(len(waves[i]) for i in idx)
             ev = self.__dict__.get("_se_h2d_done")
             if ev is not None:
@@ -454,6 +461,9 @@ class ToneColorConverter(OpenVoiceBaseClass):
             ev.record(torch.cuda.current_stream(dev))
             self._se_h2d_done = ev
             wlen = torch.tensor([len(waves[i]) for i in idx], dtype=torch.int64).to(dev)
+            if sr is not None:
+                wav = nat.resample(wav, wlen, sr, self.hps.data.sampling_rate, out_pitch=max(lens[i] for i in idx))
+                wlen = torch.tensor([lens[i] for i in idx], dtype=torch.int64).to(dev)
             spec, frames = nat.spectrogram(wav, wlen)                     # = spectrogram_torch (api.py:126-128)
             g = nat.reference_encoder(spec, frames)                        # = model.ref_enc per clip (api.py:130)
             for j, i in enumerate(idx):
@@ -462,11 +472,12 @@ class ToneColorConverter(OpenVoiceBaseClass):
 
     # ------------------------------------------------------------------ conversion
     def convert(self, audio_src_path, src_se, tgt_se, output_path=None, tau=0.3, message="default",
-                noise=None):
+                noise=None, sr: Optional[int] = None):
         """openvoice/api.py:141-160.  Returns float32 samples (256 * (L // 256) of them) or writes
-        ``output_path``.  ``noise`` ([1,192,T]) optionally replaces the random draw (tests)."""
+        ``output_path``.  ``noise`` ([1,192,T]) optionally replaces the random draw (tests).  ``sr``: rate of a NumPy
+        waveform that is not at the model's rate (see ``convert_batch``)."""
         audio = self.convert_batch([audio_src_path], src_se, tgt_se, tau=tau, messages=[message],
-                                   noise=None if noise is None else [noise])[0]
+                                   noise=None if noise is None else [noise], sr=sr)[0]
         if output_path is None:
             return audio
         _write_audio(output_path, audio, self.hps.data.sampling_rate)
@@ -474,12 +485,18 @@ class ToneColorConverter(OpenVoiceBaseClass):
     @torch.no_grad()
     def convert_batch(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: float = 0.3,
                       messages: Optional[Sequence[str]] = None, noise: Optional[Sequence] = None,
-                      max_batch: int = 64) -> List[np.ndarray]:
+                      max_batch: int = 64, sr: Optional[int] = None) -> List[np.ndarray]:
         """Convert a list of utterances (paths or waveforms at the model sampling rate); every item
         gets exactly what ``convert`` would return for it alone.  ``src_se`` / ``tgt_se`` are either
-        one [1,gin,1] embedding for all items or a sequence of per-item embeddings."""
+        one [1,gin,1] embedding for all items or a sequence of per-item embeddings.
+
+        ``sr``: sampling rate of the NumPy waveform items when it is not the model's.  They are uploaded as they are
+        and resampled on the device (``scipy.signal.resample_poly`` arithmetic, within one fp32 ulp of it) into the
+        buffer the spectrogram reads; the output stays at the model's rate, as in the reference.  A file path item with
+        ``sr`` is refused (files are decoded and resampled on load); so is a rate pair the resampler does not take."""
         hps = self.hps
         n = len(audios)
+        rate = self._input_rate(audios, sr)
         waves = [_load_audio(a, hps.data.sampling_rate) for a in audios]
         src = self._stack_se(src_se, n)
         tgt = self._stack_se(tgt_se, n)
@@ -489,7 +506,7 @@ class ToneColorConverter(OpenVoiceBaseClass):
         for lo in range(0, n, max_batch):
             idx = order[lo: lo + max_batch]
             res = self._convert_chunk([waves[i] for i in idx], src[idx], tgt[idx], tau,
-                                      None if noise is None else [noise[i] for i in idx])
+                                      None if noise is None else [noise[i] for i in idx], rate)
             for i, a in zip(idx, res):
                 msg = messages[i] if messages is not None else "default"
                 out[i] = self.add_watermark(a, msg)
@@ -498,12 +515,14 @@ class ToneColorConverter(OpenVoiceBaseClass):
     # ------------------------------------------------------------------ one utterance per stream
     @torch.no_grad()
     def convert_concurrent(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: float = 0.3, streams: int = 4,
-                           messages: Optional[Sequence[str]] = None) -> List[np.ndarray]:
+                           messages: Optional[Sequence[str]] = None, sr: Optional[int] = None) -> List[np.ndarray]:
         """Serve many SMALL independent requests: utterance i runs alone (batch 1, exactly ``convert``) on CUDA
         stream ``i % streams``, each stream with its own converter replica (context + workspace), so the
         latency-bound kernels of different requests overlap on the GPU -- north_star's "one utterance per stream".
-        For large batches ``convert_batch`` (one launch sequence for the whole batch) is the faster path."""
+        For large batches ``convert_batch`` (one launch sequence for the whole batch) is the faster path.  ``sr`` as in
+        ``convert_batch``."""
         n = len(audios)
+        rate = self._input_rate(audios, sr)
         src = self._stack_se(src_se, n)
         tgt = self._stack_se(tgt_se, n)
         reps = self._replicas(max(1, min(streams, n)))
@@ -516,7 +535,7 @@ class ToneColorConverter(OpenVoiceBaseClass):
                 conv, stream = reps[j % S]
                 with torch.cuda.stream(stream):
                     pending.append(conv._enqueue_single(_load_audio(audios[i], self.hps.data.sampling_rate), src[i: i + 1],
-                                                        tgt[i: i + 1], tau, j // S))
+                                                        tgt[i: i + 1], tau, j // S, rate))
             for _, stream in reps:
                 stream.synchronize()
             for i, (host, n_samples) in zip(wave, pending):
@@ -535,17 +554,21 @@ class ToneColorConverter(OpenVoiceBaseClass):
             reps.append((twin, torch.cuda.Stream(device=self.device)))
         return reps[:count]
 
-    def _enqueue_single(self, wave, src, tgt, tau, slot):
+    def _enqueue_single(self, wave, src, tgt, tau, slot, sr=None):
         """Asynchronous batch-1 conversion on the current stream, staging through pinned slot ``slot``;
-        returns (pinned host buffer, samples).  The caller synchronises the stream before reading / reusing it."""
+        returns (pinned host buffer, samples).  The caller synchronises the stream before reading / reusing it.
+        ``sr``: the wave's rate when it is not the model's (``_input_rate``): resampled on the device after upload."""
         hop = self.hps.data.hop_length
         dev = self.device
-        L = len(wave)
+        L = self._resampled_len(len(wave), sr)
         if L // hop < 1 or L <= (self.hps.data.filter_length - hop) // 2:
-            raise ValueError("audio too short")
-        stage = self._pinned(f"cin{slot}", L)
+            raise ValueError("audio too short" if sr is None else f"audio too short: {L} samples after resampling")
+        stage = self._pinned(f"cin{slot}", len(wave))
         stage.copy_(torch.from_numpy(wave))
-        wav = stage.to(dev, non_blocking=True).view(1, L)
+        wav = stage.to(dev, non_blocking=True).view(1, len(wave))
+        if sr is not None:
+            wav = self.model.native.resample(wav, torch.tensor([len(wave)], dtype=torch.int64, device=dev), sr,
+                                             self.hps.data.sampling_rate)
         wlen = torch.tensor([L], dtype=torch.int64, device=dev)
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())
         o, _ = self.model.native.convert_waveform(wav, wlen, src, tgt, tau=float(tau), seed=seed)
@@ -560,14 +583,19 @@ class ToneColorConverter(OpenVoiceBaseClass):
 
     @torch.no_grad()
     def convert_long(self, audio_src_path, src_se, tgt_se, output_path=None, tau=0.3, message="default",
-                     window_frames: int = 2048, noise=None, max_batch: int = 32):
+                     window_frames: int = 2048, noise=None, max_batch: int = 32, sr: Optional[int] = None):
         """Row f4 (time-tiled execution): convert a clip of any length with bounded memory.  The spectrogram is
         cut into windows of ``window_frames`` frames plus a halo of the path's receptive field on both sides; the
         windows run as one ragged batch and only their interiors are kept, so the result equals ``convert`` on the
-        whole clip (same noise tensor: drawn once for the whole clip, or passed as ``noise`` [192, T])."""
+        whole clip (same noise tensor: drawn once for the whole clip, or passed as ``noise`` [192, T]).  ``sr``: rate of
+        a NumPy waveform that is not at the model's; it is resampled on the device first (see ``convert_batch``)."""
         hps = self.hps
         hop, dev = hps.data.hop_length, self.device
+        rate = self._input_rate([audio_src_path], sr)
         wav = torch.from_numpy(_load_audio(audio_src_path, hps.data.sampling_rate)).to(dev)
+        if rate is not None:
+            wav = self.model.native.resample(wav[None].contiguous(), torch.tensor([wav.numel()], dtype=torch.int64, device=dev),
+                                             rate, hps.data.sampling_rate)[0]
         L = wav.numel()
         spec, _ = self.model.native.spectrogram(wav[None].contiguous(), torch.tensor([L], dtype=torch.int64, device=dev))
         T = spec.shape[2]
@@ -602,6 +630,25 @@ class ToneColorConverter(OpenVoiceBaseClass):
             return audio
         _write_audio(output_path, audio, hps.data.sampling_rate)
 
+    def _input_rate(self, audios, sr) -> Optional[int]:
+        """The rate to resample the NumPy waveforms of ``audios`` from, or None when they are at the model's rate
+        (``sr`` None or equal to it: the staging code is then exactly the one without resampling).  A file path is
+        decoded and resampled on load, so one combined with ``sr`` raises ValueError, as does a rate pair the device
+        resampler refuses -- both before anything is launched."""
+        model_sr = int(self.hps.data.sampling_rate)
+        if sr is None or int(sr) == model_sr:
+            return None
+        for i, a in enumerate(audios):
+            if isinstance(a, str):
+                raise ValueError(f"item {i} is a file path ({a!r}): sr= describes NumPy waveforms; files are decoded and "
+                                 f"resampled to {model_sr} Hz on load")
+        resample_span(int(sr), model_sr)
+        return int(sr)
+
+    def _resampled_len(self, n: int, sr: Optional[int]) -> int:
+        """Samples at the model's rate of ``n`` samples at ``sr`` (None: already at the model's rate)."""
+        return n if sr is None else resample_span(sr, self.hps.data.sampling_rate, n)[0]
+
     def _stack_se(self, se, n):
         if isinstance(se, (list, tuple)):
             se = torch.cat([s.reshape(1, -1) for s in se], 0)
@@ -611,43 +658,56 @@ class ToneColorConverter(OpenVoiceBaseClass):
         assert se.shape[0] == n, "one speaker embedding per utterance (or a single one for all)"
         return se
 
-    def _enqueue_chunk(self, waves, src, tgt, tau, noise, slot=0):
+    def _enqueue_chunk(self, waves, src, tgt, tau, noise, slot=0, sr=None):
         """Stage, upload and launch one ragged batch on the current stream WITHOUT synchronising the host.
-        Returns (o [B, 256 * Tmax] on the device, frames per item)."""
+        Returns (o [B, 256 * Tmax] on the device, frames per item).  ``sr``: the waves' rate when it is not the
+        model's (``_input_rate``): the raw samples are uploaded and resampled on the device into the slot's buffer."""
         hps = self.hps
         hop = hps.data.hop_length
         B = len(waves)
-        frames = [len(w) // hop for w in waves]
+        lens_in = [len(w) for w in waves]
+        lens = [self._resampled_len(n, sr) for n in lens_in]
+        after = "" if sr is None else " after resampling"
+        frames = [n // hop for n in lens]
         if min(frames) < 1:
-            raise ValueError("audio shorter than one hop")
+            raise ValueError("audio shorter than one hop" + after)
         Tmax = max(frames)
         dev = self.device
-        if min(len(w) for w in waves) <= (hps.data.filter_length - hop) // 2:
-            raise ValueError("audio shorter than the STFT reflect padding")   # torch raises here too
+        if min(lens) <= (hps.data.filter_length - hop) // 2:
+            raise ValueError("audio shorter than the STFT reflect padding" + after)   # torch raises here too
         # host -> device: one pinned staging buffer per slot (cached across calls: cudaHostAlloc is slow), one copy;
         # a slot is restaged only after its previous upload has left it
         # the padded length is rounded up to 16 hops: batches of similar length share one launch signature, so the native
         # library replays their CUDA graph; every item still runs at its own exact length (ragged), so nothing changes
-        Lmax = -(-max(len(w) for w in waves) // (16 * hop)) * (16 * hop)
+        Lmax = -(-max(lens) // (16 * hop)) * (16 * hop)
+        Lin = Lmax if sr is None else max(lens_in)       # staged samples per row
         ev = self.__dict__.setdefault("_h2d_done", {}).get(slot)
         if ev is not None:
             ev.synchronize()
-        stage = self._pinned(f"in{slot}", B * Lmax).view(B, Lmax)
+        stage = self._pinned(f"in{slot}", B * Lin).view(B, Lin)
         stage_np = stage.numpy()
-        lens = np.array([len(w) for w in waves], dtype=np.int64)
 
         def put(b):
             w = waves[b]
             stage_np[b, : len(w)] = w
-            if len(w) < Lmax:
+            if len(w) < Lin:
                 stage_np[b, len(w):] = 0.0
         _parallel(put, B)
         # device-side buffers are cached per slot too: with every address stable, a repeated (batch, length) call is
-        # replayed from a CUDA graph by the native library (include/ovc.h: OVC_OPT_GRAPH)
+        # replayed from a CUDA graph by the native library (include/ovc.h: OVC_OPT_GRAPH); the resampler writes into
+        # the same per-slot buffer the spectrogram reads
         wav = self._dev(f"wav{slot}", B * Lmax, torch.float32).view(B, Lmax)
-        wav.copy_(stage, non_blocking=True)
+        if sr is None:
+            wav.copy_(stage, non_blocking=True)
+        else:
+            raw = self._dev(f"raw{slot}", B * Lin, torch.float32).view(B, Lin)
+            raw.copy_(stage, non_blocking=True)
+            rlen_pin = self._pinned_i64(f"rlen{slot}", B)
+            rlen_pin.copy_(torch.tensor(lens_in, dtype=torch.int64))
+            rlen = self._dev(f"rlen{slot}", B, torch.int64)
+            rlen.copy_(rlen_pin, non_blocking=True)
         lens_pin = self._pinned_i64(f"len{slot}", B)
-        lens_pin.copy_(torch.from_numpy(lens))
+        lens_pin.copy_(torch.tensor(lens, dtype=torch.int64))
         wlen = self._dev(f"len{slot}", B, torch.int64)
         wlen.copy_(lens_pin, non_blocking=True)
         src_d = self._dev(f"src{slot}", src.numel(), torch.float32).view(B, -1)
@@ -657,6 +717,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(dev))
         self._h2d_done[slot] = ev
+        if sr is not None:
+            self.model.native.resample(raw, rlen, sr, hps.data.sampling_rate, out=wav)
         nz = None
         if noise is not None:
             nz = torch.zeros(B, hps.model.inter_channels, Lmax // hop, device=dev, dtype=torch.float32)
@@ -670,9 +732,9 @@ class ToneColorConverter(OpenVoiceBaseClass):
                                                   frames_out=self._dev(f"fr{slot}", B, torch.int64))
         return o.view(B, -1), frames
 
-    def _convert_chunk(self, waves, src, tgt, tau, noise):
+    def _convert_chunk(self, waves, src, tgt, tau, noise, sr=None):
         hop = self.hps.data.hop_length
-        o, frames = self._enqueue_chunk(waves, src, tgt, tau, noise)
+        o, frames = self._enqueue_chunk(waves, src, tgt, tau, noise, sr=sr)
         host = self._pinned("out", o.numel()).view(o.shape)
         host.copy_(o, non_blocking=True)
         torch.cuda.current_stream(self.device).synchronize()
@@ -680,15 +742,17 @@ class ToneColorConverter(OpenVoiceBaseClass):
         return _parallel(lambda b: audio[b, : frames[b] * hop].copy(), len(waves))
 
     @torch.no_grad()
-    def convert_batch_device(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: float = 0.3, slot: int = 0):
+    def convert_batch_device(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: float = 0.3, slot: int = 0,
+                             sr: Optional[int] = None):
         """``convert_batch`` up to the device: stages and launches ONE ragged batch asynchronously on the current
         stream and returns (o [n, max samples] float32 on the device, samples per item).  No host synchronisation,
         no device -> host copy: the building block of ``distributed.convert_sharded_async`` (waveforms gathered
         GPU-to-GPU over NCCL) and of pipelined serving.  ``slot`` picks the pinned upload buffer (alternate 0 / 1
-        between in-flight calls)."""
+        between in-flight calls).  ``sr`` as in ``convert_batch``."""
+        rate = self._input_rate(audios, sr)
         waves = [_load_audio(a, self.hps.data.sampling_rate) for a in audios]
         n = len(waves)
-        o, frames = self._enqueue_chunk(waves, self._stack_se(src_se, n), self._stack_se(tgt_se, n), tau, None, slot)
+        o, frames = self._enqueue_chunk(waves, self._stack_se(src_se, n), self._stack_se(tgt_se, n), tau, None, slot, rate)
         hop = self.hps.data.hop_length
         return o, [f * hop for f in frames]
 

@@ -18,6 +18,7 @@
 #include "ovc_tcconv.cuh"
 #include "ovc_tts.cuh"
 #include "ovc_refenc.cuh"
+#include "ovc_resample.cuh"
 #include "ovc_variants.h"
 
 namespace ovc {
@@ -208,6 +209,10 @@ struct ovc_ctx {
   int re_gru_in = 0;           // columns of ref_enc.gru.weight_ih_l0
   float* d_re = nullptr;
   size_t re_floats = 0;
+
+  // ovc_resample: one fp64 polyphase bank per reduced (up, down) pair, built on first use and kept
+  std::map<std::pair<int64_t, int64_t>, double*> rs_banks;
+  bool rs_smem_opt_in = false;   // resample_kernel's dynamic shared-memory limit raised (once per context)
 
   // workspace
   float* d_ws = nullptr;
@@ -1418,6 +1423,7 @@ void ovc_destroy(ovc_ctx* c) {
   if (c->d_cond_sel) cudaFree(c->d_cond_sel);
   if (c->d_tcw) cudaFree(c->d_tcw);
   if (c->d_re) cudaFree(c->d_re);
+  for (auto& kv : c->rs_banks) cudaFree(kv.second);
   if (c->d_tw) cudaFree(c->d_tw);
   if (c->d_win) cudaFree(c->d_win);
   drop_graphs(c);
@@ -1594,6 +1600,74 @@ int ovc_reference_encoder_ragged(ovc_ctx* c, const float* spec, const int64_t* l
                                  void* stream) {
   if (!lengths) return fail(OVC_ERR_INVALID, "null lengths in ovc_reference_encoder_ragged");
   return run_refenc(c, spec, (const long long*)lengths, N, Tmax, out, stream);
+}
+
+static int resample_plan(int sr_in, int sr_out, ovc_rs::Plan* p) {
+  if (ovc_rs::make_plan(sr_in, sr_out, p) != 0)
+    return fail(OVC_ERR_INVALID, "cannot resample %d Hz -> %d Hz: both rates must be positive and the reduced ratio "
+                "up/down must have max(up, down) <= %lld", sr_in, sr_out, (long long)ovc_rs::MAX_M);
+  return OVC_OK;
+}
+
+int ovc_resample_span(int sr_in, int sr_out, int64_t n_in, int64_t m0, int64_t m1, int64_t* out4) {
+  ovc_rs::Plan p;
+  TRY(resample_plan(sr_in, sr_out, &p));
+  if (!out4 || n_in < 0 || m0 < 0 || m1 <= m0) return fail(OVC_ERR_INVALID, "bad argument to ovc_resample_span");
+  int64_t lo, hi;
+  ovc_rs::span(p, m0, m1, &lo, &hi);
+  out4[0] = ovc_rs::n_out(p, n_in);
+  out4[1] = ovc_rs::n_ready(p, n_in);
+  out4[2] = lo;
+  out4[3] = hi;
+  return OVC_OK;
+}
+
+int ovc_resample(ovc_ctx* c, int sr_in, int sr_out, const float* in, const int64_t* in_lengths, int B, int64_t in_pitch,
+                 int64_t in_start, float* out, int64_t out_pitch, int64_t out_start, void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  ovc_rs::Plan p;
+  TRY(resample_plan(sr_in, sr_out, &p));
+  if (!in || !in_lengths || !out) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (B < 1 || B > 65535 || in_pitch < 0 || out_pitch < 0 || out_start < 0)
+    return fail(OVC_ERR_INVALID, "bad sizes B=%d in_pitch=%lld out_pitch=%lld out_start=%lld", B, (long long)in_pitch,
+                (long long)out_pitch, (long long)out_start);
+  if (out_pitch == 0) return OVC_OK;
+  ON_DEVICE(c);
+  double*& bank = c->rs_banks[{p.up, p.down}];
+  if (!bank) {
+    const std::vector<double> h = ovc_rs::design_bank(p);
+    CK(cudaMalloc(&bank, h.size() * sizeof(double)));
+    // ordered on the call's stream (a non-blocking stream does not wait for the legacy default stream) and finished
+    // before the pageable source goes out of scope
+    CK(cudaMemcpyAsync(bank, h.data(), h.size() * sizeof(double), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    CK(cudaStreamSynchronize((cudaStream_t)stream));
+  }
+  // tile of up to 256 outputs whose staged span fits the opt-in shared memory; staged as doubles when one output's does
+  const int64_t smem_max = 200 * 1024;
+  const bool dbl = resample_stage_len(p, 1) * (int64_t)sizeof(double) <= smem_max;
+  const int64_t elem = dbl ? sizeof(double) : sizeof(float);
+  int tile = 256;
+  while (tile > 1 && resample_stage_len(p, tile) * elem > smem_max) tile /= 2;
+  const size_t smem = (size_t)(resample_stage_len(p, tile) * elem);
+  const int64_t tiles = (out_pitch + tile - 1) / tile;
+  if (tiles > 0x7fffffffLL) return fail(OVC_ERR_INVALID, "out_pitch %lld too large", (long long)out_pitch);
+  const dim3 grid((unsigned)tiles, B);
+  const int threads = std::min(256, (tile + 31) / 32 * 32);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!c->rs_smem_opt_in) {
+    CK(cudaFuncSetAttribute(resample_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+    CK(cudaFuncSetAttribute(resample_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+    c->rs_smem_opt_in = true;
+  }
+  if (dbl) {
+    resample_kernel<double><<<grid, threads, smem, st>>>(p, bank, in, in_pitch, in_start, (const int64_t*)in_lengths, out,
+                                                         out_pitch, out_start, tile);
+  } else {
+    resample_kernel<float><<<grid, threads, smem, st>>>(p, bank, in, in_pitch, in_start, (const int64_t*)in_lengths, out,
+                                                        out_pitch, out_start, tile);
+  }
+  CK(cudaGetLastError());
+  return OVC_OK;
 }
 
 int ovc_tts_info(const ovc_ctx* c, int32_t* out8) {

@@ -18,20 +18,101 @@ concatenated output equals ``convert`` on the whole clip with the same noise (``
 <= 2e-6 * rms, the fp32 reordering between tile geometries), whatever the chunking of the input.
 Algorithmic latency: (128 + window_frames) * 256 samples; compute per emitted frame: (window + 256) / window of the
 offline cost.
+
+Audio that is not at the model's rate (48 kHz from WebRTC and most sound cards, 16 kHz from telephony) goes through
+``StreamingResampler``: ``StreamingConverter(..., input_sr=48000, output_sr=48000)`` resamples the input to the model's
+rate and the converted audio back, each on the device, and each bit-identical to resampling the whole signal at once
+(no clicks at chunk boundaries).  The two filters add their look-ahead to the latency: 10 max(up, down) / up input
+samples each, 0.45 ms for 48 kHz -> 22.05 kHz and 0.45 ms for 22.05 kHz -> 48 kHz, 0.91 ms in all
+(``StreamingResampler.lookahead_s`` computes it from the library's span function).
 """
 from typing import Callable, Optional
 
 import numpy as np
 import torch
 
+from ._native import STREAM_OPEN, resample_span
+
+
+class StreamingResampler:
+    """Stateful ``ovc_resample`` (scipy.signal.resample_poly arithmetic) from ``sr_in`` to ``sr_out``.
+
+    ``push(x)`` returns every output sample whose input support has arrived; ``flush()`` ends the stream and returns
+    the rest, up to n_out(total) = ceil(total * sr_out / sr_in).  Only the input tail that future outputs read is kept
+    (about 20 max(up, down) / up samples).  Every output is computed by the same fp64 sum as the one-shot call, so for
+    any chunking the concatenated output equals ``NativeConverter.resample`` of the whole signal bit for bit.
+    ``native``: a ``NativeConverter`` (or anything with a ``.native`` one, such as ``NativeSynthesizer``)."""
+
+    def __init__(self, native, sr_in: int, sr_out: int):
+        self.native = getattr(native, "native", native)
+        self.sr_in, self.sr_out = int(sr_in), int(sr_out)
+        resample_span(self.sr_in, self.sr_out)            # ValueError for a pair the resampler refuses
+        self.dev = torch.device("cuda", self.native.device_index)
+        self.buf = np.zeros(0, dtype=np.float32)          # input samples [b0, b0 + len(buf))
+        self.b0 = 0
+        self.n_in = 0
+        self.emitted = 0
+        self.closed = False
+
+    @property
+    def state_samples(self) -> int:
+        return int(len(self.buf))
+
+    @property
+    def lookahead_s(self) -> float:
+        """Seconds of input an output sample waits for past its own time: the filter's half support."""
+        m = 10 ** 6
+        hi = resample_span(self.sr_in, self.sr_out, 0, m, m + 1)[3]
+        return (hi - 1) / self.sr_in - m / self.sr_out
+
+    def _emit(self, m1: int, length: int) -> np.ndarray:
+        m0 = self.emitted
+        if m1 <= m0:
+            return np.zeros(0, dtype=np.float32)
+        _, _, lo, hi = resample_span(self.sr_in, self.sr_out, 0, m0, m1)
+        lo, hi = max(lo, 0), min(hi, self.n_in)
+        seg = self.buf[lo - self.b0: hi - self.b0] if hi > lo else np.zeros(1, dtype=np.float32)
+        start = lo if hi > lo else self.n_in              # no sample needed: one that reads as 0
+        x = torch.from_numpy(np.ascontiguousarray(seg)).to(self.dev)[None]
+        ln = torch.tensor([length], dtype=torch.int64, device=self.dev)
+        y = self.native.resample(x, ln, self.sr_in, self.sr_out, out_pitch=m1 - m0, in_start=start, out_start=m0)
+        self.emitted = m1
+        keep = max(0, resample_span(self.sr_in, self.sr_out, 0, m1, m1 + 1)[2])
+        if keep > self.b0:
+            self.buf = self.buf[keep - self.b0:]
+            self.b0 = keep
+        return y[0].cpu().numpy()
+
+    @torch.no_grad()
+    def push(self, samples) -> np.ndarray:
+        assert not self.closed, "the stream has been flushed"
+        x = np.asarray(samples, dtype=np.float32).reshape(-1)
+        self.buf = np.concatenate([self.buf, x])
+        self.n_in += len(x)
+        return self._emit(resample_span(self.sr_in, self.sr_out, self.n_in)[1], STREAM_OPEN)
+
+    @torch.no_grad()
+    def flush(self) -> np.ndarray:
+        assert not self.closed
+        self.closed = True
+        return self._emit(resample_span(self.sr_in, self.sr_out, self.n_in)[0], self.n_in)
+
 
 class StreamingConverter:
     def __init__(self, converter, src_se, tgt_se, tau: float = 0.3, window_frames: int = 256,
-                 noise_fn: Optional[Callable[[int, int], torch.Tensor]] = None, seed: Optional[int] = None):
+                 noise_fn: Optional[Callable[[int, int], torch.Tensor]] = None, seed: Optional[int] = None,
+                 input_sr: Optional[int] = None, output_sr: Optional[int] = None):
         """``converter``: a ToneColorConverter.  ``noise_fn(t0, t1) -> [inter_channels, t1 - t0]`` supplies the noise of
-        absolute frames [t0, t1) (tests pass slices of one tensor); default: a seeded device generator."""
+        absolute frames [t0, t1) (tests pass slices of one tensor); default: a seeded device generator.
+        ``input_sr`` / ``output_sr``: rates of the pushed and of the returned audio when they are not the model's
+        (``StreamingResampler`` on each side; None: the model's rate)."""
         self.conv = converter
         hp = converter.hps
+        self.rs_in = self.rs_out = None
+        if input_sr is not None and int(input_sr) != int(hp.data.sampling_rate):
+            self.rs_in = StreamingResampler(converter.model, input_sr, hp.data.sampling_rate)
+        if output_sr is not None and int(output_sr) != int(hp.data.sampling_rate):
+            self.rs_out = StreamingResampler(converter.model, hp.data.sampling_rate, output_sr)
         self.hop = hp.data.hop_length
         self.nfft = hp.data.filter_length
         self.pad = (self.nfft - self.hop) // 2            # reflect padding of spectrogram_torch
@@ -123,9 +204,25 @@ class StreamingConverter:
     # ------------------------------------------------------------------ public
     @torch.no_grad()
     def push(self, samples) -> np.ndarray:
-        """Feed float32 samples at the model's sampling rate; returns the converted samples that became final."""
+        """Feed float32 samples (at ``input_sr``, default the model's rate); returns the converted samples that became
+        final (at ``output_sr``, default the model's rate)."""
         assert not self.closed, "the stream has been flushed"
         x = np.asarray(samples, dtype=np.float32).reshape(-1)
+        if self.rs_in is not None:
+            x = self.rs_in.push(x)
+        y = self._push(x)
+        return y if self.rs_out is None else self.rs_out.push(y)
+
+    @torch.no_grad()
+    def flush(self) -> np.ndarray:
+        """End of the stream: converts what is left (the last frames use the right reflect padding, exactly like the
+        whole-clip spectrogram).  Total output = hop * (samples_in // hop) at the model's rate, as ``convert`` returns
+        (then resampled to ``output_sr``)."""
+        assert not self.closed
+        y = self._flush() if self.rs_in is None else np.concatenate([self._push(self.rs_in.flush()), self._flush()])
+        return y if self.rs_out is None else np.concatenate([self.rs_out.push(y), self.rs_out.flush()])
+
+    def _push(self, x: np.ndarray) -> np.ndarray:
         self.audio = np.concatenate([self.audio, x])
         self.n_in += len(x)
         self._extend_spec(final=False)
@@ -135,11 +232,7 @@ class StreamingConverter:
             outs.append(self._convert_window(self.emitted, self.emitted + self.W, None))
         return np.concatenate(outs) if outs else np.zeros(0, dtype=np.float32)
 
-    @torch.no_grad()
-    def flush(self) -> np.ndarray:
-        """End of the stream: converts what is left (the last frames use the right reflect padding, exactly like the
-        whole-clip spectrogram).  Total output = hop * (samples_in // hop), as ``convert`` returns."""
-        assert not self.closed
+    def _flush(self) -> np.ndarray:
         self.closed = True
         T = self.n_in // self.hop
         if T < 1 or self.n_in <= self.pad:
