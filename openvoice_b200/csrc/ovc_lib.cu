@@ -186,7 +186,7 @@ struct ovc_ctx {
   // of the SMs (OVC_OPT_BRANCHES; taken when B * Tmax <= par_frames = 512 frames)
   bool use_branches = true;
   int par_frames = 512;
-  bool use_pair = true;        // OVC_OPT_PAIR: the HBM-bound ResBlock conv pairs (C <= 64, k = 3) as ONE kernel (tcconv_kernel<C, true>)
+  bool use_pair = true;        // OVC_OPT_PAIR: the ResBlock conv pairs of the C <= 128 stages as ONE kernel (tcconv_kernel<C, true>, tc_pair_fuses)
   cudaStream_t br_stream[2] = {nullptr, nullptr};
   cudaEvent_t br_ev[4] = {nullptr, nullptr, nullptr, nullptr};
   size_t post_w_off = 0;
@@ -656,6 +656,7 @@ static int finalize(ovc_ctx* c) {
   CK(cudaFuncSetAttribute(tcconv_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<128, false>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tcconv_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<64, false>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tcconv_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<32, false>::SMEM_BYTES));
+  CK(cudaFuncSetAttribute(tcconv_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<128, true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tcconv_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<64, true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tcconv_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<32, true>::SMEM_BYTES));
   if (c->d_cond_wrow) cudaFree(c->d_cond_wrow);
@@ -806,11 +807,12 @@ static int prof_end(Run& r, int variant, int family, double flops, double bytes,
   c->ev_tag.push_back(tag);
   return OVC_OK;
 }
-enum { V_TCPAIR64 = -12, V_TCPAIR32 = -13, V_TC128 = -1, V_TC64 = -2, V_TC32 = -3, V_TRANSPOSE = -4, V_TTS_DENSE = -5, V_TTS_LN = -6, V_TTS_SCORES = -7,
+enum { V_TCPAIR128 = -14, V_TCPAIR64 = -12, V_TCPAIR32 = -13, V_TC128 = -1, V_TC64 = -2, V_TC32 = -3, V_TRANSPOSE = -4, V_TTS_DENSE = -5, V_TTS_LN = -6, V_TTS_SCORES = -7,
        V_TTS_ATTN = -8, V_TTS_DW = -9, V_TTS_SPLINE = -10, V_TTS_MISC = -11 };
 static const char* variant_name(int v) {
   if (v >= 0) return kInfo[v].name;
   switch (v) {
+    case V_TCPAIR128: return "PAIR_N128";
     case V_TCPAIR64: return "PAIR_N64";
     case V_TCPAIR32: return "PAIR_N32";
     case V_TC128: return "TC3_N128";
@@ -892,8 +894,8 @@ static int launch_tc(Run& r, const TcLayer& T, const float* x, float* y, const f
   return OVC_OK;
 }
 
-// one ResBlock conv pair (c1 dilated, c2 dilation 1, residual = the pair's input) as ONE kernel: C = 64 / 32 stages,
-// where tc_pair_fits (ovc_tcpack.h) accepts the pair
+// one ResBlock conv pair (c1 dilated, c2 dilation 1, residual = the pair's input) as ONE kernel: C = 128 / 64 / 32
+// stages, where tc_pair_fuses (ovc_tcpack.h) accepts the pair
 static int launch_pair(Run& r, const TcLayer& T1, const TcLayer& T2, const float* x, float* y, int t_len, int mul, float slope,
                        float scale, int accumulate) {
   TcConvArgs a{};
@@ -911,12 +913,13 @@ static int launch_pair(Run& r, const TcLayer& T1, const TcLayer& T2, const float
   const int n_tt = g.n_tt, total = g.total;
   TRY(prof_begin(r));
   dim3 pg((unsigned)g.grid_x, 1, 1);
-  if (C == 64) CK(launch_ex(tcconv_kernel<64, true>, pg, TCN_THREADS, TcnCfg<64, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
+  if (C == 128) CK(launch_ex(tcconv_kernel<128, true>, pg, TCN_THREADS, TcnCfg<128, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
+  else if (C == 64) CK(launch_ex(tcconv_kernel<64, true>, pg, TCN_THREADS, TcnCfg<64, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
   else CK(launch_ex(tcconv_kernel<32, true>, pg, TCN_THREADS, TcnCfg<32, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
   CK(cudaGetLastError());
   r.c->launches++;
   const double units = (double)r.B * t_len;
-  TRY(prof_end(r, C == 64 ? V_TCPAIR64 : V_TCPAIR32, 1, 2.0 * 2.0 * C * C * T1.K * units, 4.0 * C * (2 + (accumulate ? 1 : 0)) * units,
+  TRY(prof_end(r, C == 128 ? V_TCPAIR128 : C == 64 ? V_TCPAIR64 : V_TCPAIR32, 1, 2.0 * 2.0 * C * C * T1.K * units, 4.0 * C * (2 + (accumulate ? 1 : 0)) * units,
                (C << 16) | (T1.K << 8) | T1.DIL));
   return OVC_OK;
 }
@@ -1182,7 +1185,7 @@ static int run_dec(Run& r, const WsLayout& W, float* ws, const float* cond, cons
       if (!par) {
         for (int j = 0; j < 3; ++j) {
           bool fused = c->use_pair;
-          for (int d = 0; d < 3; ++d) fused = fused && tc_pair_fits(c->tc_c1[i * 3 + j][d], c->tc_c2[i * 3 + j][d]);
+          for (int d = 0; d < 3; ++d) fused = fused && tc_pair_fuses(c->tc_c1[i * 3 + j][d], c->tc_c2[i * 3 + j][d]);
           if (fused) {
             // one kernel per conv pair; a pair never runs in place (its tiles read x with a halo), so the running
             // activation ping-pongs bufA -> bufB -> bufC -> bufD (bufC is free: the intermediate stays on chip)
@@ -1782,7 +1785,9 @@ int ovc_profile_detail(ovc_ctx* c, int max, char* names /* max x 16 */, double* 
     CK(cudaEventElapsedTime(&m, c->ev[i], c->ev[i + 1]));
     if (names) {
       const int tag = c->ev_tag[i / 2], v = c->ev_variant[i / 2];
-      if (tag && (v == V_TCPAIR64 || v == V_TCPAIR32)) snprintf(names + 16 * n, 16, "P%dk%dd%d", tag >> 16, (tag >> 8) & 255, tag & 255);
+      // the C = 128 pair is named T128P...: per-kernel tables group names by their first four characters
+      if (tag && v == V_TCPAIR128) snprintf(names + 16 * n, 16, "T128Pk%dd%d", (tag >> 8) & 255, tag & 255);
+      else if (tag && (v == V_TCPAIR64 || v == V_TCPAIR32)) snprintf(names + 16 * n, 16, "P%dk%dd%d", tag >> 16, (tag >> 8) & 255, tag & 255);
       else if (tag) snprintf(names + 16 * n, 16, "T%dc%dk%dd%d", v == V_TC128 ? 128 : v == V_TC64 ? 64 : 32, tag >> 16, (tag >> 8) & 255, tag & 255);
       else { strncpy(names + 16 * n, variant_name(v), 15); names[16 * n + 15] = 0; }
     }

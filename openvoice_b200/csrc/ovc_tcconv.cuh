@@ -168,10 +168,10 @@ constexpr int TCN_NCT = 96;        // converter threads (warps 1-3)
 
 template <int TN, bool PAIR>
 struct TcnCfg {
-  static_assert(!PAIR || TN == 32 || TN == 64, "conv pairs: C = 32 or 64");
+  static_assert(!PAIR || TN == 32 || TN == 64 || TN == 128, "conv pairs: C = 32, 64 or 128");
   static constexpr int KCH = 32, NKC = KCH / 8;                   // channels per converted A chunk
   static constexpr int ROWS = 194;                                // A pitch in rows: >= 128 + 2 * TCN_HMAX, = 2 (mod 8)
-  static constexpr int ROWS2 = 146;                               // PAIR: conv-2 A pitch: 128 + 2 * H2 rows, H2 <= 9
+  static constexpr int ROWS2 = TCN_ROWS2;                         // PAIR: conv-2 A pitch: 128 + 2 * H2 rows, H2 <= 9
   static constexpr int NABUF = 2;
   static constexpr int RING = tc_ring_slots(TN, PAIR);            // weight slots (ovc_tcpack.h)
   static constexpr int SLOT_BYTES = 2 * 2 * TN * 16;
@@ -206,7 +206,7 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
   const int n_slots = (a.Cin / 16) * a.K;      // weight slots per conv
   const int n_w = PAIR ? 2 * n_slots : n_slots;
   const bool resident = n_w <= RING;
-  if (H1 > TCN_HMAX || (PAIR && (!resident || 128 + 2 * H2 > ROWS2))) __trap();   // host: tc_tile_n / tc_pair_fits (ovc_tcpack.h)
+  if (H1 > TCN_HMAX || (PAIR && 128 + 2 * H2 > ROWS2)) __trap();   // host: tc_tile_n / tc_pair_fuses (ovc_tcpack.h)
   constexpr uint32_t BYTES = Cfg::SLOT_BYTES;
 
   if (tid == 0) {
@@ -249,14 +249,17 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
           // the CTA can exit (its shared memory may be handed to the next kernel's CTA)
           for (int it = 0; it < n_w; ++it) mbar_wait(&b_full[it], 0u);
         } else {
+          // streamed: every tile takes conv 1's slots (and a pair's conv-2 slots after them) in the MMA order
           int slot = 0;
           uint32_t phase = 1;   // the first pass over the ring finds every slot free
           TCN_FOR_TILES
             (void)b;
-            for (int it = 0; it < n_slots; ++it) {
+            for (int it = 0; it < n_w; ++it) {
+              const unsigned char* src = it < n_slots ? wt + (size_t)it * BYTES
+                                                      : reinterpret_cast<const unsigned char*>(a.w2) + (size_t)(it - n_slots) * BYTES;
               mbar_wait(&b_empty[slot], phase);
               mbar_expect_tx(&b_full[slot], BYTES);
-              tma_bulk_g2s(bring + slot * BYTES, wt + (size_t)it * BYTES, BYTES, &b_full[slot]);
+              tma_bulk_g2s(bring + slot * BYTES, src, BYTES, &b_full[slot]);
               if (++slot == RING) { slot = 0; phase ^= 1; }
             }
           }
@@ -394,15 +397,26 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> tensor-core (async) proxy
         named_bar_sync(2, 256);   // every row of the conv-2 operand is written
-        // ---- conv 2 (dilation 1, weights in the resident slots after conv 1's)
+        // ---- conv 2 (dilation 1, weights in the resident slots after conv 1's, or the next ones of the stream)
         const uint64_t a2_proto = tc::make_desc(0, LBO_A2, SBO);
         tc::fence_regs(d);
         tc::wgmma_fence();
         bool first2 = true;
+        int prev = -1;
         for (int kk = 0; kk < TN / 16; ++kk) {
           uint64_t a_cur = a2_proto + ((tc::smem_addr(a2buf) + 64 * wg * 16 + 2 * kk * LBO_A2) >> 4);
           for (int tap = 0; tap < a.K; ++tap) {
-            tc_mma_step<TN>(d, a_cur, a_cur + A2_LO16, b_ring + (uint32_t)(n_slots + kk * a.K + tap) * SLOT16, three, first2);
+            if (resident) {
+              tc_mma_step<TN>(d, a_cur, a_cur + A2_LO16, b_ring + (uint32_t)(n_slots + kk * a.K + tap) * SLOT16, three, first2);
+            } else {
+              mbar_wait(&b_full[slot], bphase);
+              tc_mma_step<TN>(d, a_cur, a_cur + A2_LO16, b_ring + (uint32_t)slot * SLOT16, three, first2);
+              tc::wgmma_commit();
+              tc::wgmma_wait<1>();                              // the previous step's MMAs have read their slot
+              if (leader && prev >= 0) mbar_arrive(&b_empty[prev]);
+              prev = slot;
+              if (++slot == RING) { slot = 0; bphase ^= 1; }
+            }
             first2 = false;
             a_cur += 1;
           }
@@ -410,6 +424,7 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
         tc::wgmma_commit();
         tc::wgmma_wait<0>();
         tc::fence_regs(d);
+        if (leader && prev >= 0) mbar_arrive(&b_empty[prev]);
         TcConvArgs e = a;
         e.y_ld = TN; e.r = a.x; e.bias = a.bias2; e.bias_bs = 0; e.epi = 0;
         tc_epilogue<TN>(e, d, b, t0, 0, min(lim, t0 + R), row_a);

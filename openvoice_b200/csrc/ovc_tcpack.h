@@ -12,10 +12,13 @@
 namespace ovc {
 
 constexpr int TCN_HMAX = 25;   // largest conv-1 halo (k = 11, dilation 5): the staged A tile holds 128 + 2 * 25 rows
+constexpr int TCN_ROWS2 = 146;  // conv pair: rows of the on-chip conv-2 operand, 128 + 2 * H2 with conv-2 halo H2 <= 9
 
 // weight slots (16 channels x 1 tap, hi and lo parts) in the shared-memory ring: TN = 32 holds k = 11 resident,
-// TN = 64 k = 3; pairs hold both convs
-constexpr int tc_ring_slots(int TN, bool pair) { return pair ? (TN == 32 ? 44 : 24) : (TN == 32 ? 22 : 12); }
+// TN = 64 k = 3; pairs hold both convs resident up to TN = 32 k = 11 and TN = 64 k = 3, and stream the rest
+constexpr int tc_ring_slots(int TN, bool pair) {
+  return pair ? (TN == 32 ? 44 : TN == 64 ? 24 : 12) : (TN == 32 ? 22 : 12);
+}
 
 // the geometry of one packed conv (TN = 0: the conv does not fit the tensor-core kernels)
 struct TcGeom {
@@ -82,14 +85,23 @@ inline float tc_ups_weight(RAW raw, int s, int kk, int cout, int row, int ci, in
   return (kidx >= 0 && kidx < kk) ? raw(ci, co, kidx) : 0.f;
 }
 
-// a ResBlock conv pair runs as ONE kernel only where both convs' weights stay resident in shared memory next to the
-// operand tiles (C = 32 / 64, conv 2 of dilation 1), and only for the pairs whose traffic is dominated by HBM (k <= 5):
-// at larger k a tile's 128 - (k - 1) output steps waste more of the MMA work
+// the pairs whose two convs' weights stay resident in shared memory next to the operand tiles (C = 32 / 64, conv 2 of
+// dilation 1, k <= 5).  The pair kernel also streams the weights of larger pairs through its ring (tc_pair_fuses).
 inline bool tc_pair_fits(const TcGeom& T1, const TcGeom& T2) {
   if (!(T1.TN == 32 || T1.TN == 64)) return false;
   const int ring = tc_ring_slots(T1.TN, true);
   return T1.Ntot == T1.TN && T1.Cin == T1.TN && T2.Ntot == T1.TN && T2.Cin == T1.TN && T2.TN == T1.TN && T2.K == T1.K &&
          T2.DIL == 1 && (T1.K - 1) / 2 * T1.DIL <= TCN_HMAX && 2 * (T1.Cin / 16) * T1.K <= ring && T1.K <= 5;
+}
+
+// a ResBlock conv pair runs as ONE kernel (tcconv_kernel<C, true>) when it is a square C = 32 / 64 / 128 pair, conv 2
+// of dilation 1 and the same k, whose conv-2 halo fits the on-chip operand.  That includes every pair tc_pair_fits
+// accepts; the kernel streams the weights of the others through its ring.  Measured per (C, k) on an H100, every
+// generator pair of the C <= 128 stages is faster fused than as two launches (DESIGN.md, fused ResBlock conv pair).
+inline bool tc_pair_fuses(const TcGeom& T1, const TcGeom& T2) {
+  if (!(T1.TN == 32 || T1.TN == 64 || T1.TN == 128)) return false;
+  return T1.Ntot == T1.TN && T1.Cin == T1.TN && T2.Ntot == T1.TN && T2.Cin == T1.TN && T2.TN == T1.TN && T2.K == T1.K &&
+         T2.DIL == 1 && (T1.K - 1) / 2 * T1.DIL <= TCN_HMAX && 128 + 2 * ((T2.K - 1) / 2) <= TCN_ROWS2;
 }
 
 // persistent launch: the CTAs of one column tile (grid.y) walk the (utterance, time tile) list, tile = b * n_tt + i
