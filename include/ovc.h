@@ -25,9 +25,10 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 5   /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 6   /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
-                               * 5: ovc_resample, ovc_resample_span */
+                               * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
+                               * ovc_philox_normals */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -103,7 +104,10 @@ OVC_API size_t ovc_workspace_floats(const ovc_ctx* ctx, int B, int Tmax);
  *   g_src    [B, gin] source tone-colour embedding (sid_src, [B,gin,1])        (models.py:493)
  *   g_tgt    [B, gin] target tone-colour embedding (sid_tgt)
  *   noise    [B, inter, Tmax] N(0,1) draws standing in for randn_like at models.py:220,
- *            or NULL: the kernel then draws Philox4x32-10 normals from `seed`
+ *            or NULL: the kernel then draws Philox4x32-10 normals from `seed`.  Counter layout: item b, channel c,
+ *            frame t draws philox(key = seed; stream = b, channel = c, frame = t), i.e. ovc_philox_normals(seed, b, 0,
+ *            inter, 0, Tmax).  With ovc_voice_conversion_items the key, stream and frame offset can be given per item:
+ *            philox(key = seed[b]; stream[b], c, (frame0[b] + t) mod 2^32)
  *   tau      scales the noise term only                                        (models.py:220)
  *   ragged   0: reference batch semantics -- the (unmasked) generator runs over all Tmax frames
  *               of every item exactly as SynthesizerTrn.voice_conversion does on a padded batch
@@ -116,6 +120,47 @@ OVC_API int ovc_voice_conversion(ovc_ctx* ctx, const float* spec, const int64_t*
                          const float* g_src, const float* g_tgt, const float* noise,
                          uint64_t seed, float tau, int B, int Tmax, int ragged,
                          float* o_hat, float* z, float* z_p, float* z_hat, void* stream);
+
+/* Per-item sampling parameters: each pointer is a DEVICE array of B values, or NULL for "the call's scalar / the
+ * default".  With a request's own seed, stream and frame offset, its noise no longer depends on where it sits in a
+ * batch, which stream serves it or which window of a longer clip is being converted.  The arrays are read on the device
+ * when the kernels run: a call that repeats the same pointers is replayed from its CUDA graph (OVC_OPT_GRAPH) and
+ * follows the arrays' current contents.  Which entry point reads which field:
+ *   seed           all four: the Philox key of item b (replaces `seed`; for ovc_tts_decode the decode key, which
+ *                  SynthesizerTrn.infer-style callers set to the encode key + 1)
+ *   stream         all four: counter word 0 of item b (default b)
+ *   frame0         voice conversion / convert_waveform: frame counter offset, item b's frame t draws at
+ *                  (frame0[b] + t) mod 2^32 (default 0) -- a window starting at frame lo of a longer clip passes lo
+ *   tau            voice conversion / convert_waveform (replaces `tau`)
+ *   noise_scale_w, length_scale, sdp_ratio   ovc_tts_encode (length_scale values must be positive)
+ *   noise_scale    ovc_tts_decode
+ * Fields an entry point does not list are ignored.  An explicit noise / noise_w tensor still wins over every key
+ * field; the scale fields apply to it too.  NULL fields evaluate exactly the same expressions as the entry points
+ * without _items: a struct of NULLs (or items == NULL) gives bit-identical results. */
+typedef struct ovc_item_params {
+  const uint64_t* seed;
+  const int64_t* stream;
+  const int64_t* frame0;
+  const float* tau;
+  const float* noise_scale;
+  const float* noise_scale_w;
+  const float* length_scale;
+  const float* sdp_ratio;
+} ovc_item_params;
+
+/* ovc_voice_conversion with per-item parameters; `items` is a HOST pointer (NULL = none). */
+OVC_API int ovc_voice_conversion_items(ovc_ctx* ctx, const float* spec, const int64_t* lengths,
+                                       const float* g_src, const float* g_tgt, const float* noise,
+                                       uint64_t seed, float tau, int B, int Tmax, int ragged,
+                                       float* o_hat, float* z, float* z_p, float* z_hat, void* stream,
+                                       const ovc_item_params* items);
+
+/* out[c][t] = the Philox normal at (key = seed; stream, channel c0 + c, frame (frame0 + t) mod 2^32), c < C, t < T:
+ * exactly the value the kernels draw in-kernel at that counter (see `noise` above; the TTS noise_w rows are channels
+ * 0x7700 and 0x7701).  out [C, T] fp32 on the caller's current device; only enqueues on `cuda_stream`.  For tests and
+ * for callers that must hand a kernel the noise a request would have drawn. */
+OVC_API int ovc_philox_normals(uint64_t seed, int64_t stream, int64_t c0, int C, int64_t frame0, int T, float* out,
+                               void* cuda_stream);
 
 /* Front end of convert (row a2): linear magnitude spectrogram, replaces spectrogram_torch
  * (openvoice/mel_processing.py:40-75; call sites api.py:126-128,150-152) for n_fft = win = 1024,
@@ -135,6 +180,11 @@ OVC_API int ovc_spectrogram(ovc_ctx* ctx, const float* wav, const int64_t* wav_l
 OVC_API int ovc_convert_waveform(ovc_ctx* ctx, const float* wav, const int64_t* wav_lengths, int B, int Lmax,
                                  const float* g_src, const float* g_tgt, const float* noise, uint64_t seed,
                                  float tau, float* o_hat, int64_t* frames, void* stream);
+/* ovc_convert_waveform with per-item parameters (ovc_item_params; `items` a host pointer, NULL = none). */
+OVC_API int ovc_convert_waveform_items(ovc_ctx* ctx, const float* wav, const int64_t* wav_lengths, int B, int Lmax,
+                                       const float* g_src, const float* g_tgt, const float* noise, uint64_t seed,
+                                       float tau, float* o_hat, int64_t* frames, void* stream,
+                                       const ovc_item_params* items);
 
 /* Tone-colour embedding of extract_se (row f2): ReferenceEncoder.forward (openvoice/models.py:339-359; call site
  * openvoice/api.py:130) on device -- LayerNorm over frequency, 6 x (Conv2d 3x3 s2 + ReLU), GRU(128) last state,
@@ -204,6 +254,17 @@ OVC_API int ovc_tts_encode(ovc_ctx* ctx, const int64_t* tokens, const int64_t* x
                            int B, int T, int64_t* y_lengths, float* w_ceil, float* logw, void* stream);
 OVC_API int ovc_tts_decode(ovc_ctx* ctx, const float* noise, uint64_t seed, float noise_scale, int B, int Ymax, int max_len,
                            int ragged, float* o, float* z, float* z_p, void* stream);
+/* The two halves with per-item parameters (ovc_item_params; `items` a host pointer, NULL = none).  The Philox draws:
+ * noise_w row r of item b = philox(key; stream, 0x7700 + r, t) with the encode key, z_p noise = philox(key; stream, c, y)
+ * with the decode key (key = seed[b] or `seed`, stream = stream[b] or b).  Sentence j of a batch-1-per-request infer
+ * with seed s is therefore reproduced inside any batch by seed = s (encode), s + 1 (decode), stream = j. */
+OVC_API int ovc_tts_encode_items(ovc_ctx* ctx, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid,
+                                 const float* noise_w, uint64_t seed, float noise_scale_w, float length_scale, float sdp_ratio,
+                                 int B, int T, int64_t* y_lengths, float* w_ceil, float* logw, void* stream,
+                                 const ovc_item_params* items);
+OVC_API int ovc_tts_decode_items(ovc_ctx* ctx, const float* noise, uint64_t seed, float noise_scale, int B, int Ymax,
+                                 int max_len, int ragged, float* o, float* z, float* z_p, void* stream,
+                                 const ovc_item_params* items);
 
 /* Arithmetic of the convolutions (generator ResBlocks = 90 % of the FLOPs, WaveNet stacks, upsamplers):
  *   0            fp32 FFMA on the CUDA cores

@@ -13,14 +13,15 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
     "ovc_profile_enable", "ovc_profile_read", "ovc_profile_detail", "ovc_debug_enable", "ovc_debug_fetch",
     "ovc_spectrogram", "ovc_convert_waveform", "ovc_set_precision", "ovc_reference_encoder",
     "ovc_tts_info", "ovc_tts_encode", "ovc_tts_decode", "ovc_set_option", "ovc_graph_replays",
-    "ovc_reference_encoder_ragged", "ovc_resample", "ovc_resample_span",
+    "ovc_reference_encoder_ragged", "ovc_resample", "ovc_resample_span", "ovc_voice_conversion_items",
+    "ovc_convert_waveform_items", "ovc_tts_encode_items", "ovc_tts_decode_items", "ovc_philox_normals",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample input length of a stream that has not ended
@@ -36,6 +37,44 @@ class OvcHParams(C.Structure):
         ("upsample_kernel_sizes", C.c_int32 * 4), ("upsample_initial_channel", C.c_int32),
         ("zero_g", C.c_int32), ("hop_length", C.c_int32),
     ]
+
+
+class ItemParams(C.Structure):
+    """struct ovc_item_params of include/ovc.h: per-item device arrays ([B] each, NULL = the call's value)."""
+    _fields_ = [
+        ("seed", C.c_void_p), ("stream", C.c_void_p), ("frame0", C.c_void_p), ("tau", C.c_void_p),
+        ("noise_scale", C.c_void_p), ("noise_scale_w", C.c_void_p), ("length_scale", C.c_void_p),
+        ("sdp_ratio", C.c_void_p),
+    ]
+
+
+# dtype of each ItemParams field's device array (seeds travel as int64 holding the uint64 bit pattern)
+ITEM_FIELDS = {"seed": "int64", "stream": "int64", "frame0": "int64", "tau": "float32", "noise_scale": "float32",
+               "noise_scale_w": "float32", "length_scale": "float32", "sdp_ratio": "float32"}
+
+
+def item_params(items: Optional[dict], B: int) -> Optional[ItemParams]:
+    """ItemParams from ``{field: [B] cuda tensor or None}`` (None -> no struct: the entry point without items).  Each
+    tensor must be contiguous, on the device and of the field's dtype (``ITEM_FIELDS``); the caller keeps the tensors
+    alive until the call's kernels have run."""
+    if items is None:
+        return None
+    import torch
+    s = ItemParams()
+    for k, t in items.items():
+        if k not in ITEM_FIELDS:
+            raise ValueError(f"unknown item parameter {k!r} (known: {sorted(ITEM_FIELDS)})")
+        if t is None:
+            continue
+        assert t.is_cuda and t.is_contiguous() and t.dtype == getattr(torch, ITEM_FIELDS[k]), k
+        if tuple(t.shape) != (B,):
+            raise ValueError(f"item parameter {k!r} has shape {tuple(t.shape)}, expected ({B},)")
+        setattr(s, k, t.data_ptr())
+    return s
+
+
+def _items_ref(s: Optional[ItemParams]):
+    return C.byref(s) if s is not None else None
 
 
 PRECISIONS = {"fp32": 0, "f16x3": 1, "f16": 2}
@@ -99,6 +138,13 @@ def load_library(path: Optional[str] = None):
     lib.ovc_resample.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]
     lib.ovc_resample_span.argtypes = [C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.POINTER(C.c_int64)]
+    P = C.POINTER(ItemParams)
+    lib.ovc_voice_conversion_items.argtypes = lib.ovc_voice_conversion.argtypes + [P]
+    lib.ovc_convert_waveform_items.argtypes = lib.ovc_convert_waveform.argtypes + [P]
+    lib.ovc_tts_encode_items.argtypes = lib.ovc_tts_encode.argtypes + [P]
+    lib.ovc_tts_decode_items.argtypes = lib.ovc_tts_decode.argtypes + [P]
+    lib.ovc_philox_normals.argtypes = [C.c_uint64, C.c_int64, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_void_p,
+                                       C.c_void_p]
     if lib.ovc_abi_version() != ABI_VERSION:
         raise OvcError(f"ABI mismatch: library {lib.ovc_abi_version()} vs binding {ABI_VERSION}")
     _lib = lib
@@ -148,6 +194,21 @@ def hparams_struct(hps) -> OvcHParams:
     s.zero_g = 1 if get(model, "zero_g", False) else 0
     s.hop_length = int(get(data, "hop_length"))
     return s
+
+
+def philox_normals(seed: int, stream: int, c0: int, channels: int, frame0: int, T: int, device=None, stream_obj=None):
+    """[channels, T] float32 cuda tensor of the in-kernel Philox draws at (key = seed; stream, c0 + c, frame0 + t)
+    (include/ovc.h: ovc_philox_normals): the noise a per-item-keyed call draws, as an explicit tensor."""
+    import torch
+    lib = load_library()
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    out = torch.empty(int(channels), int(T), device=dev, dtype=torch.float32)
+    st = stream_obj if stream_obj is not None else torch.cuda.current_stream(dev)
+    with torch.cuda.device(dev):
+        rc = lib.ovc_philox_normals(C.c_uint64(int(seed) & (2 ** 64 - 1)), int(stream), int(c0), int(channels),
+                                    int(frame0), int(T), C.c_void_p(out.data_ptr()), C.c_void_p(st.cuda_stream))
+    _check(lib, rc, "ovc_philox_normals")
+    return out
 
 
 def resample_span(sr_in: int, sr_out: int, n_in: int = 0, m0: int = 0, m1: int = 1) -> Tuple[int, int, int, int]:
@@ -217,9 +278,10 @@ class NativeConverter:
 
     # ---- hot path --------------------------------------------------------------------------
     def voice_conversion(self, spec, lengths, g_src, g_tgt, noise=None, tau: float = 0.3, seed: int = 0,
-                         ragged: bool = False, latents: bool = True, stream=None):
+                         ragged: bool = False, latents: bool = True, stream=None, items: Optional[dict] = None):
         """spec [B,S,T] f32 cuda, lengths [B] i64 cuda, g_* [B,gin(,1)] f32 cuda.
-        Returns (o_hat [B,1,hop*T], (z, z_p, z_hat) or None).  Asynchronous on `stream`."""
+        Returns (o_hat [B,1,hop*T], (z, z_p, z_hat) or None).  Asynchronous on `stream`.  ``items``: per-item
+        parameters ``{"seed", "stream", "frame0", "tau": [B] cuda tensor}`` (see ``item_params``), or None."""
         import torch
         assert spec.is_cuda and spec.dtype == torch.float32 and spec.is_contiguous()
         assert lengths.is_cuda and lengths.dtype == torch.int64 and lengths.is_contiguous()
@@ -237,11 +299,12 @@ class NativeConverter:
                         for _ in range(3))
         st = stream if stream is not None else torch.cuda.current_stream(spec.device)
         p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-        rc = self.lib.ovc_voice_conversion(
+        it = item_params(items, B)
+        rc = self.lib.ovc_voice_conversion_items(
             self.handle, p(spec), p(lengths), p(gs), p(gt), p(noise), C.c_uint64(seed & (2 ** 64 - 1)),
             C.c_float(tau), B, T, 1 if ragged else 0, p(o),
             p(lat[0]) if lat else None, p(lat[1]) if lat else None, p(lat[2]) if lat else None,
-            C.c_void_p(st.cuda_stream))
+            C.c_void_p(st.cuda_stream), _items_ref(it))
         _check(self.lib, rc, "ovc_voice_conversion")
         return o, lat
 
@@ -262,11 +325,11 @@ class NativeConverter:
         return spec, frames
 
     def convert_waveform(self, wav, wav_lengths, g_src, g_tgt, noise=None, tau: float = 0.3, seed: int = 0, stream=None,
-                         out=None, frames_out=None):
+                         out=None, frames_out=None, items: Optional[dict] = None):
         """The device work of ToneColorConverter.convert for a batch: wav [B, Lmax] f32 cuda ->
         (o_hat [B, hop * (Lmax // hop)], frames [B]).  Asynchronous on `stream`.  ``out`` / ``frames_out`` let the
         caller supply the result buffers: with every buffer at a stable address, a repeated call is replayed from a
-        CUDA graph (include/ovc.h: OVC_OPT_GRAPH)."""
+        CUDA graph (include/ovc.h: OVC_OPT_GRAPH).  ``items`` as in ``voice_conversion``."""
         import torch
         assert wav.is_cuda and wav.dtype == torch.float32 and wav.is_contiguous() and wav.dim() == 2
         assert wav_lengths.is_cuda and wav_lengths.dtype == torch.int64
@@ -288,11 +351,12 @@ class NativeConverter:
         else:
             frames = torch.empty(B, device=wav.device, dtype=torch.int64)
         st = stream if stream is not None else torch.cuda.current_stream(wav.device)
-        rc = self.lib.ovc_convert_waveform(
+        it = item_params(items, B)
+        rc = self.lib.ovc_convert_waveform_items(
             self.handle, C.c_void_p(wav.data_ptr()), C.c_void_p(wav_lengths.data_ptr()), B, L, C.c_void_p(gs.data_ptr()),
             C.c_void_p(gt.data_ptr()), C.c_void_p(noise.data_ptr()) if noise is not None else None,
             C.c_uint64(seed & (2 ** 64 - 1)), C.c_float(tau), C.c_void_p(o.data_ptr()), C.c_void_p(frames.data_ptr()),
-            C.c_void_p(st.cuda_stream))
+            C.c_void_p(st.cuda_stream), _items_ref(it))
         _check(self.lib, rc, "ovc_convert_waveform")
         return o, frames
 
@@ -358,9 +422,10 @@ class NativeConverter:
         return dict(zip(keys, (int(v) for v in out)))
 
     def tts_encode(self, tokens, x_lengths, sid, noise_w=None, seed: int = 0, noise_scale_w: float = 1.0,
-                   length_scale: float = 1.0, sdp_ratio: float = 0.2, stream=None):
+                   length_scale: float = 1.0, sdp_ratio: float = 0.2, stream=None, items: Optional[dict] = None):
         """tokens [B,T] i64 cuda, x_lengths [B] i64 cuda, sid [B] i64 cuda, noise_w [B,2,T] or None (Philox).
-        Returns (y_lengths [B] i64, w_ceil [B,T], logw [B,T]), all on the device; asynchronous on `stream`."""
+        Returns (y_lengths [B] i64, w_ceil [B,T], logw [B,T]), all on the device; asynchronous on `stream`.
+        ``items``: per-item ``{"seed", "stream", "noise_scale_w", "length_scale", "sdp_ratio"}`` (``item_params``)."""
         import torch
         for t in (tokens, x_lengths, sid):
             assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()
@@ -373,15 +438,19 @@ class NativeConverter:
         logw = torch.empty(B, T, device=tokens.device, dtype=torch.float32)
         st = stream if stream is not None else torch.cuda.current_stream(tokens.device)
         p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-        rc = self.lib.ovc_tts_encode(self.handle, p(tokens), p(x_lengths), p(sid), p(noise_w), C.c_uint64(seed & (2 ** 64 - 1)),
-                                     C.c_float(noise_scale_w), C.c_float(length_scale), C.c_float(sdp_ratio), B, T,
-                                     p(y_lengths), p(w_ceil), p(logw), C.c_void_p(st.cuda_stream))
+        it = item_params(items, B)
+        rc = self.lib.ovc_tts_encode_items(self.handle, p(tokens), p(x_lengths), p(sid), p(noise_w),
+                                           C.c_uint64(seed & (2 ** 64 - 1)), C.c_float(noise_scale_w),
+                                           C.c_float(length_scale), C.c_float(sdp_ratio), B, T, p(y_lengths), p(w_ceil),
+                                           p(logw), C.c_void_p(st.cuda_stream), _items_ref(it))
         _check(self.lib, rc, "ovc_tts_encode")
         return y_lengths, w_ceil, logw
 
     def tts_decode(self, B: int, y_max: int, device, noise=None, seed: int = 0, noise_scale: float = 1.0,
-                   ragged: bool = False, latents: bool = False, max_len: Optional[int] = None, stream=None):
-        """Second half of infer() for the last tts_encode.  Returns (o [B,1,hop*min(y_max, max_len)], (z, z_p) or None)."""
+                   ragged: bool = False, latents: bool = False, max_len: Optional[int] = None, stream=None,
+                   items: Optional[dict] = None):
+        """Second half of infer() for the last tts_encode.  Returns (o [B,1,hop*min(y_max, max_len)], (z, z_p) or None).
+        ``items``: per-item ``{"seed" (the decode key), "stream", "noise_scale"}`` (``item_params``)."""
         import torch
         C_ = self.hp.inter_channels
         if noise is not None:
@@ -392,9 +461,10 @@ class NativeConverter:
         lat = tuple(torch.empty(B, C_, y_max, device=device, dtype=torch.float32) for _ in range(2)) if latents else None
         st = stream if stream is not None else torch.cuda.current_stream(device)
         p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-        rc = self.lib.ovc_tts_decode(self.handle, p(noise), C.c_uint64(seed & (2 ** 64 - 1)), C.c_float(noise_scale), B,
-                                     int(y_max), cut, 1 if ragged else 0, p(o), p(lat[0]) if lat else None,
-                                     p(lat[1]) if lat else None, C.c_void_p(st.cuda_stream))
+        it = item_params(items, B)
+        rc = self.lib.ovc_tts_decode_items(self.handle, p(noise), C.c_uint64(seed & (2 ** 64 - 1)), C.c_float(noise_scale),
+                                           B, int(y_max), cut, 1 if ragged else 0, p(o), p(lat[0]) if lat else None,
+                                           p(lat[1]) if lat else None, C.c_void_p(st.cuda_stream), _items_ref(it))
         _check(self.lib, rc, "ovc_tts_decode")
         return o, lat
 

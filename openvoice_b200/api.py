@@ -10,8 +10,9 @@ CUDA only: there is no CPU path.
 """
 from __future__ import annotations
 
+import math
 import os
-from typing import List, Optional, Sequence, Union
+from typing import List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -22,6 +23,39 @@ from .ref_enc import ReferenceEncoder
 from .schema import hot_path_keys, ref_enc_keys, tts_keys
 
 AudioLike = Union[str, np.ndarray]
+
+
+def check_seeds(seeds, n: int, what: str = "seeds") -> Optional[List[int]]:
+    """Per-item Philox keys: None, or ``n`` integers in [0, 2^64).  ValueError otherwise (before any launch)."""
+    if seeds is None:
+        return None
+    seeds = list(seeds)
+    if len(seeds) != n:
+        raise ValueError(f"{len(seeds)} {what} for {n} items")
+    for i, s in enumerate(seeds):
+        if isinstance(s, (bool, np.bool_)) or not isinstance(s, (int, np.integer)) or not 0 <= int(s) < 2 ** 64:
+            raise ValueError(f"{what}[{i}] = {s!r} is not an integer in [0, 2^64)")
+    return [int(s) for s in seeds]
+
+
+def check_per_item(value, n: int, what: str, positive: bool = False) -> Tuple[float, Optional[List[float]]]:
+    """A sampling parameter given as one float for all items or one per item: returns (scalar, None) or
+    (first value, per-item list).  A per-item sequence of the wrong length, or a non-finite value (non-positive with
+    ``positive``), raises ValueError (before any launch)."""
+    if np.ndim(value) == 0:
+        return float(value), None
+    vals = [float(v) for v in value]
+    if len(vals) != n:
+        raise ValueError(f"{len(vals)} values of {what} for {n} items")
+    for i, v in enumerate(vals):
+        if not math.isfinite(v) or (positive and not v > 0):
+            raise ValueError(f"{what}[{i}] = {v!r} is not {'a positive' if positive else 'a finite'} number")
+    return (vals[0] if vals else 0.0), vals
+
+
+def seed_array(seeds: Sequence[int]) -> np.ndarray:
+    """int64 array holding the uint64 bit patterns of ``seeds`` (the device arrays of ovc_item_params.seed)."""
+    return np.asarray([int(s) & (2 ** 64 - 1) for s in seeds], dtype=np.uint64).view(np.int64)
 
 
 def _load_audio(src: AudioLike, sr: int) -> np.ndarray:
@@ -187,14 +221,33 @@ class NativeSynthesizer:
 
     @torch.no_grad()
     def voice_conversion(self, y, y_lengths, sid_src, sid_tgt, tau: float = 1.0, noise=None,
-                         ragged: bool = False, seed: Optional[int] = None, latents: bool = True):
+                         ragged: bool = False, seed: Optional[int] = None, latents: bool = True,
+                         seeds: Optional[Sequence[int]] = None, taus: Optional[Sequence[float]] = None,
+                         frame0: Optional[Sequence[int]] = None, streams: Optional[Sequence[int]] = None):
         """(o_hat, y_mask, (z, z_p, z_hat)) = SynthesizerTrn.voice_conversion
         (openvoice/models.py:492-499).  ``noise`` ([B,192,T]) replaces the reference's
         ``randn_like``; when None, Philox normals are drawn in-kernel from ``seed`` (default: a
         draw from torch's global CPU generator, so ``torch.manual_seed`` makes runs repeatable).
-        ``ragged=True`` converts every item at its exact length (what ``convert`` does)."""
-        y = y.to(self.device, torch.float32).contiguous()
+        ``ragged=True`` converts every item at its exact length (what ``convert`` does).
+
+        Per-item sampling (include/ovc.h: ovc_item_params): ``seeds`` gives item b its own Philox key, drawn at stream
+        ``streams[b]`` (default 0 for every item: a request's own noise, independent of its batch index) and frame
+        ``frame0[b] + t`` (default 0: ``frame0`` places a window of a longer clip at its absolute frames); ``taus``
+        one tau per item.  Without ``seeds`` the call's seed keys every item at stream b, as before.  A seed with
+        ``noise``, a length that is not B, a non-finite tau, a seed outside [0, 2^64) or a frame counter past 2^32
+        raises ValueError."""
         B, _, T = y.shape
+        seeds = check_seeds(seeds, B)
+        taus = check_per_item(taus, B, "taus")[1] if taus is not None else None
+        if noise is not None and seeds is not None:
+            raise ValueError("pass either noise or seeds, not both")
+        f0 = None if frame0 is None else [int(v) for v in frame0]
+        if f0 is not None and (len(f0) != B or any(v < 0 or v + T > 2 ** 32 for v in f0)):
+            raise ValueError(f"frame0 needs {B} values with 0 <= frame0 and frame0 + {T} <= 2^32")
+        st_ = None if streams is None else [int(v) for v in streams]
+        if st_ is not None and (len(st_) != B or any(not 0 <= v < 2 ** 32 for v in st_)):
+            raise ValueError(f"streams needs {B} values in [0, 2^32)")
+        y = y.to(self.device, torch.float32).contiguous()
         y_lengths = y_lengths.to(self.device, torch.int64).contiguous()
         sid_src = self._expand_se(sid_src, B)
         sid_tgt = self._expand_se(sid_tgt, B)
@@ -202,21 +255,38 @@ class NativeSynthesizer:
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
         if noise is not None:
             noise = noise.to(self.device, torch.float32)
+        items = None
+        if seeds is not None or taus is not None or f0 is not None or st_ is not None:
+            dev = self.device
+            if seeds is not None and st_ is None:
+                st_ = [0] * B
+            items = {
+                "seed": None if seeds is None else torch.from_numpy(seed_array(seeds)).to(dev),
+                "stream": None if st_ is None else torch.tensor(st_, dtype=torch.int64, device=dev),
+                "frame0": None if f0 is None else torch.tensor(f0, dtype=torch.int64, device=dev),
+                "tau": None if taus is None else torch.tensor(taus, dtype=torch.float32, device=dev),
+            }
         o, lat = self.native.voice_conversion(y, y_lengths, sid_src, sid_tgt, noise=noise, tau=float(tau),
-                                              seed=seed or 0, ragged=ragged, latents=latents)
+                                              seed=seed or 0, ragged=ragged, latents=latents, items=items)
         y_mask = (torch.arange(T, device=self.device)[None, :] < y_lengths[:, None]).unsqueeze(1).to(torch.float32)
         return o, y_mask, lat
 
     @torch.no_grad()
     def infer(self, x, x_lengths, sid=None, noise_scale=1, length_scale=1, noise_scale_w=1.0, sdp_ratio=0.2,
               max_len=None, noise_w=None, noise=None, ragged: bool = False, seed: Optional[int] = None,
-              latents: bool = True):
+              latents: bool = True, seeds: Optional[Sequence[int]] = None, streams: Optional[Sequence[int]] = None):
         """(o, attn, y_mask, (z, z_p, None, None)) = SynthesizerTrn.infer (openvoice/models.py:467-490) for a V1
         base-speaker checkpoint.  ``x`` [B,T] token ids, ``x_lengths`` [B], ``sid`` [B] speaker ids.
         ``noise_w`` ([B,2,T]) / ``noise`` ([B,192,>=Ty]) replace the two random draws (models.py:173, 487); when None,
         Philox normals are drawn in-kernel from ``seed``.  The expanded m_p / logs_p of the reference's return
         tuple are not materialised (they only feed z_p).  One host sync, where the reference has one too
-        (y_lengths sizes every later tensor, models.py:476-478)."""
+        (y_lengths sizes every later tensor, models.py:476-478).
+
+        Per-item sampling (include/ovc.h: ovc_item_params): ``noise_scale``, ``length_scale``, ``noise_scale_w`` and
+        ``sdp_ratio`` each take one value per item as well as a scalar; ``seeds`` gives item b its own key (the
+        duration noise draws from ``seeds[b]``, the prior noise from ``seeds[b] + 1``, as a scalar ``seed`` does) at
+        stream ``streams[b]`` (default: b).  Sentence j of a call with ``seed=s`` is reproduced in any batch by
+        ``seeds[i] = s, streams[i] = j`` and the same parameters."""
         info = self.native.tts_info()
         if not info["has_tts"]:
             raise RuntimeError("this checkpoint has no enc_p / dp / sdp / emb_g: infer() needs a V1 base speaker")
@@ -232,18 +302,37 @@ class NativeSynthesizer:
         if int(sid.min()) < 0 or int(sid.max()) >= info["n_speakers"]:
             raise ValueError(f"speaker ids must lie in [0, {info['n_speakers']})")
         sid = sid.to(self.device).contiguous()
+        seeds = check_seeds(seeds, B)
+        if streams is not None:
+            streams = [int(v) for v in streams]
+            if len(streams) != B or any(not 0 <= v < 2 ** 32 for v in streams):
+                raise ValueError(f"streams needs {B} values in [0, 2^32)")
+        noise_scale, ns_b = check_per_item(noise_scale, B, "noise_scale")
+        length_scale, ls_b = check_per_item(length_scale, B, "length_scale", positive=True)
+        noise_scale_w, nsw_b = check_per_item(noise_scale_w, B, "noise_scale_w")
+        sdp_ratio, sr_b = check_per_item(sdp_ratio, B, "sdp_ratio")
         if seed is None:
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
         if noise_w is not None:
             noise_w = noise_w.to(self.device, torch.float32)
+        dev = self.device
+        f32 = lambda v: None if v is None else torch.tensor(v, dtype=torch.float32, device=dev)  # noqa: E731
+        key = None if seeds is None else torch.from_numpy(seed_array(seeds)).to(dev)
+        key1 = None if seeds is None else torch.from_numpy(seed_array([s + 1 for s in seeds])).to(dev)
+        stream_d = None if streams is None else torch.tensor(streams, dtype=torch.int64, device=dev)
+        enc_items = dec_items = None
+        if any(v is not None for v in (seeds, streams, nsw_b, ls_b, sr_b, ns_b)):
+            enc_items = {"seed": key, "stream": stream_d, "noise_scale_w": f32(nsw_b), "length_scale": f32(ls_b),
+                         "sdp_ratio": f32(sr_b)}
+            dec_items = {"seed": key1, "stream": stream_d, "noise_scale": f32(ns_b)}
         y_lengths, w_ceil, _ = self.native.tts_encode(x, x_lengths, sid, noise_w=noise_w, seed=seed,
                                                       noise_scale_w=float(noise_scale_w), length_scale=float(length_scale),
-                                                      sdp_ratio=float(sdp_ratio))
+                                                      sdp_ratio=float(sdp_ratio), items=enc_items)
         Ty = int(y_lengths.max().item())                       # the sync
         if noise is not None:
             noise = noise.to(self.device, torch.float32)[:, :, :Ty].contiguous()
         o, lat = self.native.tts_decode(B, Ty, self.device, noise=noise, seed=seed + 1, noise_scale=float(noise_scale),
-                                        ragged=ragged, latents=latents, max_len=max_len)
+                                        ragged=ragged, latents=latents, max_len=max_len, items=dec_items)
         ar = torch.arange(Ty, device=self.device)
         y_mask = (ar[None, :] < y_lengths[:, None]).unsqueeze(1).to(torch.float32)
         cum = torch.cumsum(w_ceil, 1)                          # commons.generate_path (commons.py:128-142)
@@ -325,36 +414,84 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
             seqs.append(ids)
         return seqs
 
+    def _sentences(self, text, language):
+        mark = self.language_marks.get(language.lower(), None)
+        assert mark is not None, f"language {language} is not supported"
+        frontend = self.text_frontend or self._reference_frontend
+        return frontend(text, mark)
+
     @torch.no_grad()
-    def tts_from_ids(self, sequences, speaker, speed=1.0, noise_scale=0.667, noise_scale_w=0.6, sdp_ratio=0.2,
-                     seed: Optional[int] = None) -> List[np.ndarray]:
-        """All sentences in ONE batched infer() (the reference loops over them at batch 1, api.py:79-91); every
-        sentence gets what its own batch-1 call would give (ragged decode)."""
-        speaker_id = self.hps.speakers[speaker] if isinstance(speaker, str) else int(speaker)
+    def tts_batch(self, requests: Sequence[dict]) -> List[np.ndarray]:
+        """Many TTS requests in ONE ragged ``infer``, each with its own speaker, speed, seed and noise parameters.
+        A request is a dict: ``ids`` (list of token-id lists, one per sentence) or ``text`` (+ ``language``, default
+        "English", through the text front end), ``speaker``, and optionally ``speed`` (1.0), ``seed`` (default: one
+        drawn from torch's global generator), ``noise_scale`` (0.667), ``noise_scale_w`` (0.6), ``sdp_ratio`` (0.2).
+        Sentence j of request r draws at (seed_r, stream j) with request r's parameters, so each returned array equals
+        ``audio_numpy_concat(tts_from_ids(ids, speaker, speed=..., seed=seed_r, ...), sr, speed)`` bit for bit: the
+        sentences joined with 50 ms / speed gaps, as ``tts`` does.  Returns one array per request."""
+        reqs = list(requests)
+        seqs, sid, seeds, streams, owner = [], [], [], [], []
+        par = {"noise_scale": [], "noise_scale_w": [], "length_scale": [], "sdp_ratio": []}
+        speeds = []
+        for r, q in enumerate(reqs):
+            ids = q["ids"] if "ids" in q else self._sentences(q["text"], q.get("language", "English"))
+            spk = q["speaker"]
+            spk = self.hps.speakers[spk] if isinstance(spk, str) else int(spk)
+            speed = float(q.get("speed", 1.0))
+            if not (math.isfinite(speed) and speed > 0):
+                raise ValueError(f"request {r}: speed {speed!r} must be a positive number")
+            seed = q.get("seed")
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None else check_seeds([seed], 1, "seed")[0]
+            speeds.append(speed)
+            for j, q_ids in enumerate(ids):
+                seqs.append(list(q_ids))
+                sid.append(spk)
+                seeds.append(seed)
+                streams.append(j)
+                owner.append(r)
+                par["noise_scale"].append(float(q.get("noise_scale", 0.667)))
+                par["noise_scale_w"].append(float(q.get("noise_scale_w", 0.6)))
+                par["length_scale"].append(1.0 / speed)
+                par["sdp_ratio"].append(float(q.get("sdp_ratio", 0.2)))
+        sr = self.hps.data.sampling_rate
+        audio = self._infer_sentences(seqs, sid, seeds=seeds, streams=streams, **par) if seqs else []
+        per: List[List[np.ndarray]] = [[] for _ in reqs]
+        for r, a in zip(owner, audio):
+            per[r].append(a)
+        return [self.audio_numpy_concat(per[r], sr=sr, speed=speeds[r]) for r in range(len(reqs))]
+
+    def _infer_sentences(self, sequences, sid, **kw) -> List[np.ndarray]:
+        """One ragged infer over token-id lists with per-sentence speaker ids; each sentence's samples."""
         n = len(sequences)
-        if n == 0:      # the reference's loop over zero sentences yields no audio (api.py:79-91)
-            return []
         T = max(len(q) for q in sequences)
         x = torch.zeros(n, T, dtype=torch.int64)
         for i, q in enumerate(sequences):
             x[i, :len(q)] = torch.as_tensor(q, dtype=torch.int64)
         lens = torch.tensor([len(q) for q in sequences], dtype=torch.int64)
-        sid = torch.full((n,), speaker_id, dtype=torch.int64)
-        o, _, y_mask, _ = self.model.infer(x, lens, sid=sid, noise_scale=noise_scale, noise_scale_w=noise_scale_w,
-                                           length_scale=1.0 / speed, sdp_ratio=sdp_ratio, ragged=True, seed=seed,
-                                           latents=False)
+        o, _, y_mask, _ = self.model.infer(x, lens, sid=torch.as_tensor(sid, dtype=torch.int64), ragged=True,
+                                           latents=False, **kw)
         frames = y_mask[:, 0].sum(1).long().cpu()
         o = o[:, 0].float().cpu().numpy()
         hop = self.hps.data.hop_length
         return [o[i, : int(frames[i]) * hop].copy() for i in range(n)]
 
-    def tts(self, text, output_path, speaker, language="English", speed=1.0):
-        """openvoice/api.py:73-98."""
-        mark = self.language_marks.get(language.lower(), None)
-        assert mark is not None, f"language {language} is not supported"
-        frontend = self.text_frontend or self._reference_frontend
-        sequences = frontend(text, mark)
-        audio_list = self.tts_from_ids(sequences, speaker, speed=speed)
+    @torch.no_grad()
+    def tts_from_ids(self, sequences, speaker, speed=1.0, noise_scale=0.667, noise_scale_w=0.6, sdp_ratio=0.2,
+                     seed: Optional[int] = None) -> List[np.ndarray]:
+        """All sentences in ONE batched infer() (the reference loops over them at batch 1, api.py:79-91); every
+        sentence gets what its own batch-1 call would give (ragged decode).  ``seed``: the call's key (sentence j
+        draws at stream j); default: one drawn from torch's global generator."""
+        speaker_id = self.hps.speakers[speaker] if isinstance(speaker, str) else int(speaker)
+        n = len(sequences)
+        if n == 0:      # the reference's loop over zero sentences yields no audio (api.py:79-91)
+            return []
+        return self._infer_sentences(sequences, [speaker_id] * n, noise_scale=noise_scale, noise_scale_w=noise_scale_w,
+                                     length_scale=1.0 / speed, sdp_ratio=sdp_ratio, seed=seed)
+
+    def tts(self, text, output_path, speaker, language="English", speed=1.0, seed: Optional[int] = None):
+        """openvoice/api.py:73-98.  ``seed``: the request's key (``tts_from_ids``); same seed, same audio."""
+        sequences = self._sentences(text, language)
+        audio_list = self.tts_from_ids(sequences, speaker, speed=speed, seed=seed)
         audio = self.audio_numpy_concat(audio_list, sr=self.hps.data.sampling_rate, speed=speed)
         if output_path is None:
             return audio
@@ -472,20 +609,23 @@ class ToneColorConverter(OpenVoiceBaseClass):
 
     # ------------------------------------------------------------------ conversion
     def convert(self, audio_src_path, src_se, tgt_se, output_path=None, tau=0.3, message="default",
-                noise=None, sr: Optional[int] = None):
+                noise=None, sr: Optional[int] = None, seed: Optional[int] = None):
         """openvoice/api.py:141-160.  Returns float32 samples (256 * (L // 256) of them) or writes
         ``output_path``.  ``noise`` ([1,192,T]) optionally replaces the random draw (tests).  ``sr``: rate of a NumPy
-        waveform that is not at the model's rate (see ``convert_batch``)."""
+        waveform that is not at the model's rate (see ``convert_batch``).  ``seed``: the request's own noise key
+        (see ``convert_batch``'s ``seeds``): the same seed reproduces the same audio in any batch, stream or window."""
         audio = self.convert_batch([audio_src_path], src_se, tgt_se, tau=tau, messages=[message],
-                                   noise=None if noise is None else [noise], sr=sr)[0]
+                                   noise=None if noise is None else [noise], sr=sr,
+                                   seeds=None if seed is None else [seed])[0]
         if output_path is None:
             return audio
         _write_audio(output_path, audio, self.hps.data.sampling_rate)
 
     @torch.no_grad()
-    def convert_batch(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: float = 0.3,
+    def convert_batch(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: Union[float, Sequence[float]] = 0.3,
                       messages: Optional[Sequence[str]] = None, noise: Optional[Sequence] = None,
-                      max_batch: int = 64, sr: Optional[int] = None) -> List[np.ndarray]:
+                      max_batch: int = 64, sr: Optional[int] = None,
+                      seeds: Optional[Sequence[int]] = None) -> List[np.ndarray]:
         """Convert a list of utterances (paths or waveforms at the model sampling rate); every item
         gets exactly what ``convert`` would return for it alone.  ``src_se`` / ``tgt_se`` are either
         one [1,gin,1] embedding for all items or a sequence of per-item embeddings.
@@ -493,9 +633,20 @@ class ToneColorConverter(OpenVoiceBaseClass):
         ``sr``: sampling rate of the NumPy waveform items when it is not the model's.  They are uploaded as they are
         and resampled on the device (``scipy.signal.resample_poly`` arithmetic, within one fp32 ulp of it) into the
         buffer the spectrogram reads; the output stays at the model's rate, as in the reference.  A file path item with
-        ``sr`` is refused (files are decoded and resampled on load); so is a rate pair the resampler does not take."""
+        ``sr`` is refused (files are decoded and resampled on load); so is a rate pair the resampler does not take.
+
+        ``tau``: one value for all items or one per item.  ``seeds``: one Philox key per item, in [0, 2^64).  Item i
+        then draws its noise from ``seeds[i]`` alone (include/ovc.h: ovc_item_params, stream 0), so its audio equals
+        ``convert(audios[i], seed=seeds[i], tau=tau_i)`` bit for bit wherever it sits: batch order, ``max_batch``,
+        ``convert_concurrent``, sharding.  Without ``seeds`` one key drawn from torch's global generator serves the
+        call, as in the reference's ``randn_like``.  ``seeds`` with ``noise``, a length that is not ``len(audios)``
+        or an invalid value raises ValueError before anything is launched."""
         hps = self.hps
         n = len(audios)
+        tau, taus = check_per_item(tau, n, "tau")
+        seeds = check_seeds(seeds, n)
+        if noise is not None and seeds is not None:
+            raise ValueError("pass either noise or seeds, not both")
         rate = self._input_rate(audios, sr)
         waves = [_load_audio(a, hps.data.sampling_rate) for a in audios]
         src = self._stack_se(src_se, n)
@@ -505,8 +656,10 @@ class ToneColorConverter(OpenVoiceBaseClass):
         hop = hps.data.hop_length
         for lo in range(0, n, max_batch):
             idx = order[lo: lo + max_batch]
-            res = self._convert_chunk([waves[i] for i in idx], src[idx], tgt[idx], tau,
-                                      None if noise is None else [noise[i] for i in idx], rate)
+            res = self._convert_chunk([waves[i] for i in idx], src[idx], tgt[idx],
+                                      tau if taus is None else [taus[i] for i in idx],
+                                      None if noise is None else [noise[i] for i in idx], rate,
+                                      None if seeds is None else [seeds[i] for i in idx])
             for i, a in zip(idx, res):
                 msg = messages[i] if messages is not None else "default"
                 out[i] = self.add_watermark(a, msg)
@@ -514,14 +667,17 @@ class ToneColorConverter(OpenVoiceBaseClass):
 
     # ------------------------------------------------------------------ one utterance per stream
     @torch.no_grad()
-    def convert_concurrent(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: float = 0.3, streams: int = 4,
-                           messages: Optional[Sequence[str]] = None, sr: Optional[int] = None) -> List[np.ndarray]:
+    def convert_concurrent(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: Union[float, Sequence[float]] = 0.3,
+                           streams: int = 4, messages: Optional[Sequence[str]] = None, sr: Optional[int] = None,
+                           seeds: Optional[Sequence[int]] = None) -> List[np.ndarray]:
         """Serve many SMALL independent requests: utterance i runs alone (batch 1, exactly ``convert``) on CUDA
         stream ``i % streams``, each stream with its own converter replica (context + workspace), so the
         latency-bound kernels of different requests overlap on the GPU -- north_star's "one utterance per stream".
-        For large batches ``convert_batch`` (one launch sequence for the whole batch) is the faster path.  ``sr`` as in
-        ``convert_batch``."""
+        For large batches ``convert_batch`` (one launch sequence for the whole batch) is the faster path.  ``sr``,
+        ``tau`` (scalar or per item) and ``seeds`` as in ``convert_batch``."""
         n = len(audios)
+        tau, taus = check_per_item(tau, n, "tau")
+        seeds = check_seeds(seeds, n)
         rate = self._input_rate(audios, sr)
         src = self._stack_se(src_se, n)
         tgt = self._stack_se(tgt_se, n)
@@ -535,7 +691,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
                 conv, stream = reps[j % S]
                 with torch.cuda.stream(stream):
                     pending.append(conv._enqueue_single(_load_audio(audios[i], self.hps.data.sampling_rate), src[i: i + 1],
-                                                        tgt[i: i + 1], tau, j // S, rate))
+                                                        tgt[i: i + 1], tau if taus is None else taus[i], j // S, rate,
+                                                        None if seeds is None else seeds[i]))
             for _, stream in reps:
                 stream.synchronize()
             for i, (host, n_samples) in zip(wave, pending):
@@ -554,10 +711,11 @@ class ToneColorConverter(OpenVoiceBaseClass):
             reps.append((twin, torch.cuda.Stream(device=self.device)))
         return reps[:count]
 
-    def _enqueue_single(self, wave, src, tgt, tau, slot, sr=None):
+    def _enqueue_single(self, wave, src, tgt, tau, slot, sr=None, seed=None):
         """Asynchronous batch-1 conversion on the current stream, staging through pinned slot ``slot``;
         returns (pinned host buffer, samples).  The caller synchronises the stream before reading / reusing it.
-        ``sr``: the wave's rate when it is not the model's (``_input_rate``): resampled on the device after upload."""
+        ``sr``: the wave's rate when it is not the model's (``_input_rate``): resampled on the device after upload.
+        ``seed``: the request's own key (stream 0), else one drawn from torch's global generator."""
         hop = self.hps.data.hop_length
         dev = self.device
         L = self._resampled_len(len(wave), sr)
@@ -570,8 +728,9 @@ class ToneColorConverter(OpenVoiceBaseClass):
             wav = self.model.native.resample(wav, torch.tensor([len(wave)], dtype=torch.int64, device=dev), sr,
                                              self.hps.data.sampling_rate)
         wlen = torch.tensor([L], dtype=torch.int64, device=dev)
+        items = None if seed is None else self._item_arrays(f"c{slot}", [seed], None)
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        o, _ = self.model.native.convert_waveform(wav, wlen, src, tgt, tau=float(tau), seed=seed)
+        o, _ = self.model.native.convert_waveform(wav, wlen, src, tgt, tau=float(tau), seed=seed, items=items)
         host = self._pinned(f"cout{slot}", o.numel())
         host.copy_(o.view(-1), non_blocking=True)
         return host, (L // hop) * hop
@@ -583,13 +742,20 @@ class ToneColorConverter(OpenVoiceBaseClass):
 
     @torch.no_grad()
     def convert_long(self, audio_src_path, src_se, tgt_se, output_path=None, tau=0.3, message="default",
-                     window_frames: int = 2048, noise=None, max_batch: int = 32, sr: Optional[int] = None):
+                     window_frames: int = 2048, noise=None, max_batch: int = 32, sr: Optional[int] = None,
+                     seed: Optional[int] = None):
         """Row f4 (time-tiled execution): convert a clip of any length with bounded memory.  The spectrogram is
         cut into windows of ``window_frames`` frames plus a halo of the path's receptive field on both sides; the
         windows run as one ragged batch and only their interiors are kept, so the result equals ``convert`` on the
         whole clip (same noise tensor: drawn once for the whole clip, or passed as ``noise`` [192, T]).  ``sr``: rate of
-        a NumPy waveform that is not at the model's; it is resampled on the device first (see ``convert_batch``)."""
+        a NumPy waveform that is not at the model's; it is resampled on the device first (see ``convert_batch``).
+        ``seed``: the request's own key; each window then draws the whole clip's noise at its absolute frames in-kernel
+        (frame0 = the window's first frame), so the result matches ``convert(seed=seed)`` and no noise tensor is
+        built.  ``seed`` with ``noise`` raises ValueError."""
         hps = self.hps
+        seed = None if seed is None else check_seeds([seed], 1, "seed")[0]
+        if seed is not None and noise is not None:
+            raise ValueError("pass either noise or seed, not both")
         hop, dev = hps.data.hop_length, self.device
         rate = self._input_rate([audio_src_path], sr)
         wav = torch.from_numpy(_load_audio(audio_src_path, hps.data.sampling_rate)).to(dev)
@@ -600,11 +766,12 @@ class ToneColorConverter(OpenVoiceBaseClass):
         spec, _ = self.model.native.spectrogram(wav[None].contiguous(), torch.tensor([L], dtype=torch.int64, device=dev))
         T = spec.shape[2]
         C = hps.model.inter_channels
-        if noise is None:
-            gen = torch.Generator(device=dev)
-            gen.manual_seed(int(torch.randint(0, 2 ** 62, (1,)).item()))
-            noise = torch.randn(C, T, device=dev, generator=gen)
-        noise = noise.to(dev, torch.float32).reshape(C, T)
+        if seed is None:
+            if noise is None:
+                gen = torch.Generator(device=dev)
+                gen.manual_seed(int(torch.randint(0, 2 ** 62, (1,)).item()))
+                noise = torch.randn(C, T, device=dev, generator=gen)
+            noise = noise.to(dev, torch.float32).reshape(C, T)
         H = self.HALO_FRAMES
         starts = list(range(0, T, window_frames))
         wins = [(max(0, s - H), min(T, s + window_frames + H), s, min(T, s + window_frames)) for s in starts]
@@ -616,13 +783,15 @@ class ToneColorConverter(OpenVoiceBaseClass):
             chunk = wins[i0: i0 + max_batch]
             B = len(chunk)
             sp = torch.zeros(B, spec.shape[1], Wmax, device=dev)
-            nz = torch.zeros(B, C, Wmax, device=dev)
+            nz = None if seed is not None else torch.zeros(B, C, Wmax, device=dev)
             for b, (lo, hi, _, _) in enumerate(chunk):
                 sp[b, :, : hi - lo] = spec[0, :, lo:hi]
-                nz[b, :, : hi - lo] = noise[:, lo:hi]
+                if nz is not None:
+                    nz[b, :, : hi - lo] = noise[:, lo:hi]
             lens = torch.tensor([hi - lo for lo, hi, _, _ in chunk], dtype=torch.int64, device=dev)
+            keyed = {} if seed is None else dict(seeds=[seed] * B, frame0=[lo for lo, _, _, _ in chunk])
             o, _, _ = self.model.voice_conversion(sp, lens, src.expand(B, -1), tgt.expand(B, -1), tau=tau, noise=nz,
-                                                  ragged=True, latents=False)
+                                                  ragged=True, latents=False, **keyed)
             for b, (lo, hi, s, e) in enumerate(chunk):
                 out[s * hop: e * hop] = o[b, 0, (s - lo) * hop: (e - lo) * hop]
         audio = self.add_watermark(out.cpu().numpy(), message)
@@ -658,10 +827,11 @@ class ToneColorConverter(OpenVoiceBaseClass):
         assert se.shape[0] == n, "one speaker embedding per utterance (or a single one for all)"
         return se
 
-    def _enqueue_chunk(self, waves, src, tgt, tau, noise, slot=0, sr=None):
+    def _enqueue_chunk(self, waves, src, tgt, tau, noise, slot=0, sr=None, seeds=None):
         """Stage, upload and launch one ragged batch on the current stream WITHOUT synchronising the host.
         Returns (o [B, 256 * Tmax] on the device, frames per item).  ``sr``: the waves' rate when it is not the
-        model's (``_input_rate``): the raw samples are uploaded and resampled on the device into the slot's buffer."""
+        model's (``_input_rate``): the raw samples are uploaded and resampled on the device into the slot's buffer.
+        ``tau``: a float or one per item; ``seeds``: None or one key per item (validated by the caller)."""
         hps = self.hps
         hop = hps.data.hop_length
         B = len(waves)
@@ -714,6 +884,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
         src_d.copy_(src.reshape(B, -1), non_blocking=True)
         tgt_d = self._dev(f"tgt{slot}", tgt.numel(), torch.float32).view(B, -1)
         tgt_d.copy_(tgt.reshape(B, -1), non_blocking=True)
+        taus = None if np.ndim(tau) == 0 else list(tau)
+        items = None if seeds is None and taus is None else self._item_arrays(f"b{slot}", seeds, taus)
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(dev))
         self._h2d_done[slot] = ev
@@ -727,14 +899,36 @@ class ToneColorConverter(OpenVoiceBaseClass):
                 nz[b, :, : q.shape[1]] = q.to(dev)
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())
         # spectrogram + voice_conversion, every item at its own exact length (api.py:148-154)
-        o, _ = self.model.native.convert_waveform(wav, wlen, src_d, tgt_d, noise=nz, tau=float(tau), seed=seed,
+        o, _ = self.model.native.convert_waveform(wav, wlen, src_d, tgt_d, noise=nz,
+                                                  tau=float(tau) if taus is None else taus[0], seed=seed,
                                                   out=self._dev(f"out{slot}", B * (Lmax // hop) * hop, torch.float32),
-                                                  frames_out=self._dev(f"fr{slot}", B, torch.int64))
+                                                  frames_out=self._dev(f"fr{slot}", B, torch.int64), items=items)
         return o.view(B, -1), frames
 
-    def _convert_chunk(self, waves, src, tgt, tau, noise, sr=None):
+    def _item_arrays(self, slot, seeds, taus) -> dict:
+        """Per-item parameter arrays of one call, staged through pinned buffers into device buffers that stay at the
+        slot's addresses (a repeated call is still replayed from its CUDA graph, with the new values).  Seeded items draw
+        at stream 0.  The caller restages a slot only after the previous call on it has consumed its upload."""
+        B = len(seeds) if seeds is not None else len(taus)
+        items = {}
+        if seeds is not None:
+            pin = self._pinned_i64(f"iseed{slot}", 2 * B)
+            pin[:B].copy_(torch.from_numpy(seed_array(seeds)))
+            pin[B:].zero_()
+            d = self._dev(f"iseed{slot}", 2 * B, torch.int64)
+            d.copy_(pin, non_blocking=True)
+            items["seed"], items["stream"] = d[:B], d[B:]
+        if taus is not None:
+            pin = self._pinned(f"itau{slot}", B)
+            pin.copy_(torch.tensor(taus, dtype=torch.float32))
+            d = self._dev(f"itau{slot}", B, torch.float32)
+            d.copy_(pin, non_blocking=True)
+            items["tau"] = d
+        return items
+
+    def _convert_chunk(self, waves, src, tgt, tau, noise, sr=None, seeds=None):
         hop = self.hps.data.hop_length
-        o, frames = self._enqueue_chunk(waves, src, tgt, tau, noise, sr=sr)
+        o, frames = self._enqueue_chunk(waves, src, tgt, tau, noise, sr=sr, seeds=seeds)
         host = self._pinned("out", o.numel()).view(o.shape)
         host.copy_(o, non_blocking=True)
         torch.cuda.current_stream(self.device).synchronize()
@@ -742,17 +936,20 @@ class ToneColorConverter(OpenVoiceBaseClass):
         return _parallel(lambda b: audio[b, : frames[b] * hop].copy(), len(waves))
 
     @torch.no_grad()
-    def convert_batch_device(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: float = 0.3, slot: int = 0,
-                             sr: Optional[int] = None):
+    def convert_batch_device(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: Union[float, Sequence[float]] = 0.3,
+                             slot: int = 0, sr: Optional[int] = None, seeds: Optional[Sequence[int]] = None):
         """``convert_batch`` up to the device: stages and launches ONE ragged batch asynchronously on the current
         stream and returns (o [n, max samples] float32 on the device, samples per item).  No host synchronisation,
         no device -> host copy: the building block of ``distributed.convert_sharded_async`` (waveforms gathered
         GPU-to-GPU over NCCL) and of pipelined serving.  ``slot`` picks the pinned upload buffer (alternate 0 / 1
-        between in-flight calls).  ``sr`` as in ``convert_batch``."""
+        between in-flight calls).  ``sr``, ``tau`` (scalar or per item) and ``seeds`` as in ``convert_batch``."""
+        n = len(audios)
+        tau, taus = check_per_item(tau, n, "tau")
+        seeds = check_seeds(seeds, n)
         rate = self._input_rate(audios, sr)
         waves = [_load_audio(a, self.hps.data.sampling_rate) for a in audios]
-        n = len(waves)
-        o, frames = self._enqueue_chunk(waves, self._stack_se(src_se, n), self._stack_se(tgt_se, n), tau, None, slot, rate)
+        o, frames = self._enqueue_chunk(waves, self._stack_se(src_se, n), self._stack_se(tgt_se, n),
+                                        tau if taus is None else taus, None, slot, rate, seeds)
         hop = self.hps.data.hop_length
         return o, [f * hop for f in frames]
 

@@ -39,8 +39,15 @@ enum EpiKind : int {
 
 enum : int { F_ACCUM = 1, F_FIRST = 2 };
 
+// Per-item overrides of a call's noise key and scalars, one [B] device array each, NULL = the call's value (the layout
+// of include/ovc.h's ovc_item_params).  The kernels read them at run time, so new contents need no new launch sequence.
+struct ItemParams {
+  const unsigned long long* seed; const long long* stream; const long long* frame0;
+  const float* tau; const float* noise_scale; const float* noise_scale_w; const float* length_scale; const float* sdp_ratio;
+};
+
 // per-call scalars that live in device memory so that a captured launch sequence (CUDA graph) can be replayed with new values
-struct CallParams { unsigned long long seed; float tau; float pad; };
+struct CallParams { unsigned long long seed; float tau; float pad; ItemParams items; };
 
 struct ConvArgs {
   // input activations, [B][cin][x_pitch] (time fastest)
@@ -123,8 +130,13 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 __device__ __forceinline__ float lrelu(float v, float slope) { return v > 0.f ? v : v * slope; }
 __device__ __forceinline__ float sigmoidf_acc(float v) { return 1.f / (1.f + expf(-v)); }
 
-// Philox4x32-10 -> one standard normal per (b, channel, t) counter (used when no explicit noise
-// tensor is supplied; the reference draws torch.randn_like at models.py:220).
+// Philox4x32-10 -> one standard normal per counter (used when no explicit noise tensor is supplied; the reference draws
+// torch.randn_like at models.py:220).  Counter layout of every in-kernel draw:
+//   key = seed (64 bits), x0 = stream, x1 = channel, x2 = frame, x3 = 0x0B200
+// A call without per-item keys draws item b's enc_q noise with stream = b and frame = t; with ovc_item_params the key,
+// stream and frame offset come from the item: stream = stream[b], frame = (frame0[b] + t) mod 2^32.  TTS: the
+// noise_w rows use channels 0x7700 / 0x7701 (key = the encode seed), the z_p noise channels 0..inter-1 (key = the
+// decode seed).  ovc_philox_normals writes the same draws into a tensor.
 __device__ __forceinline__ float philox_normal(unsigned long long seed, uint32_t c0, uint32_t c1, uint32_t c2) {
   uint32_t k0 = static_cast<uint32_t>(seed), k1 = static_cast<uint32_t>(seed >> 32);
   uint32_t x0 = c0, x1 = c1, x2 = c2, x3 = 0x0B200u;
@@ -455,8 +467,16 @@ __global__ void __launch_bounds__(C::THREADS, C::MIN_BLOCKS) conv1d_f32(const Co
     const int ch0 = row0 / 2;
     float* yb = a.y + (size_t)b * a.y_bs;
     const float* nb = a.r ? a.r + (size_t)b * a.r_bs : nullptr;
-    const unsigned long long seed = a.callp ? a.callp->seed : a.seed;
-    const float tau = a.callp ? a.callp->tau : a.tau;
+    unsigned long long seed = a.callp ? a.callp->seed : a.seed;
+    float tau = a.callp ? a.callp->tau : a.tau;
+    uint32_t stream = (uint32_t)b, f0 = 0u;
+    if (a.callp) {
+      const ItemParams& it = a.callp->items;
+      if (it.seed) seed = it.seed[b];
+      if (it.stream) stream = (uint32_t)it.stream[b];
+      if (it.frame0) f0 = (uint32_t)it.frame0[b];
+      if (it.tau) tau = it.tau[b];
+    }
 #pragma unroll
     for (int c = 0; c < 2; ++c) {
       const int t = t0 + tb + 32 * c;
@@ -468,7 +488,7 @@ __global__ void __launch_bounds__(C::THREADS, C::MIN_BLOCKS) conv1d_f32(const Co
             const float m = acc[c][r][j] + bias[r];
             const float logs = acc[c][r + 4][j] + bias[r + 4];
             const float nz = nb ? nb[(size_t)(ch0 + r) * a.r_pitch + t + j]
-                                : philox_normal(seed, (uint32_t)b, (uint32_t)(ch0 + r), (uint32_t)(t + j));
+                                : philox_normal(seed, stream, (uint32_t)(ch0 + r), f0 + (uint32_t)(t + j));
             yb[(size_t)(ch0 + r) * a.y_pitch + t + j] = m + nz * tau * expf(logs);
           }
         }

@@ -1025,9 +1025,23 @@ static void drop_graphs(ovc_ctx* c) {
   c->graphs.clear();
 }
 
-__global__ void set_call_params_kernel(CallParams* p, unsigned long long seed, float tau) {
+__global__ void set_call_params_kernel(CallParams* p, unsigned long long seed, float tau, ItemParams items) {
   p->seed = seed;
   p->tau = tau;
+  p->items = items;
+}
+
+static_assert(sizeof(ItemParams) == sizeof(ovc_item_params), "ItemParams mirrors ovc_item_params");
+static ItemParams item_params(const ovc_item_params* p) {   // NULL -> every field NULL
+  ItemParams r{};
+  if (p) memcpy(&r, p, sizeof r);
+  return r;
+}
+static void append_item_key(std::vector<uintptr_t>& key, const ItemParams& it) {
+  for (const void* q : {(const void*)it.seed, (const void*)it.stream, (const void*)it.frame0, (const void*)it.tau,
+                        (const void*)it.noise_scale, (const void*)it.noise_scale_w, (const void*)it.length_scale,
+                        (const void*)it.sdp_ratio})
+    key.push_back((uintptr_t)q);
 }
 
 // Run `body(stream)` -- a pure launch sequence -- directly, or replay it from a CUDA graph when the same signature `key`
@@ -1087,9 +1101,9 @@ static int run_graphed(ovc_ctx* c, const std::vector<uintptr_t>& key, cudaStream
   return OVC_OK;
 }
 
-static int set_call_params(ovc_ctx* c, uint64_t seed, float tau, cudaStream_t st) {
+static int set_call_params(ovc_ctx* c, uint64_t seed, float tau, const ItemParams& items, cudaStream_t st) {
   if (!c->d_callp) CK(cudaMalloc(&c->d_callp, sizeof(CallParams)));
-  set_call_params_kernel<<<1, 1, 0, st>>>(c->d_callp, seed, tau);
+  set_call_params_kernel<<<1, 1, 0, st>>>(c->d_callp, seed, tau, items);
   CK(cudaGetLastError());
   return OVC_OK;
 }
@@ -1364,7 +1378,7 @@ static int run_vc(ovc_ctx* c, const float* spec, int spec_pitch, const long long
     p.r = noise; p.r_bs = 192LL * Tmax; p.r_pitch = Tmax;
     p.lens_in = lens; p.lens_out = lens; p.mul_in = 1; p.mul_out = 1;
     p.slope = 1.f; p.tau = tau; p.seed = seed;
-    p.callp = c->d_callp;       // set_call_params_kernel wrote (seed, tau) there earlier on this stream
+    p.callp = c->d_callp;       // set_call_params_kernel wrote (seed, tau, per-item arrays) there earlier on this stream
     TRY(launch(r, c->enc_proj, p, Tmax));
   }
   auto copy_latent = [&](float* dst) -> int { return copy_latent_out(r, W, ws, dst); };
@@ -1469,6 +1483,13 @@ size_t ovc_workspace_floats(const ovc_ctx* c, int B, int Tmax) {
 int ovc_voice_conversion(ovc_ctx* c, const float* spec, const int64_t* lengths, const float* g_src, const float* g_tgt,
                          const float* noise, uint64_t seed, float tau, int B, int Tmax, int ragged, float* o_hat, float* z,
                          float* z_p, float* z_hat, void* stream) {
+  return ovc_voice_conversion_items(c, spec, lengths, g_src, g_tgt, noise, seed, tau, B, Tmax, ragged, o_hat, z, z_p, z_hat,
+                                    stream, nullptr);
+}
+
+int ovc_voice_conversion_items(ovc_ctx* c, const float* spec, const int64_t* lengths, const float* g_src, const float* g_tgt,
+                               const float* noise, uint64_t seed, float tau, int B, int Tmax, int ragged, float* o_hat,
+                               float* z, float* z_p, float* z_hat, void* stream, const ovc_item_params* items) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
   if (!spec || !lengths || !g_src || !g_tgt || !o_hat) return fail(OVC_ERR_INVALID, "null tensor argument");
@@ -1479,10 +1500,12 @@ int ovc_voice_conversion(ovc_ctx* c, const float* spec, const int64_t* lengths, 
   c->ev_used = c->prof ? c->ev_used : 0;
   cudaStream_t st = (cudaStream_t)stream;
   TRY(ensure_ws(c, ws_layout(c, B, Tmax), B, Tmax, st));
-  TRY(set_call_params(c, seed, tau, st));
-  const std::vector<uintptr_t> key = {1, (uintptr_t)spec, (uintptr_t)lengths, (uintptr_t)g_src, (uintptr_t)g_tgt, (uintptr_t)noise,
-                                      (uintptr_t)o_hat, (uintptr_t)z, (uintptr_t)z_p, (uintptr_t)z_hat, (uintptr_t)B, (uintptr_t)Tmax,
-                                      (uintptr_t)ragged, option_bits(c)};
+  const ItemParams it = item_params(items);
+  TRY(set_call_params(c, seed, tau, it, st));
+  std::vector<uintptr_t> key = {1, (uintptr_t)spec, (uintptr_t)lengths, (uintptr_t)g_src, (uintptr_t)g_tgt, (uintptr_t)noise,
+                                (uintptr_t)o_hat, (uintptr_t)z, (uintptr_t)z_p, (uintptr_t)z_hat, (uintptr_t)B, (uintptr_t)Tmax,
+                                (uintptr_t)ragged, option_bits(c)};
+  append_item_key(key, it);
   return run_graphed(c, key, st, [&](cudaStream_t s) {
     return run_vc(c, spec, Tmax, (const long long*)lengths, g_src, g_tgt, noise, seed, tau, B, Tmax, ragged, o_hat, z, z_p, z_hat, s);
   });
@@ -1513,6 +1536,12 @@ int ovc_spectrogram(ovc_ctx* c, const float* wav, const int64_t* wav_lengths, in
 int ovc_convert_waveform(ovc_ctx* c, const float* wav, const int64_t* wav_lengths, int B, int Lmax, const float* g_src,
                          const float* g_tgt, const float* noise, uint64_t seed, float tau, float* o_hat, int64_t* frames,
                          void* stream) {
+  return ovc_convert_waveform_items(c, wav, wav_lengths, B, Lmax, g_src, g_tgt, noise, seed, tau, o_hat, frames, stream, nullptr);
+}
+
+int ovc_convert_waveform_items(ovc_ctx* c, const float* wav, const int64_t* wav_lengths, int B, int Lmax, const float* g_src,
+                               const float* g_tgt, const float* noise, uint64_t seed, float tau, float* o_hat, int64_t* frames,
+                               void* stream, const ovc_item_params* items) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
   if (!wav || !wav_lengths || !g_src || !g_tgt || !o_hat) return fail(OVC_ERR_INVALID, "null tensor argument");
@@ -1523,9 +1552,11 @@ int ovc_convert_waveform(ovc_ctx* c, const float* wav, const int64_t* wav_length
   cudaStream_t st = (cudaStream_t)stream;
   const WsLayout W = ws_layout(c, B, Tmax);
   TRY(ensure_ws(c, W, B, Tmax, st));
-  TRY(set_call_params(c, seed, tau, st));
-  const std::vector<uintptr_t> key = {2, (uintptr_t)wav, (uintptr_t)wav_lengths, (uintptr_t)g_src, (uintptr_t)g_tgt, (uintptr_t)noise,
-                                      (uintptr_t)o_hat, (uintptr_t)frames, (uintptr_t)B, (uintptr_t)Lmax, option_bits(c)};
+  const ItemParams it = item_params(items);
+  TRY(set_call_params(c, seed, tau, it, st));
+  std::vector<uintptr_t> key = {2, (uintptr_t)wav, (uintptr_t)wav_lengths, (uintptr_t)g_src, (uintptr_t)g_tgt, (uintptr_t)noise,
+                                (uintptr_t)o_hat, (uintptr_t)frames, (uintptr_t)B, (uintptr_t)Lmax, option_bits(c)};
+  append_item_key(key, it);
   return run_graphed(c, key, st, [&](cudaStream_t s) {
     float* spec = c->d_ws + W.spec;
     long long* fr = reinterpret_cast<long long*>(c->d_ws + W.frames);
@@ -1685,6 +1716,13 @@ int ovc_tts_info(const ovc_ctx* c, int32_t* out8) {
 int ovc_tts_encode(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid, const float* noise_w,
                    uint64_t seed, float noise_scale_w, float length_scale, float sdp_ratio, int B, int T, int64_t* y_lengths,
                    float* w_ceil, float* logw, void* stream) {
+  return ovc_tts_encode_items(c, tokens, x_lengths, sid, noise_w, seed, noise_scale_w, length_scale, sdp_ratio, B, T, y_lengths,
+                              w_ceil, logw, stream, nullptr);
+}
+
+int ovc_tts_encode_items(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid, const float* noise_w,
+                         uint64_t seed, float noise_scale_w, float length_scale, float sdp_ratio, int B, int T,
+                         int64_t* y_lengths, float* w_ceil, float* logw, void* stream, const ovc_item_params* items) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
   if (!c->tts.ready) return fail(OVC_ERR_STATE, "the checkpoint has no TTS members (enc_p / dp / sdp / emb_g): not a V1 base speaker");
@@ -1695,11 +1733,17 @@ int ovc_tts_encode(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, 
   ON_DEVICE(c);
   c->ev_used = c->prof ? c->ev_used : 0;
   return run_tts_encode(c, (const long long*)tokens, (const long long*)x_lengths, (const long long*)sid, noise_w, seed,
-                        noise_scale_w, length_scale, sdp_ratio, B, T, (long long*)y_lengths, w_ceil, logw, (cudaStream_t)stream);
+                        noise_scale_w, length_scale, sdp_ratio, B, T, (long long*)y_lengths, w_ceil, logw, item_params(items),
+                        (cudaStream_t)stream);
 }
 
 int ovc_tts_decode(ovc_ctx* c, const float* noise, uint64_t seed, float noise_scale, int B, int Ymax, int max_len, int ragged,
                    float* o, float* z, float* z_p, void* stream) {
+  return ovc_tts_decode_items(c, noise, seed, noise_scale, B, Ymax, max_len, ragged, o, z, z_p, stream, nullptr);
+}
+
+int ovc_tts_decode_items(ovc_ctx* c, const float* noise, uint64_t seed, float noise_scale, int B, int Ymax, int max_len,
+                         int ragged, float* o, float* z, float* z_p, void* stream, const ovc_item_params* items) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
   if (c->tts_B < 1) return fail(OVC_ERR_STATE, "ovc_tts_decode needs a preceding ovc_tts_encode");
@@ -1710,7 +1754,16 @@ int ovc_tts_decode(ovc_ctx* c, const float* noise, uint64_t seed, float noise_sc
   ON_DEVICE(c);
   c->ev_used = c->prof ? c->ev_used : 0;
   if (max_len < 0) return fail(OVC_ERR_INVALID, "max_len must be >= 0 (0 = no limit)");
-  return run_tts_decode(c, noise, seed, noise_scale, B, Ymax, max_len, ragged, o, z, z_p, (cudaStream_t)stream);
+  return run_tts_decode(c, noise, seed, noise_scale, B, Ymax, max_len, ragged, o, z, z_p, item_params(items),
+                        (cudaStream_t)stream);
+}
+
+int ovc_philox_normals(uint64_t seed, int64_t stream, int64_t c0, int C, int64_t frame0, int T, float* out, void* cuda_stream) {
+  if (!out || C < 1 || T < 1 || C > 65535) return fail(OVC_ERR_INVALID, "bad argument to ovc_philox_normals (C=%d, T=%d)", C, T);
+  philox_normals_kernel<<<dim3((T + 127) / 128, C), 128, 0, (cudaStream_t)cuda_stream>>>(
+      seed, (uint32_t)stream, (uint32_t)c0, (uint32_t)frame0, T, out);
+  CK(cudaGetLastError());
+  return OVC_OK;
 }
 
 int ovc_set_precision(ovc_ctx* c, int mode) {

@@ -284,12 +284,17 @@ __global__ void tts_cf_tail_kernel(const float* h, const long long* lens, const 
 }
 
 // z = noise_w * noise_scale_w (explicit) or Philox normals                       models.py:173        grid (ceil(T/128), B)
-__global__ void tts_noise_w_kernel(const float* noise_w, unsigned long long seed, float scale, int T, float* z0, float* z1) {
+// it.seed / it.stream / it.noise_scale_w, when set, replace the call's seed, stream b and scale for item b
+__global__ void tts_noise_w_kernel(const float* noise_w, unsigned long long seed, float scale, int T, float* z0, float* z1,
+                                   ItemParams it) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
   if (t >= T) return;
   const size_t o = (size_t)b * T + t;
-  z0[o] = (noise_w ? noise_w[((size_t)b * 2 + 0) * T + t] : philox_normal(seed, (uint32_t)b, 0x7700u, (uint32_t)t)) * scale;
-  z1[o] = (noise_w ? noise_w[((size_t)b * 2 + 1) * T + t] : philox_normal(seed, (uint32_t)b, 0x7701u, (uint32_t)t)) * scale;
+  if (it.seed) seed = it.seed[b];
+  const uint32_t stream = it.stream ? (uint32_t)it.stream[b] : (uint32_t)b;
+  if (it.noise_scale_w) scale = it.noise_scale_w[b];
+  z0[o] = (noise_w ? noise_w[((size_t)b * 2 + 0) * T + t] : philox_normal(seed, stream, 0x7700u, (uint32_t)t)) * scale;
+  z1[o] = (noise_w ? noise_w[((size_t)b * 2 + 1) * T + t] : philox_normal(seed, stream, 0x7701u, (uint32_t)t)) * scale;
 }
 
 // DurationPredictor.proj (C -> 1) or ElementwiseAffine^-1 on the SDP output      models.py:99, modules.py:398-399
@@ -306,33 +311,48 @@ __global__ void tts_logw_kernel(const float* x, const long long* lens, const flo
   out[o] = acc;
 }
 
-// one thread per utterance                                                       models.py:474-481
+// one thread per utterance; it.sdp_ratio / it.length_scale, when set, replace the call's values  models.py:474-481
 __global__ void tts_durations_kernel(const float* logw_sdp, const float* logw_dp, const long long* lens, float ratio,
                                      float length_scale, int B, int T, float* logw, float* w_ceil, int* cum,
-                                     long long* y_len) {
+                                     long long* y_len, ItemParams it) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const size_t o = (size_t)b * T;
+  if (it.sdp_ratio) ratio = it.sdp_ratio[b];
+  if (it.length_scale) length_scale = it.length_scale[b];
   y_len[b] = ovc_tts::durations_row(logw_sdp + o, logw_dp + o, ratio, length_scale, T, tts_len(lens, b, T), logw + o, w_ceil + o,
                                     cum + o);
 }
 
 // z_p[b][c][y] = m_p[tok(y)][c] + noise * exp(logs_p[tok(y)][c]) * noise_scale   models.py:484-487
 // stats [B][T][2C] (m | logs), z_p [B][C][P]; frames at or past y_len are zero.  grid (ceil(Ty/128), C, B)
+// it.seed / it.stream / it.noise_scale, when set, replace the call's seed, stream b and noise_scale for item b
 __global__ void tts_expand_kernel(const float* stats, const int* cum, const long long* y_len, const float* noise,
                                   long long noise_bs, int noise_pitch, unsigned long long seed, float noise_scale, int T,
-                                  int C, int Ty, int P, float* z_p) {
+                                  int C, int Ty, int P, float* z_p, ItemParams it) {
   const int y = blockIdx.x * blockDim.x + threadIdx.x, c = blockIdx.y, b = blockIdx.z;
   if (y >= P) return;
   float v = 0.f;
   if (y < Ty && y < y_len[b]) {
     const int j = ovc_tts::frame_token(cum + (size_t)b * T, T, y);
     const float* s = stats + ((size_t)b * T + j) * 2 * C;
+    if (it.seed) seed = it.seed[b];
+    const uint32_t stream = it.stream ? (uint32_t)it.stream[b] : (uint32_t)b;
+    if (it.noise_scale) noise_scale = it.noise_scale[b];
     const float nz = noise ? noise[(size_t)b * noise_bs + (size_t)c * noise_pitch + y]
-                           : philox_normal(seed, (uint32_t)b, (uint32_t)c, (uint32_t)y);
+                           : philox_normal(seed, stream, (uint32_t)c, (uint32_t)y);
     v = s[c] + nz * expf(s[C + c]) * noise_scale;
   }
   z_p[((size_t)b * C + c) * P + y] = v;
+}
+
+// out[c][t] = philox_normal(seed, stream, c0 + c, frame0 + t): the draws the kernels above make, as a tensor
+// (ovc_philox_normals).  grid (ceil(T/128), C)
+__global__ void philox_normals_kernel(unsigned long long seed, uint32_t stream, uint32_t c0, uint32_t frame0, int T,
+                                      float* out) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x, c = blockIdx.y;
+  if (t >= T) return;
+  out[(size_t)c * T + t] = philox_normal(seed, stream, c0 + (uint32_t)c, frame0 + (uint32_t)t);
 }
 
 }  // namespace ovc

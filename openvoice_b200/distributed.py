@@ -105,11 +105,14 @@ def convert_sharded(convert_fn: Callable[..., List[np.ndarray]], audios: Sequenc
                     device: str = "cpu", **kw) -> Optional[List[np.ndarray]]:
     """Every rank holds the same utterance list; each converts its LPT shard with ``convert_fn``
     (normally ``ToneColorConverter.convert_batch``) and rank 0 receives all results in order.
-    ``src_se`` / ``tgt_se``: one embedding for all items, or a per-item sequence."""
+    ``src_se`` / ``tgt_se``: one embedding for all items, or a per-item sequence.  A per-item ``seeds`` or ``tau``
+    keyword follows its utterance into the shard that converts it (``convert_fn`` receives the shard's values), so with
+    ``seeds`` every result is independent of the world size."""
     rank, world = _world()
     shards = lpt_shard([len(a) for a in audios], world)
     mine = shards[rank]
     pick = (lambda se: [se[i] for i in mine]) if isinstance(src_se, (list, tuple)) else (lambda se: se)
+    kw = _pick_per_item(kw, mine, len(audios))
     res = convert_fn([audios[i] for i in mine], pick(src_se),
                      [tgt_se[i] for i in mine] if isinstance(tgt_se, (list, tuple)) else tgt_se, **kw) if mine else []
     return gather_waveforms(res, mine, len(audios), device=device)
@@ -139,13 +142,28 @@ class ShardedJob:
         return out  # type: ignore[return-value]
 
 
-def convert_sharded_async(converter, audios: Sequence[np.ndarray], src_se, tgt_se, tau: float = 0.3, dst: int = 0,
-                          copy: bool = False) -> ShardedJob:
+def _pick_per_item(kw: dict, mine: List[int], n: int) -> dict:
+    """``kw`` with its per-item ``seeds`` / ``tau`` sequences cut down to the items ``mine`` (checked against ``n``
+    first, so every rank refuses the same malformed call)."""
+    from .api import check_per_item, check_seeds
+    kw = dict(kw)
+    if kw.get("seeds") is not None:
+        seeds = check_seeds(kw["seeds"], n)
+        kw["seeds"] = [seeds[i] for i in mine]
+    if "tau" in kw and np.ndim(kw["tau"]) != 0:
+        taus = check_per_item(kw["tau"], n, "tau")[1]
+        kw["tau"] = [taus[i] for i in mine]
+    return kw
+
+
+def convert_sharded_async(converter, audios: Sequence[np.ndarray], src_se, tgt_se, tau=0.3, dst: int = 0,
+                          copy: bool = False, seeds: Optional[Sequence[int]] = None) -> ShardedJob:
     """Every rank holds the same utterance list; each enqueues its LPT shard with
     ``converter.convert_batch_device`` (no host sync), the padded result blocks are gathered on rank ``dst`` by
     ONE device-to-device collective on a side stream, and rank ``dst`` alone downloads them.  Shapes of every
     rank's block follow from the shared list, so no size exchange is needed.  Returns at once; call ``.result()``.
-    ``src_se`` / ``tgt_se``: one embedding for all items, or a per-item sequence."""
+    ``src_se`` / ``tgt_se``: one embedding for all items, or a per-item sequence.  ``tau`` (scalar or per item) and
+    ``seeds`` (one key per item) follow their utterance as in ``convert_sharded``."""
     import torch
     rank, world = _world()
     hop = converter.hps.data.hop_length
@@ -157,6 +175,7 @@ def convert_sharded_async(converter, audios: Sequence[np.ndarray], src_se, tgt_s
     l_max = -(-max(len(a) for a in audios) // (16 * hop)) * (16 * hop) if samples else 0
     mine = shards[rank]
     pick = (lambda se: [se[i] for i in mine]) if isinstance(src_se, (list, tuple)) else (lambda se: se)
+    per = _pick_per_item({"tau": tau, "seeds": seeds}, mine, len(audios))
     state = converter.__dict__.setdefault("_shard_state", {"n": 0})
     k = state["n"] % 2
     state["n"] += 1
@@ -168,7 +187,8 @@ def convert_sharded_async(converter, audios: Sequence[np.ndarray], src_se, tgt_s
     if mine:
         o, _ = converter.convert_batch_device([audios[i] for i in mine], pick(src_se),
                                               [tgt_se[i] for i in mine] if isinstance(tgt_se, (list, tuple)) else tgt_se,
-                                              tau=tau, slot=k)
+                                              tau=per["tau"], slot=k,
+                                              **({} if seeds is None else {"seeds": per["seeds"]}))
     else:
         o = torch.zeros(0, max(l_max, 1), dtype=torch.float32, device=converter.device)
     table = [[(i, samples[i]) for i in sh] for sh in shards]

@@ -101,11 +101,20 @@ class StreamingResampler:
 class StreamingConverter:
     def __init__(self, converter, src_se, tgt_se, tau: float = 0.3, window_frames: int = 256,
                  noise_fn: Optional[Callable[[int, int], torch.Tensor]] = None, seed: Optional[int] = None,
-                 input_sr: Optional[int] = None, output_sr: Optional[int] = None):
+                 input_sr: Optional[int] = None, output_sr: Optional[int] = None, request_seed: Optional[int] = None):
         """``converter``: a ToneColorConverter.  ``noise_fn(t0, t1) -> [inter_channels, t1 - t0]`` supplies the noise of
         absolute frames [t0, t1) (tests pass slices of one tensor); default: a seeded device generator.
         ``input_sr`` / ``output_sr``: rates of the pushed and of the returned audio when they are not the model's
-        (``StreamingResampler`` on each side; None: the model's rate)."""
+        (``StreamingResampler`` on each side; None: the model's rate).
+        ``request_seed``: the request's own key, as ``ToneColorConverter.convert(seed=...)`` takes it: each window draws
+        its noise in-kernel at its absolute frames, so the stream gives ``convert(seed=request_seed)`` and no noise is
+        kept.  It excludes ``noise_fn`` and ``seed`` (ValueError)."""
+        from .api import check_seeds
+        if request_seed is not None:
+            if noise_fn is not None or seed is not None:
+                raise ValueError("request_seed replaces noise_fn and seed: pass only one of them")
+            request_seed = check_seeds([request_seed], 1, "request_seed")[0]
+        self.request_seed = request_seed
         self.conv = converter
         hp = converter.hps
         self.rs_in = self.rs_out = None
@@ -125,7 +134,7 @@ class StreamingConverter:
         self.dev = converter.device
         self.src = converter._stack_se(src_se, 1)
         self.tgt = converter._stack_se(tgt_se, 1)
-        if noise_fn is None:
+        if noise_fn is None and request_seed is None:
             gen = torch.Generator(device=self.dev)
             gen.manual_seed(int(seed if seed is not None else torch.randint(0, 2 ** 62, (1,)).item()))
             noise_fn = lambda t0, t1: torch.randn(self.C, t1 - t0, device=self.dev, generator=gen)  # noqa: E731
@@ -175,7 +184,8 @@ class StreamingConverter:
         new = sp[:, :, lead: lead + (upto - have)]
         assert new.shape[2] == upto - have, (new.shape, upto, have, lead)
         self.spec = torch.cat([self.spec, new], 2)
-        self.noise = torch.cat([self.noise, self.noise_fn(have, upto).to(self.dev, torch.float32).reshape(self.C, -1)], 1)
+        if self.request_seed is None:
+            self.noise = torch.cat([self.noise, self.noise_fn(have, upto).to(self.dev, torch.float32).reshape(self.C, -1)], 1)
         # audio before the support of the next frame (and its 2 lead frames) is no longer needed
         keep_from = max(0, (upto - 2) * hop - pad)
         if keep_from > self.a0:
@@ -187,17 +197,22 @@ class StreamingConverter:
         lo = max(0, e0 - self.H)
         hi = e1 + self.H if t_end is None else min(t_end, e1 + self.H)
         sp = self.spec[:, :, lo - self.f0: hi - self.f0].contiguous()
-        nz = self.noise[None, :, lo - self.f0: hi - self.f0].contiguous()
         lens = torch.tensor([hi - lo], dtype=torch.int64, device=self.dev)
-        o, _, _ = self.conv.model.voice_conversion(sp, lens, self.src, self.tgt, tau=self.tau, noise=nz, ragged=True,
-                                                   latents=False)
+        if self.request_seed is None:
+            nz = self.noise[None, :, lo - self.f0: hi - self.f0].contiguous()
+            o, _, _ = self.conv.model.voice_conversion(sp, lens, self.src, self.tgt, tau=self.tau, noise=nz, ragged=True,
+                                                       latents=False)
+        else:
+            o, _, _ = self.conv.model.voice_conversion(sp, lens, self.src, self.tgt, tau=self.tau, ragged=True,
+                                                       latents=False, seeds=[self.request_seed], frame0=[lo])
         out = o[0, 0, (e0 - lo) * self.hop: (e1 - lo) * self.hop].cpu().numpy().copy()
         self.emitted = e1
         # frames before the next window's left halo can go
         drop = max(0, e1 - self.H) - self.f0
         if drop > 0:
             self.spec = self.spec[:, :, drop:]
-            self.noise = self.noise[:, drop:]
+            if self.request_seed is None:
+                self.noise = self.noise[:, drop:]
             self.f0 += drop
         return out
 
