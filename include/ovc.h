@@ -25,10 +25,10 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 6   /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 7  /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
-                               * ovc_philox_normals */
+                               * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -265,6 +265,37 @@ OVC_API int ovc_tts_encode_items(ovc_ctx* ctx, const int64_t* tokens, const int6
 OVC_API int ovc_tts_decode_items(ovc_ctx* ctx, const float* noise, uint64_t seed, float noise_scale, int B, int Ymax,
                                  int max_len, int ragged, float* o, float* z, float* z_p, void* stream,
                                  const ovc_item_params* items);
+
+/* Streaming decode: the decode half in time windows, from encode state the caller owns.
+ *
+ * ovc_tts_encode_state copies what the pending ovc_tts_encode left in the context into caller buffers (device to
+ * device, only enqueued on `stream`): stats [B][T][2 inter] (m_p | logs_p per token), cum [B][T] int32 (cumulative
+ * frame durations: token j covers frames [cum[j-1], cum[j])) and g [B][gin] (the speaker vectors emb_g(sid)).  Together
+ * with the encode's y_lengths they are everything the decode reads, so a later ovc_tts_encode cannot disturb a decode
+ * that uses the copies.
+ *
+ * ovc_tts_decode_windows decodes W windows of N such encoded rows (stats, cum, g, y_lengths [N], T as encoded).  Every
+ * per-window value is a [W] device array:
+ *   row          encoded row of window w (int64; clamped into [0, N))
+ *   frame0, len  the window covers frames [frame0[w], frame0[w] + len[w]) of its row (int64)
+ *   seed         decode key (uint64), stream (int64), noise_scale (float)
+ * Window w's frame frame0[w] + t, t < len[w], is expanded exactly as the whole decode expands that frame: the token
+ * of the absolute frame, the Philox draw at counter (key = seed[w]; stream[w], channel c, (frame0[w] + t) mod 2^32),
+ * which is the whole decode's counter for that frame with the same key and stream (see ovc_tts_decode_items).  The flow
+ * and the generator then run on the window alone, at its own length: the frames of it inside [0, y_lengths[row]),
+ * at most Wmax.  A window [lo, hi) that extends its interior [e0, e1) by the decode's receptive field on both sides
+ * (flow reverse +-32 frames, generator +-14; clipped at the row's ends) gives the whole decode's samples of
+ * [e0, e1) to fp32 reordering; a window of the whole row gives them bit for bit.  Outputs:
+ *   o    [W][hop * Wmax]      window w's samples, zero past hop * (its decode length)
+ *   z_p  [W][inter][Wmax]     or NULL; the expanded prior sample, zero past the window's decode length
+ * Frames outside the row, or past len[w], are zeros and nothing is read out of bounds whatever the arrays hold.  A call
+ * that repeats its (W, Wmax, buffers, options) is replayed from a CUDA graph (OVC_OPT_GRAPH) and follows the arrays'
+ * new contents.  Null buffers or non-positive sizes are OVC_ERR_INVALID. */
+OVC_API int ovc_tts_encode_state(ovc_ctx* ctx, float* stats, int32_t* cum, float* g, void* stream);
+OVC_API int ovc_tts_decode_windows(ovc_ctx* ctx, const float* stats, const int32_t* cum, const float* g,
+                                   const int64_t* y_lengths, int N, int T, const int64_t* row, const int64_t* frame0,
+                                   const int64_t* len, int W, int Wmax, const uint64_t* seed, const int64_t* stream,
+                                   const float* noise_scale, float* o, float* z_p, void* cuda_stream);
 
 /* Arithmetic of the convolutions (generator ResBlocks = 90 % of the FLOPs, WaveNet stacks, upsamplers):
  *   0            fp32 FFMA on the CUDA cores

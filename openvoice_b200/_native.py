@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -22,6 +22,7 @@ EXPORTS = (
     "ovc_tts_info", "ovc_tts_encode", "ovc_tts_decode", "ovc_set_option", "ovc_graph_replays",
     "ovc_reference_encoder_ragged", "ovc_resample", "ovc_resample_span", "ovc_voice_conversion_items",
     "ovc_convert_waveform_items", "ovc_tts_encode_items", "ovc_tts_decode_items", "ovc_philox_normals",
+    "ovc_tts_encode_state", "ovc_tts_decode_windows",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample input length of a stream that has not ended
@@ -145,6 +146,9 @@ def load_library(path: Optional[str] = None):
     lib.ovc_tts_decode_items.argtypes = lib.ovc_tts_decode.argtypes + [P]
     lib.ovc_philox_normals.argtypes = [C.c_uint64, C.c_int64, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_void_p,
                                        C.c_void_p]
+    lib.ovc_tts_encode_state.argtypes = [C.c_void_p] * 5
+    lib.ovc_tts_decode_windows.argtypes = ([C.c_void_p] * 5 + [C.c_int, C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int]
+                                           + [C.c_void_p] * 6)
     if lib.ovc_abi_version() != ABI_VERSION:
         raise OvcError(f"ABI mismatch: library {lib.ovc_abi_version()} vs binding {ABI_VERSION}")
     _lib = lib
@@ -467,6 +471,77 @@ class NativeConverter:
                                            p(lat[1]) if lat else None, C.c_void_p(st.cuda_stream), _items_ref(it))
         _check(self.lib, rc, "ovc_tts_decode")
         return o, lat
+
+    def tts_encode_state(self, B: int, T: int, device, stream=None):
+        """Caller-owned copies of what the last ``tts_encode`` (B rows of T tokens) left in the context (include/ovc.h:
+        ovc_tts_encode_state): (stats [B,T,2*inter] f32, cum [B,T] int32, g [B,gin] f32) on the device.  A later
+        ``tts_encode`` does not touch them.  Asynchronous on `stream`."""
+        import torch
+        stats = torch.empty(B, T, 2 * self.hp.inter_channels, device=device, dtype=torch.float32)
+        cum = torch.empty(B, T, device=device, dtype=torch.int32)
+        g = torch.empty(B, self.hp.gin_channels, device=device, dtype=torch.float32)
+        st = stream if stream is not None else torch.cuda.current_stream(device)
+        rc = self.lib.ovc_tts_encode_state(self.handle, C.c_void_p(stats.data_ptr()), C.c_void_p(cum.data_ptr()),
+                                           C.c_void_p(g.data_ptr()), C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_tts_encode_state")
+        return stats, cum, g
+
+    def tts_decode_windows(self, stats, cum, g, y_lengths, row, frame0, length, seed, streams, noise_scale, w_max: int,
+                           latents: bool = False, slot: int = 0, stream=None):
+        """Decode W windows of caller-owned encode state (``tts_encode_state`` + the encode's y_lengths; include/ovc.h:
+        ovc_tts_decode_windows).  ``row``, ``frame0``, ``length``, ``seed`` (decode keys in [0, 2^64)), ``streams`` and
+        ``noise_scale`` are host sequences of W values.  They are staged through slot ``slot``'s pinned and device
+        buffers, and ``o`` is written into the slot's device buffer: with every address stable, a repeated (W, w_max)
+        call is replayed from a CUDA graph with the new values.  Returns (o [W, hop * w_max], z_p [W, inter, w_max] or
+        None); ``o`` is overwritten by the next call on the slot.  Asynchronous on `stream`."""
+        import numpy as np
+        import torch
+        W = len(row)
+        vals = [row, frame0, length, seed, streams, noise_scale]
+        if W < 1 or any(len(v) != W for v in vals):
+            raise ValueError(f"tts_decode_windows: every per-window sequence needs the same length >= 1, got "
+                             f"{[len(v) for v in vals]}")
+        N, T = cum.shape
+        dev = cum.device
+        for t, dt, shape in ((stats, torch.float32, (N, T, 2 * self.hp.inter_channels)), (cum, torch.int32, (N, T)),
+                             (g, torch.float32, (N, self.hp.gin_channels)), (y_lengths, torch.int64, (N,))):
+            assert t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, t.shape)
+        cache = self.__dict__.setdefault("_win_bufs", {})
+        ev = cache.get(("ev", slot))
+        if ev is not None:
+            ev.synchronize()                  # the slot's previous upload has left the pinned buffers
+        ints = np.empty((5, W), dtype=np.int64)
+        ints[0], ints[1], ints[2], ints[4] = row, frame0, length, streams
+        ints[3] = np.asarray([int(s) & (2 ** 64 - 1) for s in seed], dtype=np.uint64).view(np.int64)
+
+        def buf(name, numel, dtype, pinned=False):
+            b = cache.get((name, slot))
+            if b is None or b.numel() < numel:
+                b = torch.empty(int(numel * 1.25) + 64, dtype=dtype, device="cpu" if pinned else dev)
+                b = b.pin_memory() if pinned else b
+                cache[(name, slot)] = b
+            return b[:numel]
+        pin_i, pin_f = buf("pin_i", 5 * W, torch.int64, True), buf("pin_f", W, torch.float32, True)
+        pin_i.copy_(torch.from_numpy(ints.reshape(-1)))
+        pin_f.copy_(torch.tensor([float(v) for v in noise_scale], dtype=torch.float32))
+        d_i, d_f = buf("d_i", 5 * W, torch.int64), buf("d_f", W, torch.float32)
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        with torch.cuda.stream(st):
+            d_i.copy_(pin_i, non_blocking=True)
+            d_f.copy_(pin_f, non_blocking=True)
+            ev = torch.cuda.Event()
+            ev.record(st)
+        cache[("ev", slot)] = ev
+        hop = self.hp.hop_length
+        o = buf("o", W * hop * int(w_max), torch.float32).view(W, hop * int(w_max))
+        zp = torch.empty(W, self.hp.inter_channels, int(w_max), device=dev, dtype=torch.float32) if latents else None
+        p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+        rc = self.lib.ovc_tts_decode_windows(
+            self.handle, p(stats), p(cum), p(g), p(y_lengths), N, T, p(d_i[0:W]), p(d_i[W:2 * W]), p(d_i[2 * W:3 * W]), W,
+            int(w_max), p(d_i[3 * W:4 * W]), p(d_i[4 * W:]), p(d_f), p(o), p(zp) if zp is not None else None,
+            C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_tts_decode_windows")
+        return o, zp
 
     @property
     def last_launch_count(self) -> int:

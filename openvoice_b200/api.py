@@ -12,7 +12,7 @@ from __future__ import annotations
 
 import math
 import os
-from typing import List, Optional, Sequence, Tuple, Union
+from typing import Iterator, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -122,6 +122,44 @@ def plan_se_chunks(frames: Sequence[int], budget: int = SE_CHUNK_FRAMES) -> List
         else:
             chunks.append([i])
     return chunks
+
+
+# Receptive field of the TTS decode in frames, per direction.  After the expansion, which is pointwise in time, it runs
+# the flow in reverse and the generator.  Flow: 4 couplings x a WaveNet of 4 layers with k = 5, dilation 1, i.e. +-2 per
+# layer, +-8 per coupling, +-32 in all.  Generator: +-13.3 frames (conv_pre k = 7, the transposed convs, ResBlocks up to
+# k = 11 d = 5; ToneColorConverter.HALO_FRAMES).  That is +-45.3 frames; 64 leaves margin.  There is no enc_q and no
+# forward flow here, so this is about half of HALO_FRAMES.
+TTS_HALO_FRAMES = 64
+
+
+def plan_tts_windows(frames: int, first_window: int, window: int, halo: int) -> List[Tuple[int, int, int, int]]:
+    """Windows of one sentence of ``frames`` decoded frames: (lo, hi, e0, e1) with decoded span [lo, hi) and interior
+    [e0, e1).  The first interior has ``first_window`` frames and the others ``window`` (the last may be shorter); the
+    interiors cover [0, frames) once and in order; lo = max(0, e0 - halo) and hi = min(frames, e1 + halo)."""
+    frames, first_window, window, halo = int(frames), int(first_window), int(window), int(halo)
+    if frames < 1 or first_window < 1 or window < 1 or halo < 0:
+        raise ValueError(f"plan_tts_windows needs frames, first_window, window >= 1 and halo >= 0 (got {frames}, "
+                         f"{first_window}, {window}, {halo})")
+    out, e0 = [], 0
+    while e0 < frames:
+        e1 = min(frames, e0 + (first_window if e0 == 0 else window))
+        out.append((max(0, e0 - halo), min(frames, e1 + halo), e0, e1))
+        e0 = e1
+    return out
+
+
+class TtsState(NamedTuple):
+    """Encode state of ``NativeSynthesizer.tts_encode``, owned by the caller: device tensors stats [N,T,2*inter],
+    cum [N,T] int32, g [N,gin] and y_lengths [N], each row's decoded frames (host), and the decode key, stream and
+    noise scale ``infer`` would draw each row's prior noise with."""
+    stats: torch.Tensor
+    cum: torch.Tensor
+    g: torch.Tensor
+    y_lengths: torch.Tensor
+    frames: List[int]
+    dec_keys: List[int]
+    dec_streams: List[int]
+    dec_noise_scale: List[float]
 
 
 _POOL = None
@@ -287,6 +325,30 @@ class NativeSynthesizer:
         duration noise draws from ``seeds[b]``, the prior noise from ``seeds[b] + 1``, as a scalar ``seed`` does) at
         stream ``streams[b]`` (default: b).  Sentence j of a call with ``seed=s`` is reproduced in any batch by
         ``seeds[i] = s, streams[i] = j`` and the same parameters."""
+        a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams)
+        x, x_lengths, sid, seed, B = a["x"], a["x_lengths"], a["sid"], a["seed"], a["B"]
+        noise_scale, enc_items, dec_items = a["noise_scale"], a["enc_items"], a["dec_items"]
+        if noise_w is not None:
+            noise_w = noise_w.to(self.device, torch.float32)
+        y_lengths, w_ceil, _ = self.native.tts_encode(x, x_lengths, sid, noise_w=noise_w, seed=seed, items=enc_items,
+                                                      **a["enc_scalars"])
+        Ty = int(y_lengths.max().item())                       # the sync
+        if noise is not None:
+            noise = noise.to(self.device, torch.float32)[:, :, :Ty].contiguous()
+        o, lat = self.native.tts_decode(B, Ty, self.device, noise=noise, seed=seed + 1, noise_scale=float(noise_scale),
+                                        ragged=ragged, latents=latents, max_len=max_len, items=dec_items)
+        ar = torch.arange(Ty, device=self.device)
+        y_mask = (ar[None, :] < y_lengths[:, None]).unsqueeze(1).to(torch.float32)
+        cum = torch.cumsum(w_ceil, 1)                          # commons.generate_path (commons.py:128-142)
+        path = (ar[None, :, None] < cum[:, None, :]) & (ar[None, :, None] >= (cum - w_ceil)[:, None, :])
+        attn = (path.to(torch.float32) * y_mask.transpose(1, 2)).unsqueeze(1)      # [B,1,Ty,T]
+        z, z_p = lat if lat else (None, None)
+        return o, attn, y_mask, (z, z_p, None, None)
+
+    def _tts_args(self, x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams):
+        """The checks and device inputs ``infer`` and ``tts_encode`` share: validated tokens, lengths and speakers on the
+        device, the call's key, the per-item parameter arrays of both halves, and each row's decode key, stream and
+        noise scale as host lists (what the whole decode draws row b with)."""
         info = self.native.tts_info()
         if not info["has_tts"]:
             raise RuntimeError("this checkpoint has no enc_p / dp / sdp / emb_g: infer() needs a V1 base speaker")
@@ -313,8 +375,6 @@ class NativeSynthesizer:
         sdp_ratio, sr_b = check_per_item(sdp_ratio, B, "sdp_ratio")
         if seed is None:
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
-        if noise_w is not None:
-            noise_w = noise_w.to(self.device, torch.float32)
         dev = self.device
         f32 = lambda v: None if v is None else torch.tensor(v, dtype=torch.float32, device=dev)  # noqa: E731
         key = None if seeds is None else torch.from_numpy(seed_array(seeds)).to(dev)
@@ -325,21 +385,56 @@ class NativeSynthesizer:
             enc_items = {"seed": key, "stream": stream_d, "noise_scale_w": f32(nsw_b), "length_scale": f32(ls_b),
                          "sdp_ratio": f32(sr_b)}
             dec_items = {"seed": key1, "stream": stream_d, "noise_scale": f32(ns_b)}
-        y_lengths, w_ceil, _ = self.native.tts_encode(x, x_lengths, sid, noise_w=noise_w, seed=seed,
-                                                      noise_scale_w=float(noise_scale_w), length_scale=float(length_scale),
-                                                      sdp_ratio=float(sdp_ratio), items=enc_items)
-        Ty = int(y_lengths.max().item())                       # the sync
-        if noise is not None:
-            noise = noise.to(self.device, torch.float32)[:, :, :Ty].contiguous()
-        o, lat = self.native.tts_decode(B, Ty, self.device, noise=noise, seed=seed + 1, noise_scale=float(noise_scale),
-                                        ragged=ragged, latents=latents, max_len=max_len, items=dec_items)
-        ar = torch.arange(Ty, device=self.device)
-        y_mask = (ar[None, :] < y_lengths[:, None]).unsqueeze(1).to(torch.float32)
-        cum = torch.cumsum(w_ceil, 1)                          # commons.generate_path (commons.py:128-142)
-        path = (ar[None, :, None] < cum[:, None, :]) & (ar[None, :, None] >= (cum - w_ceil)[:, None, :])
-        attn = (path.to(torch.float32) * y_mask.transpose(1, 2)).unsqueeze(1)      # [B,1,Ty,T]
-        z, z_p = lat if lat else (None, None)
-        return o, attn, y_mask, (z, z_p, None, None)
+        return dict(x=x, x_lengths=x_lengths, sid=sid, seed=seed, B=B, noise_scale=noise_scale, enc_items=enc_items,
+                    dec_items=dec_items,
+                    enc_scalars=dict(noise_scale_w=float(noise_scale_w), length_scale=float(length_scale),
+                                     sdp_ratio=float(sdp_ratio)),
+                    dec_keys=[(seed if seeds is None else seeds[b]) + 1 for b in range(B)],
+                    dec_streams=list(range(B)) if streams is None else streams,
+                    dec_noise_scale=[noise_scale] * B if ns_b is None else ns_b)
+
+    @torch.no_grad()
+    def tts_encode(self, x, x_lengths, sid=None, noise_scale=1, length_scale=1, noise_scale_w=1.0, sdp_ratio=0.2,
+                   seed: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
+                   streams: Optional[Sequence[int]] = None) -> "TtsState":
+        """The encode half of ``infer`` (same arguments and draws), returning state the caller owns: a later
+        ``tts_encode`` or ``infer`` does not change it.  ``tts_decode_windows`` decodes any frames of its rows, each
+        row with the decode key, stream and noise scale ``infer`` would give it.  One host sync (y_lengths), as in
+        ``infer``."""
+        a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams)
+        x = a["x"]
+        y_lengths, _, _ = self.native.tts_encode(x, a["x_lengths"], a["sid"], seed=a["seed"], items=a["enc_items"],
+                                                 **a["enc_scalars"])
+        stats, cum, g = self.native.tts_encode_state(x.shape[0], x.shape[1], self.device)
+        frames = [int(v) for v in y_lengths.cpu()]             # the sync
+        return TtsState(stats, cum, g, y_lengths, frames, a["dec_keys"], a["dec_streams"], a["dec_noise_scale"])
+
+    @torch.no_grad()
+    def tts_decode_windows(self, state: "TtsState", windows: Sequence[Tuple[int, int, int]], w_max: Optional[int] = None,
+                           latents: bool = False, slot: int = 0):
+        """Decode ``windows`` = [(row, frame0, length)] of ``state`` in ONE call (include/ovc.h: ovc_tts_decode_windows):
+        window i holds frames [frame0, frame0 + length) of its row.  Returns (o [W, hop * w_max] on the device, z_p
+        [W, inter, w_max] or None); window i's samples are o[i, : hop * length], and ``o`` lives in slot ``slot``'s buffer
+        until the next call on that slot.  ``w_max`` defaults to the longest window.  A row outside the state, a negative
+        offset, a length < 1, a window past its row's end, or a w_max shorter than a window raises ValueError before
+        anything is launched."""
+        windows = [tuple(int(v) for v in w) for w in windows]
+        if not windows:
+            raise ValueError("tts_decode_windows needs at least one window")
+        n = len(state.frames)
+        for i, (r, f0, ln) in enumerate(windows):
+            if not 0 <= r < n:
+                raise ValueError(f"window {i}: row {r} outside [0, {n})")
+            if f0 < 0 or ln < 1 or f0 + ln > state.frames[r]:
+                raise ValueError(f"window {i}: frames [{f0}, {f0 + ln}) are not inside row {r}'s {state.frames[r]} frames")
+        w_max = max(ln for _, _, ln in windows) if w_max is None else int(w_max)
+        if w_max < max(ln for _, _, ln in windows):
+            raise ValueError(f"w_max {w_max} is shorter than the longest window")
+        rows = [r for r, _, _ in windows]
+        return self.native.tts_decode_windows(
+            state.stats, state.cum, state.g, state.y_lengths, rows, [f0 for _, f0, _ in windows],
+            [ln for _, _, ln in windows], [state.dec_keys[r] for r in rows], [state.dec_streams[r] for r in rows],
+            [state.dec_noise_scale[r] for r in rows], w_max, latents=latents, slot=slot)
 
     def _expand_se(self, se, B):
         se = se.to(self.device, torch.float32).reshape(se.shape[0], -1)
@@ -430,6 +525,17 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
         ``audio_numpy_concat(tts_from_ids(ids, speaker, speed=..., seed=seed_r, ...), sr, speed)`` bit for bit: the
         sentences joined with 50 ms / speed gaps, as ``tts`` does.  Returns one array per request."""
         reqs = list(requests)
+        seqs, sid, owner, speeds, kw = self._request_sentences(reqs)
+        sr = self.hps.data.sampling_rate
+        audio = self._infer_sentences(seqs, sid, **kw) if seqs else []
+        per: List[List[np.ndarray]] = [[] for _ in reqs]
+        for r, a in zip(owner, audio):
+            per[r].append(a)
+        return [self.audio_numpy_concat(per[r], sr=sr, speed=speeds[r]) for r in range(len(reqs))]
+
+    def _request_sentences(self, reqs):
+        """The sentences of ``tts_batch`` requests: (token-id lists, speaker ids, owning request, each request's speed,
+        the per-sentence ``infer`` keywords).  Sentence j of request r is keyed (seed_r, stream j) with r's parameters."""
         seqs, sid, seeds, streams, owner = [], [], [], [], []
         par = {"noise_scale": [], "noise_scale_w": [], "length_scale": [], "sdp_ratio": []}
         speeds = []
@@ -453,21 +559,77 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
                 par["noise_scale_w"].append(float(q.get("noise_scale_w", 0.6)))
                 par["length_scale"].append(1.0 / speed)
                 par["sdp_ratio"].append(float(q.get("sdp_ratio", 0.2)))
-        sr = self.hps.data.sampling_rate
-        audio = self._infer_sentences(seqs, sid, seeds=seeds, streams=streams, **par) if seqs else []
-        per: List[List[np.ndarray]] = [[] for _ in reqs]
-        for r, a in zip(owner, audio):
-            per[r].append(a)
-        return [self.audio_numpy_concat(per[r], sr=sr, speed=speeds[r]) for r in range(len(reqs))]
+        return seqs, sid, owner, speeds, dict(seeds=seeds, streams=streams, **par)
+
+    @staticmethod
+    def _pad_ids(sequences):
+        """Token-id lists -> (x [n, T] int64 zero-padded, lengths [n])."""
+        T = max(len(q) for q in sequences)
+        x = torch.zeros(len(sequences), T, dtype=torch.int64)
+        for i, q in enumerate(sequences):
+            x[i, :len(q)] = torch.as_tensor(q, dtype=torch.int64)
+        return x, torch.tensor([len(q) for q in sequences], dtype=torch.int64)
+
+    def tts_stream_batch(self, requests: Sequence[dict], window_frames: int = 256,
+                         first_window_frames: int = 32) -> Iterator[Tuple[int, np.ndarray]]:
+        """Streaming ``tts_batch``: yields ``(request_index, chunk)`` as the audio is decoded, so playback can start after
+        the first window instead of after the whole utterance.  Requests are the dicts ``tts_batch`` takes; all their
+        sentences share ONE encode.  Each step is ONE ``NativeSynthesizer.tts_decode_windows`` call over the next window
+        of every unfinished request and yields one chunk per such request, in request order.  A request's sentences are
+        decoded in order: the first sentence in windows of ``first_window_frames`` then ``window_frames`` frames, the
+        others in windows of ``window_frames``, each decoded with ``TTS_HALO_FRAMES`` frames of context on both sides
+        (``plan_tts_windows``); a sentence's last chunk ends with its 50 ms / speed of silence.  A request's chunks
+        concatenate to ``tts_batch``'s array for it (same length, same gaps) within fp32 reordering (2e-6 of its rms),
+        whatever requests it is batched with.  Malformed requests (an empty one, a speed <= 0, a bad seed) or window
+        sizes < 1 raise ValueError here, before anything is launched."""
+        window_frames, first_window_frames = int(window_frames), int(first_window_frames)
+        if window_frames < 1 or first_window_frames < 1:
+            raise ValueError(f"window_frames ({window_frames}) and first_window_frames ({first_window_frames}) must be >= 1")
+        reqs = list(requests)
+        seqs, sid, owner, speeds, kw = self._request_sentences(reqs)
+        for r in range(len(reqs)):
+            if r not in owner:
+                raise ValueError(f"request {r} has no sentences")
+        return self._stream(seqs, sid, owner, speeds, kw, window_frames, first_window_frames)
+
+    @torch.no_grad()
+    def _stream(self, seqs, sid, owner, speeds, kw, window_frames, first_window_frames):
+        if not seqs:
+            return
+        x, lens = self._pad_ids(seqs)
+        state = self.model.tts_encode(x, lens, sid=torch.as_tensor(sid, dtype=torch.int64), **kw)
+        sr, hop = self.hps.data.sampling_rate, self.hps.data.hop_length
+        # per request: its windows in order, (row, lo, hi, e0, e1, silence after the chunk)
+        plans: List[List[Tuple[int, int, int, int, int, int]]] = [[] for _ in speeds]
+        for i, r in enumerate(owner):
+            first = first_window_frames if not plans[r] else window_frames
+            wins = plan_tts_windows(state.frames[i], first, window_frames, TTS_HALO_FRAMES)
+            gap = int((sr * 0.05) / speeds[r])
+            plans[r] += [(i, lo, hi, e0, e1, gap if k == len(wins) - 1 else 0) for k, (lo, hi, e0, e1) in enumerate(wins)]
+        for step in range(max(len(p) for p in plans)):
+            live = [(r, p[step]) for r, p in enumerate(plans) if step < len(p)]
+            o, _ = self.model.tts_decode_windows(state, [(i, lo, hi - lo) for _, (i, lo, hi, _, _, _) in live])
+            host = o.cpu().numpy()
+            for k, (r, (_, lo, _, e0, e1, gap)) in enumerate(live):
+                chunk = host[k, (e0 - lo) * hop: (e1 - lo) * hop]
+                yield r, np.concatenate([chunk, np.zeros(gap, np.float32)]) if gap else chunk.copy()
+
+    def tts_stream(self, text=None, speaker=None, language="English", speed=1.0, seed: Optional[int] = None, ids=None,
+                   window_frames: int = 256, first_window_frames: int = 32) -> Iterator[np.ndarray]:
+        """``tts`` as a stream of float32 chunks (``tts_stream_batch`` with one request): the first chunk is
+        ``first_window_frames`` frames of audio, available once the encode and one small decode have run.  ``ids``
+        (token-id lists, one per sentence) replaces ``text``.  The chunks concatenate to ``tts(text, None, speaker,
+        language, speed, seed)`` within 2e-6 of its rms, with the same length and the same silences.  Feeding them to
+        ``streaming.StreamingConverter.push`` gives cloned-voice streaming."""
+        q = dict(speaker=speaker, speed=speed, seed=seed)
+        q.update({"ids": ids} if ids is not None else {"text": text, "language": language})
+        gen = self.tts_stream_batch([q], window_frames=window_frames, first_window_frames=first_window_frames)
+        return (chunk for _, chunk in gen)
 
     def _infer_sentences(self, sequences, sid, **kw) -> List[np.ndarray]:
         """One ragged infer over token-id lists with per-sentence speaker ids; each sentence's samples."""
         n = len(sequences)
-        T = max(len(q) for q in sequences)
-        x = torch.zeros(n, T, dtype=torch.int64)
-        for i, q in enumerate(sequences):
-            x[i, :len(q)] = torch.as_tensor(q, dtype=torch.int64)
-        lens = torch.tensor([len(q) for q in sequences], dtype=torch.int64)
+        x, lens = self._pad_ids(sequences)
         o, _, y_mask, _ = self.model.infer(x, lens, sid=torch.as_tensor(sid, dtype=torch.int64), ragged=True,
                                            latents=False, **kw)
         frames = y_mask[:, 0].sum(1).long().cpu()

@@ -691,7 +691,7 @@ static int finalize(ovc_ctx* c) {
 // ---------------------------------------------------------------------------------------------
 struct WsLayout {
   int P;   // frame pitch (multiple of 4)
-  size_t cond, x, skip, acts, z, dpre, bufA, bufB, bufC, bufD, bufE, bufF, spec, frames, total;
+  size_t cond, x, skip, acts, z, dpre, bufA, bufB, bufC, bufD, bufE, bufF, spec, frames, win_g, win_len, total;
   size_t brB[2], brC[2];   // per-branch ResBlock buffers of the concurrent-branch mode (small calls only)
   bool branches;
 };
@@ -720,6 +720,8 @@ static WsLayout ws_layout(const ovc_ctx* c, int B, int Tmax) {
   }
   L.spec = take((size_t)B * c->hp.spec_channels * L.P);
   L.frames = take((size_t)2 * B + 4);   // B int64
+  L.win_g = take((size_t)B * c->hp.gin_channels);   // ovc_tts_decode_windows: g of each window's row
+  L.win_len = take((size_t)2 * B + 4);              // and its decode length, B int64
   L.total = o;
   return L;
 }
@@ -1756,6 +1758,49 @@ int ovc_tts_decode_items(ovc_ctx* c, const float* noise, uint64_t seed, float no
   if (max_len < 0) return fail(OVC_ERR_INVALID, "max_len must be >= 0 (0 = no limit)");
   return run_tts_decode(c, noise, seed, noise_scale, B, Ymax, max_len, ragged, o, z, z_p, item_params(items),
                         (cudaStream_t)stream);
+}
+
+int ovc_tts_encode_state(ovc_ctx* c, float* stats, int32_t* cum, float* g, void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
+  if (c->tts_B < 1) return fail(OVC_ERR_STATE, "ovc_tts_encode_state needs a preceding ovc_tts_encode");
+  if (!stats || !cum || !g) return fail(OVC_ERR_INVALID, "null tensor argument");
+  ON_DEVICE(c);
+  const int B = c->tts_B, T = c->tts_T;
+  const TtsWs TW = tts_ws_layout(c, B, T);
+  cudaStream_t st = (cudaStream_t)stream;
+  CK(cudaMemcpyAsync(stats, c->d_tts + TW.STATS, (size_t)B * T * 2 * c->tts.C * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(cum, c->d_tts + TW.cum, (size_t)B * T * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(g, c->d_tts + TW.g, (size_t)B * c->hp.gin_channels * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return OVC_OK;
+}
+
+int ovc_tts_decode_windows(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths,
+                           int N, int T, const int64_t* row, const int64_t* frame0, const int64_t* len, int W, int Wmax,
+                           const uint64_t* seed, const int64_t* stream, const float* noise_scale, float* o, float* z_p,
+                           void* cuda_stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
+  if (!stats || !cum || !g || !y_lengths || !row || !frame0 || !len || !seed || !stream || !noise_scale || !o)
+    return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (N < 1 || T < 1 || W < 1 || Wmax < 1)
+    return fail(OVC_ERR_INVALID, "N, T, W and Wmax must be positive (got %d, %d, %d, %d)", N, T, W, Wmax);
+  if (W > 65535) return fail(OVC_ERR_INVALID, "W %d exceeds the grid limit", W);
+  if ((long long)Wmax * 256 * 64 > 2000000000LL) return fail(OVC_ERR_INVALID, "Wmax %d too large for 32-bit indexing", Wmax);
+  ON_DEVICE(c);
+  c->ev_used = c->prof ? c->ev_used : 0;
+  cudaStream_t st = (cudaStream_t)cuda_stream;
+  TRY(ensure_ws(c, ws_layout(c, W, Wmax), W, Wmax, st));
+  ItemParams it{};
+  it.seed = (const unsigned long long*)seed; it.stream = (const long long*)stream; it.noise_scale = noise_scale;
+  const TtsWindows win{(const long long*)row, (const long long*)frame0, (const long long*)len, N};
+  std::vector<uintptr_t> key = {3, (uintptr_t)stats, (uintptr_t)cum, (uintptr_t)g, (uintptr_t)y_lengths, (uintptr_t)N,
+                                (uintptr_t)T, (uintptr_t)row, (uintptr_t)frame0, (uintptr_t)len, (uintptr_t)W, (uintptr_t)Wmax,
+                                (uintptr_t)o, (uintptr_t)z_p, option_bits(c)};
+  append_item_key(key, it);
+  return run_graphed(c, key, st, [&](cudaStream_t s) {
+    return run_tts_decode_windows(c, stats, cum, g, (const long long*)y_lengths, T, win, W, Wmax, it, o, z_p, s);
+  });
 }
 
 int ovc_philox_normals(uint64_t seed, int64_t stream, int64_t c0, int C, int64_t frame0, int T, float* out, void* cuda_stream) {

@@ -324,26 +324,52 @@ __global__ void tts_durations_kernel(const float* logw_sdp, const float* logw_dp
                                     cum + o);
 }
 
+// Windows of ovc_tts_decode_windows: output row w expands encoded row row[w] at absolute frames frame0[w] + t,
+// t < len[w].  Every pointer NULL: output row b is encoded row b from frame 0 (the whole decode).
+struct TtsWindows {
+  const long long* row;      // [W], clamped into [0, N)
+  const long long* frame0;   // [W]
+  const long long* len;      // [W]
+  int N;                     // encoded rows
+};
+
 // z_p[b][c][y] = m_p[tok(y)][c] + noise * exp(logs_p[tok(y)][c]) * noise_scale   models.py:484-487
 // stats [B][T][2C] (m | logs), z_p [B][C][P]; frames at or past y_len are zero.  grid (ceil(Ty/128), C, B)
-// it.seed / it.stream / it.noise_scale, when set, replace the call's seed, stream b and noise_scale for item b
+// it.seed / it.stream / it.noise_scale, when set, replace the call's seed, stream b and noise_scale for item b.
+// With windows, row b reads encoded row r = row[b] at frame f = frame0[b] + y (token, Philox counter and y_len all
+// at f) and is zero at or past len[b]; an explicit noise tensor is indexed by the output column y.
 __global__ void tts_expand_kernel(const float* stats, const int* cum, const long long* y_len, const float* noise,
                                   long long noise_bs, int noise_pitch, unsigned long long seed, float noise_scale, int T,
-                                  int C, int Ty, int P, float* z_p, ItemParams it) {
+                                  int C, int Ty, int P, float* z_p, ItemParams it, TtsWindows win) {
   const int y = blockIdx.x * blockDim.x + threadIdx.x, c = blockIdx.y, b = blockIdx.z;
   if (y >= P) return;
+  const long long r = win.row ? min(max(win.row[b], 0LL), (long long)win.N - 1) : (long long)b;
+  const long long f = win.frame0 ? win.frame0[b] + y : (long long)y;
   float v = 0.f;
-  if (y < Ty && y < y_len[b]) {
-    const int j = ovc_tts::frame_token(cum + (size_t)b * T, T, y);
-    const float* s = stats + ((size_t)b * T + j) * 2 * C;
+  if (y < Ty && f >= 0 && f < y_len[r] && (!win.len || y < win.len[b])) {
+    const int j = ovc_tts::frame_token(cum + (size_t)r * T, T, (int)f);
+    const float* s = stats + ((size_t)r * T + j) * 2 * C;
     if (it.seed) seed = it.seed[b];
     const uint32_t stream = it.stream ? (uint32_t)it.stream[b] : (uint32_t)b;
     if (it.noise_scale) noise_scale = it.noise_scale[b];
     const float nz = noise ? noise[(size_t)b * noise_bs + (size_t)c * noise_pitch + y]
-                           : philox_normal(seed, stream, (uint32_t)c, (uint32_t)y);
+                           : philox_normal(seed, stream, (uint32_t)c, (uint32_t)f);
     v = s[c] + nz * expf(s[C + c]) * noise_scale;
   }
   z_p[((size_t)b * C + c) * P + y] = v;
+}
+
+// Per-window inputs of the flow and generator (ovc_tts_decode_windows): g_out[w] = g[row[w]], and lens[w] = the
+// frames of window w that lie inside its row, clamp(min(len[w], y_len[row[w]] - frame0[w]), 0, Tmax).  grid (W), 128
+__global__ void tts_window_rows_kernel(const float* g, const long long* y_len, int gin, TtsWindows win, int Tmax,
+                                       float* g_out, long long* lens) {
+  const int w = blockIdx.x;
+  const long long r = min(max(win.row[w], 0LL), (long long)win.N - 1);
+  for (int i = threadIdx.x; i < gin; i += blockDim.x) g_out[(size_t)w * gin + i] = g[(size_t)r * gin + i];
+  if (threadIdx.x == 0) {
+    const long long n = min(win.len[w], y_len[r] - win.frame0[w]);
+    lens[w] = n < 0 ? 0 : (n > Tmax ? Tmax : n);
+  }
 }
 
 // out[c][t] = philox_normal(seed, stream, c0 + c, frame0 + t): the draws the kernels above make, as a tensor
