@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../include/ovc.h"
+#include "ovc_convpack.h"
 #include "ovc_small.cuh"
 #include "ovc_tcconv.cuh"
 #include "ovc_tts.cuh"
@@ -333,27 +334,13 @@ static ConvLayer pack_conv(ovc_ctx* c, int variant, int rows, int cin, WF wfun, 
   L.n_chunks = (cin + vi.CI_CH - 1) / vi.CI_CH;
   L.K = trueK;
   L.cout = cout;
-  const int cin_pad = L.n_chunks * vi.CI_CH;
   L.w_off = round_up(c->h_w.size(), 64);   // 256-byte aligned blobs (TMA bulk needs 16)
-  c->h_w.resize(L.w_off + (size_t)L.row_tiles * cin_pad * vi.K * vi.CO_T, 0.f);
-  float* dst = c->h_w.data() + L.w_off;
-  for (int rt = 0; rt < L.row_tiles; ++rt)
-    for (int ci = 0; ci < cin_pad; ++ci)
-      for (int k = 0; k < vi.K; ++k)
-        for (int r = 0; r < vi.CO_T; ++r)
-          dst[(((size_t)rt * cin_pad + ci) * vi.K + k) * vi.CO_T + r] =
-              ci < cin ? wfun(rt * vi.CO_T + r, ci, k) : 0.f;
+  c->h_w.resize(L.w_off + conv_packed_floats(rows, cin, vi.K, vi.CO_T, vi.CI_CH), 0.f);
+  conv_pack_weights(c->h_w.data() + L.w_off, rows, cin, vi.K, vi.CO_T, vi.CI_CH, wfun);
   L.b_off = round_up(c->h_w.size(), 64);
   c->h_w.resize(L.b_off + bias_rows, 0.f);
   for (int r = 0; r < bias_rows; ++r) c->h_w[L.b_off + r] = bfun(r);
   return L;
-}
-
-// packed row -> original row for the paired (tanh|sigmoid, m|logs) layouts: a thread's 8 rows
-// are 4 channels of the first half followed by the same 4 channels of the second half
-static inline int paired_row(int p, int half) {
-  const int q = p / 8, r = p % 8;
-  return r < 4 ? 4 * q + r : half + 4 * q + (r - 4);
 }
 
 // column order of the tensor-core WN gate: every 32-column group = 16 tanh rows then their 16 sigmoid partners
@@ -507,7 +494,7 @@ static int finalize(ovc_ctx* c) {
   }
   int ch = 512;
   for (int i = 0; i < 4; ++i) {
-    const int s = hp.upsample_rates[i], kk = hp.upsample_kernel_sizes[i], pad = (kk - s) / 2;
+    const int s = hp.upsample_rates[i], kk = hp.upsample_kernel_sizes[i];
     const int cin = ch, cout = ch / 2;
     const std::string p = "dec.ups." + std::to_string(i);
     HostTensor w;   // [cin][cout][kk], weight-norm over dim 0 = cin (SURVEY appendix C.12)
@@ -515,19 +502,13 @@ static int finalize(ovc_ctx* c) {
     TRY(conv_weight(c, p, {cin, cout, kk}, &w));
     TRY(tensor(c, p + ".bias", {cout}, &b));
     const int variant = s == 8 ? V_UPS8_A : (cout * s >= 128 ? V_UPS2_A : V_UPS2_B);
-    // polyphase: out[co, s*n+ph] = sum_ci sum_m x[ci, n-m] * W[ci, co, s*m + ph + pad];
-    // packed row = co*s + ph, tap 0/1/2 <-> x[n-1], x[n], x[n+1] <-> m = 1, 0, -1
+    auto raw = [&](int ci, int co, int k) { return w.data[((size_t)ci * cout + co) * kk + k]; };
+    // polyphase (ovc_convpack.h): packed row = co*s + ph, tap 0/1/2 <-> x[n-1], x[n], x[n+1]
     c->dec_ups[i] = pack_conv(
-        c, variant, cout * s, cin,
-        [&](int row, int ci, int tap) {
-          const int co = row / s, ph = row % s;
-          const int kidx = s * (1 - tap) + ph + pad;
-          return (kidx >= 0 && kidx < kk) ? w.data[((size_t)ci * cout + co) * kk + kidx] : 0.f;
-        },
+        c, variant, cout * s, cin, [&](int row, int ci, int tap) { return conv_ups_weight(raw, s, kk, row, ci, tap); },
         [&](int co) { return b->data[co]; }, cout, 2, cout);
     c->dec_ups[i].out_mul = s;
     // tensor-core form: channels-last, row = ph * cout + co, so input step n yields the s output rows s*n .. s*n+s-1
-    auto raw = [&](int ci, int co, int k) { return w.data[((size_t)ci * cout + co) * kk + k]; };
     c->tc_ups[i] = pack_tc(
         c, s * cout, cin, 3, 1, [&](int row, int ci, int tap) { return tc_ups_weight(raw, s, kk, cout, row, ci, tap); },
         [&](int row) { return b->data[row % cout]; });
