@@ -25,10 +25,11 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 7  /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 8  /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
-                               * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows */
+                               * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
+                               * 8: ovc_spectrogram_ring */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -172,6 +173,20 @@ OVC_API int ovc_philox_normals(uint64_t seed, int64_t stream, int64_t c0, int C,
  *   frames       [B] int64 out (nullable): min(Tmax, wav_lengths[b] / hop)                          */
 OVC_API int ovc_spectrogram(ovc_ctx* ctx, const float* wav, const int64_t* wav_lengths, int B, int Lmax,
                             int Tmax, float* spec, int64_t* frames, void* stream);
+
+/* Magnitude-spectrogram frames of streams held in device audio rings (sample s of row r at
+ * rings[r*ring_cap + s % ring_cap]), the front end of batched live streaming: many streams' window spectrograms in one launch, no gather in between.
+ * Item b: frames [frame_lo[b], frame_lo[b] + frames[b]) of row[b] -> spec[b, :, 0:frames[b]], zeros up to Tmax.
+ * stream_len[b]: samples of the whole stream, or INT64_MAX while it is open (reflect padding at the end only once closed).
+ * Each frame is the ovc_spectrogram frame of the whole stream bit for bit, provided the ring row holds every sample the
+ * frame reads (frame t: samples [t*hop - 384, t*hop + 640), reflected at the stream's ends).
+ *   rings       [ring_rows, ring_cap] fp32 (device), ring_cap >= 1024
+ *   row, frame_lo, frames, stream_len   [B] int64 (device); read on the device and clamped so that no read leaves rings
+ *   spec        [B, spec_channels, Tmax] out: exactly the `spec` ovc_voice_conversion(_items) reads
+ * Same STFT as ovc_spectrogram (n_fft = win = 1024, hop 256).  Only enqueues on `stream`. */
+OVC_API int ovc_spectrogram_ring(ovc_ctx* ctx, const float* rings, int ring_rows, int64_t ring_cap, const int64_t* row,
+                                 const int64_t* frame_lo, const int64_t* frames, const int64_t* stream_len,
+                                 int B, int Tmax, float* spec, void* stream);
 
 /* ToneColorConverter.convert's device work in one call (openvoice/api.py:148-155, batch of B):
  * spectrogram -> voice_conversion with per-item exact lengths (ragged).  Tmax = Lmax / hop.

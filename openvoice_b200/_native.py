@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -22,10 +22,10 @@ EXPORTS = (
     "ovc_tts_info", "ovc_tts_encode", "ovc_tts_decode", "ovc_set_option", "ovc_graph_replays",
     "ovc_reference_encoder_ragged", "ovc_resample", "ovc_resample_span", "ovc_voice_conversion_items",
     "ovc_convert_waveform_items", "ovc_tts_encode_items", "ovc_tts_decode_items", "ovc_philox_normals",
-    "ovc_tts_encode_state", "ovc_tts_decode_windows",
+    "ovc_tts_encode_state", "ovc_tts_decode_windows", "ovc_spectrogram_ring",
 )
 
-STREAM_OPEN = 2 ** 63 - 1   # ovc_resample input length of a stream that has not ended
+STREAM_OPEN = 2 ** 63 - 1   # ovc_resample / ovc_spectrogram_ring length of a stream that has not ended
 
 
 class OvcHParams(C.Structure):
@@ -129,6 +129,8 @@ def load_library(path: Optional[str] = None):
     lib.ovc_debug_fetch.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64)]
     lib.ovc_spectrogram.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                     C.c_void_p, C.c_void_p]
+    lib.ovc_spectrogram_ring.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.ovc_convert_waveform.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_uint64, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.ovc_tts_info.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
@@ -282,10 +284,11 @@ class NativeConverter:
 
     # ---- hot path --------------------------------------------------------------------------
     def voice_conversion(self, spec, lengths, g_src, g_tgt, noise=None, tau: float = 0.3, seed: int = 0,
-                         ragged: bool = False, latents: bool = True, stream=None, items: Optional[dict] = None):
+                         ragged: bool = False, latents: bool = True, stream=None, items: Optional[dict] = None, out=None):
         """spec [B,S,T] f32 cuda, lengths [B] i64 cuda, g_* [B,gin(,1)] f32 cuda.
         Returns (o_hat [B,1,hop*T], (z, z_p, z_hat) or None).  Asynchronous on `stream`.  ``items``: per-item
-        parameters ``{"seed", "stream", "frame0", "tau": [B] cuda tensor}`` (see ``item_params``), or None."""
+        parameters ``{"seed", "stream", "frame0", "tau": [B] cuda tensor}`` (see ``item_params``), or None.  ``out``:
+        a caller-owned o_hat buffer of B * hop * T floats (a repeated call on stable buffers replays its CUDA graph)."""
         import torch
         assert spec.is_cuda and spec.dtype == torch.float32 and spec.is_contiguous()
         assert lengths.is_cuda and lengths.dtype == torch.int64 and lengths.is_contiguous()
@@ -296,7 +299,11 @@ class NativeConverter:
             noise = noise.contiguous().float()
             assert tuple(noise.shape) == (B, self.hp.inter_channels, T)
         hop = self.hp.hop_length
-        o = torch.empty(B, 1, hop * T, device=spec.device, dtype=torch.float32)
+        if out is not None:
+            assert out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == B * hop * T
+            o = out.view(B, 1, hop * T)
+        else:
+            o = torch.empty(B, 1, hop * T, device=spec.device, dtype=torch.float32)
         lat = None
         if latents:
             lat = tuple(torch.empty(B, self.hp.inter_channels, T, device=spec.device, dtype=torch.float32)
@@ -327,6 +334,31 @@ class NativeConverter:
                                       C.c_void_p(spec.data_ptr()), C.c_void_p(frames.data_ptr()), C.c_void_p(st.cuda_stream))
         _check(self.lib, rc, "ovc_spectrogram")
         return spec, frames
+
+    def spectrogram_ring(self, rings, row, frame_lo, frames, stream_len, Tmax: int, out=None, stream=None):
+        """Spectrogram windows of streams held in device audio rings (include/ovc.h: ovc_spectrogram_ring).
+        rings [R, cap] f32 cuda: sample s of the stream in row r at rings[r, s % cap].  row, frame_lo, frames,
+        stream_len: [B] i64 cuda; item b is frames [frame_lo[b], frame_lo[b] + frames[b]) of row[b], with reflect padding
+        at the end only when stream_len[b] != STREAM_OPEN.  Returns spec [B, S, Tmax] (zeros past frames[b]), written
+        into ``out`` when given.  Asynchronous on `stream`."""
+        import torch
+        assert rings.is_cuda and rings.dtype == torch.float32 and rings.is_contiguous() and rings.dim() == 2
+        B = row.numel()
+        for t in (row, frame_lo, frames, stream_len):
+            assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()
+            if tuple(t.shape) != (B,):
+                raise ValueError(f"spectrogram_ring: per-item arrays need shape ({B},), got {tuple(t.shape)}")
+        shape = (B, self.hp.spec_channels, int(Tmax))
+        if out is None:
+            out = torch.empty(shape, device=rings.device, dtype=torch.float32)
+        assert out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == shape
+        st = stream if stream is not None else torch.cuda.current_stream(rings.device)
+        p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+        rc = self.lib.ovc_spectrogram_ring(self.handle, p(rings), int(rings.shape[0]), int(rings.shape[1]), p(row),
+                                           p(frame_lo), p(frames), p(stream_len), B, int(Tmax), p(out),
+                                           C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_spectrogram_ring")
+        return out
 
     def convert_waveform(self, wav, wav_lengths, g_src, g_tgt, noise=None, tau: float = 0.3, seed: int = 0, stream=None,
                          out=None, frames_out=None, items: Optional[dict] = None):

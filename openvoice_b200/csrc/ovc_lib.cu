@@ -1516,6 +1516,29 @@ int ovc_spectrogram(ovc_ctx* c, const float* wav, const int64_t* wav_lengths, in
   return launch_stft(c, wav, wav_lengths, B, Lmax, Tmax, spec, Tmax, (long long*)frames, (cudaStream_t)stream);
 }
 
+static_assert(RING_OPEN == INT64_MAX, "ovc_spectrogram_ring: INT64_MAX marks an open stream");
+
+int ovc_spectrogram_ring(ovc_ctx* c, const float* rings, int ring_rows, int64_t ring_cap, const int64_t* row,
+                         const int64_t* frame_lo, const int64_t* frames, const int64_t* stream_len, int B, int Tmax,
+                         float* spec, void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
+  if (!rings || !row || !frame_lo || !frames || !stream_len || !spec) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (B < 1 || Tmax < 1 || B > 65535 || ring_rows < 1)
+    return fail(OVC_ERR_INVALID, "bad sizes B=%d Tmax=%d ring_rows=%d", B, Tmax, ring_rows);
+  if (ring_cap < STFT_N) return fail(OVC_ERR_INVALID, "ring_cap %lld is below one FFT frame (%d)", (long long)ring_cap, STFT_N);
+  if (c->hp.spec_channels != STFT_N / 2 + 1 || c->hp.hop_length != 256)
+    return fail(OVC_ERR_INVALID, "the STFT kernel is specialised for n_fft = win_length = 1024, hop 256");
+  ON_DEVICE(c);
+  dim3 grid((Tmax + STFT_FR - 1) / STFT_FR, B);
+  stft_ring_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(rings, (long long)ring_cap, ring_rows, (const long long*)row,
+                                                           (const long long*)frame_lo, (const long long*)frames,
+                                                           (const long long*)stream_len, c->hp.hop_length, spec, Tmax,
+                                                           c->d_tw, c->d_win);
+  CK(cudaGetLastError());
+  return OVC_OK;
+}
+
 int ovc_convert_waveform(ovc_ctx* c, const float* wav, const int64_t* wav_lengths, int B, int Lmax, const float* g_src,
                          const float* g_tgt, const float* noise, uint64_t seed, float tau, float* o_hat, int64_t* frames,
                          void* stream) {

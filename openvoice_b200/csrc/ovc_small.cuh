@@ -118,31 +118,20 @@ __global__ void __launch_bounds__(256) copy_latent_kernel(const float* __restric
 // ---------------------------------------------------------------------------------------------
 constexpr int STFT_N = 1024, STFT_FR = 8;
 
-__global__ void __launch_bounds__(256) stft_mag_kernel(const float* __restrict__ wav, long long wav_bs,
-                                                       const long long* __restrict__ wav_len, int hop,
-                                                       float* __restrict__ spec, long long spec_bs, int spec_pitch,
-                                                       int Tmax, const float2* __restrict__ tw,
-                                                       const float* __restrict__ win, long long* __restrict__ frames_out) {
+// The per-CTA body both STFT kernels instantiate: columns [t0, t0 + 8) of one item, column t < T transformed from the
+// samples load(t, n), n < 1024 (window applied here), columns T .. Tmax-1 written as zeros.
+template <class Load>
+__device__ __forceinline__ void stft_block(const Load& load, int T, int t0, float* __restrict__ sp, int spec_pitch, int Tmax,
+                                           const float2* __restrict__ tw, const float* __restrict__ win) {
   __shared__ float2 buf[2][STFT_N];
   __shared__ float mag[STFT_N / 2 + 1][STFT_FR + 1];
   __shared__ float2 tws[STFT_N];
-  const int tid = threadIdx.x, b = blockIdx.y, t0 = blockIdx.x * STFT_FR;
-  const int L = (int)wav_len[b];
-  const int T = min(Tmax, L / hop);
-  if (blockIdx.x == 0 && tid == 0 && frames_out) frames_out[b] = T;
+  const int tid = threadIdx.x;
   for (int i = tid; i < STFT_N; i += 256) tws[i] = tw[i];
-  const float* w = wav + (size_t)b * wav_bs;
-  const int pad = (STFT_N - hop) / 2;
   for (int fr = 0; fr < STFT_FR; ++fr) {
     const int t = t0 + fr;
     if (t < T) {   // block-uniform
-      for (int n = tid; n < STFT_N; n += 256) {
-        int idx = t * hop + n - pad;
-        if (idx < 0) idx = -idx;
-        if (idx >= L) idx = 2 * (L - 1) - idx;
-        idx = max(0, min(idx, L - 1));   // (callers guarantee L > 384; never read out of bounds regardless)
-        buf[0][n] = make_float2(w[idx] * win[n], 0.f);
-      }
+      for (int n = tid; n < STFT_N; n += 256) buf[0][n] = make_float2(load(t, n) * win[n], 0.f);
       __syncthreads();
       int src = 0;
 #pragma unroll
@@ -177,11 +166,67 @@ __global__ void __launch_bounds__(256) stft_mag_kernel(const float* __restrict__
     }
     __syncthreads();
   }
-  float* sp = spec + (size_t)b * spec_bs;
   for (int e = tid; e < (STFT_N / 2 + 1) * STFT_FR; e += 256) {
     const int f = e / STFT_FR, fr = e % STFT_FR;
     if (t0 + fr < Tmax) sp[(size_t)f * spec_pitch + t0 + fr] = mag[f][fr];
   }
+}
+
+__global__ void __launch_bounds__(256) stft_mag_kernel(const float* __restrict__ wav, long long wav_bs,
+                                                       const long long* __restrict__ wav_len, int hop,
+                                                       float* __restrict__ spec, long long spec_bs, int spec_pitch,
+                                                       int Tmax, const float2* __restrict__ tw,
+                                                       const float* __restrict__ win, long long* __restrict__ frames_out) {
+  const int b = blockIdx.y, t0 = blockIdx.x * STFT_FR;
+  const int L = (int)wav_len[b];
+  const int T = min(Tmax, L / hop);
+  if (blockIdx.x == 0 && threadIdx.x == 0 && frames_out) frames_out[b] = T;
+  const float* w = wav + (size_t)b * wav_bs;
+  const int pad = (STFT_N - hop) / 2;
+  const auto load = [&](int t, int n) {
+    int idx = t * hop + n - pad;
+    if (idx < 0) idx = -idx;
+    if (idx >= L) idx = 2 * (L - 1) - idx;
+    idx = max(0, min(idx, L - 1));   // (callers guarantee L > 384; never read out of bounds regardless)
+    return w[idx];
+  };
+  stft_block(load, T, t0, spec + (size_t)b * spec_bs, spec_pitch, Tmax, tw, win);
+}
+
+// ---------------------------------------------------------------------------------------------
+// stft_ring_kernel: stft_mag_kernel's frames read straight from per-stream audio rings, so many
+// live streams' window spectrograms come from one launch.  Sample s of the stream in row r lives
+// at rings[r * cap + s % cap].  Item b writes frames [lo[b], lo[b] + frames[b]) of row[b] into
+// columns 0 .. frames[b]-1 of spec[b] (zeros up to Tmax): the padded batch voice conversion reads.
+// Frame t reads samples t*hop + n - pad; negative indices reflect at the stream start, indices
+// at or past len[b] reflect at the stream end only once the stream has ended (len[b] !=
+// RING_OPEN).  Per-item values are clamped, so no read leaves the rings whatever they hold.
+// ---------------------------------------------------------------------------------------------
+constexpr long long RING_OPEN = 0x7fffffffffffffffLL;
+
+__global__ void __launch_bounds__(256) stft_ring_kernel(const float* __restrict__ rings, long long cap, int rows,
+                                                        const long long* __restrict__ row, const long long* __restrict__ lo,
+                                                        const long long* __restrict__ frames,
+                                                        const long long* __restrict__ len, int hop, float* __restrict__ spec,
+                                                        int Tmax, const float2* __restrict__ tw,
+                                                        const float* __restrict__ win) {
+  const int b = blockIdx.y, t0 = blockIdx.x * STFT_FR;
+  const long long r = max(0LL, min(row[b], (long long)rows - 1));
+  const long long f0 = max(0LL, min(lo[b], 1LL << 40));
+  const int T = (int)max(0LL, min(frames[b], (long long)Tmax));
+  const long long L = len[b] == RING_OPEN ? RING_OPEN : max(1LL, min(len[b], 1LL << 50));
+  const float* ring = rings + r * cap;
+  const long long pad = (STFT_N - hop) / 2;
+  const auto load = [&](int t, int n) {
+    long long idx = (f0 + t) * hop + n - pad;
+    if (idx < 0) idx = -idx;
+    if (L != RING_OPEN) {
+      if (idx >= L) idx = 2 * (L - 1) - idx;
+      idx = min(idx, L - 1);
+    }
+    return ring[max(idx, 0LL) % cap];
+  };
+  stft_block(load, T, t0, spec + (size_t)b * (STFT_N / 2 + 1) * Tmax, Tmax, Tmax, tw, win);
 }
 
 }  // namespace ovc

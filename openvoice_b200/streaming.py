@@ -25,13 +25,48 @@ rate and the converted audio back, each on the device, and each bit-identical to
 (no clicks at chunk boundaries).  The two filters add their look-ahead to the latency: 10 max(up, down) / up input
 samples each, 0.45 ms for 48 kHz -> 22.05 kHz and 0.45 ms for 22.05 kHz -> 48 kHz, 0.91 ms in all
 (``StreamingResampler.lookahead_s`` computes it from the library's span function).
+
+A server with many live callers uses ``StreamingSessions``: each session behaves exactly like its own
+``StreamingConverter(request_seed=...)``, but every ``push`` / ``close`` advances all the sessions it names with one
+batched launch sequence -- the sessions' audio lives in device rings, ``ovc_spectrogram_ring`` builds every ready
+window's spectrogram in one launch, and one ragged voice conversion converts them all.  ``ready_frames`` and
+``stream_windows`` are the readiness and window rules both classes follow.
 """
-from typing import Callable, Optional
+import math
+from typing import Callable, Dict, Iterable, List, Optional, Tuple
 
 import numpy as np
 import torch
 
 from ._native import STREAM_OPEN, resample_span
+
+
+def ready_frames(n_in: int, hop: int, nfft: int, final: bool) -> int:
+    """Spectrogram frames of a stream of ``n_in`` samples that can be computed: every frame whose STFT support
+    [t*hop - pad, t*hop - pad + nfft) has arrived, or all ``n_in // hop`` of them (right reflect padding) once the stream
+    has ended."""
+    if final:
+        return n_in // hop
+    pad = (nfft - hop) // 2
+    return min(max(0, (n_in + pad - nfft) // hop + 1), n_in // hop)
+
+
+def stream_windows(emitted: int, have: int, W: int, H: int, final: bool = False) -> List[Tuple[int, int, int, int]]:
+    """Windows (lo, hi, e0, e1) a stream converts next: frames [lo, hi) go into the call, the samples of frames [e0, e1)
+    come out.  An open stream converts a ``W``-frame window once ``emitted + W + H`` frames exist, over [e0 - H, e1 + H);
+    an ended stream (``final``, ``have`` = all its frames) converts the rest, the last windows clipped to its end."""
+    wins = []
+    while (emitted < have) if final else (emitted + W + H <= have):
+        e1 = min(have, emitted + W)
+        wins.append((max(0, emitted - H), min(have, e1 + H), emitted, e1))
+        emitted = e1
+    return wins
+
+
+def check_stream_length(n_in: int, hop: int, pad: int) -> None:
+    """ValueError for a stream that ends shorter than one hop or than the STFT reflect padding, as ``convert`` refuses."""
+    if n_in // hop < 1 or n_in <= pad:
+        raise ValueError("audio too short")
 
 
 class StreamingResampler:
@@ -164,11 +199,7 @@ class StreamingConverter:
         right reflect padding, when the stream ends)."""
         hop, pad = self.hop, self.pad
         have = self.f0 + self.spec.shape[2]               # next frame to compute
-        if final:
-            upto = self.n_in // hop
-        else:
-            upto = max(0, (self.n_in + pad - self.nfft) // hop + 1)
-            upto = min(upto, self.n_in // hop)
+        upto = ready_frames(self.n_in, hop, self.nfft, final)
         if upto <= have:
             return
         # segment of audio that gives frames [have, upto) away from its own reflect-padded ends: the native STFT pads
@@ -192,10 +223,8 @@ class StreamingConverter:
             self.audio = self.audio[keep_from - self.a0:]
             self.a0 = keep_from
 
-    def _convert_window(self, e0: int, e1: int, t_end: Optional[int]) -> np.ndarray:
-        """Samples of frames [e0, e1): one ragged batch-1 call over [e0 - H, e1 + H) clipped to the stream."""
-        lo = max(0, e0 - self.H)
-        hi = e1 + self.H if t_end is None else min(t_end, e1 + self.H)
+    def _convert_window(self, lo: int, hi: int, e0: int, e1: int) -> np.ndarray:
+        """Samples of frames [e0, e1): one ragged batch-1 call over the window's frames [lo, hi)."""
         sp = self.spec[:, :, lo - self.f0: hi - self.f0].contiguous()
         lens = torch.tensor([hi - lo], dtype=torch.int64, device=self.dev)
         if self.request_seed is None:
@@ -241,20 +270,262 @@ class StreamingConverter:
         self.audio = np.concatenate([self.audio, x])
         self.n_in += len(x)
         self._extend_spec(final=False)
-        outs = []
         have = self.f0 + self.spec.shape[2]
-        while self.emitted + self.W + self.H <= have:
-            outs.append(self._convert_window(self.emitted, self.emitted + self.W, None))
+        outs = [self._convert_window(*w) for w in stream_windows(self.emitted, have, self.W, self.H)]
         return np.concatenate(outs) if outs else np.zeros(0, dtype=np.float32)
 
     def _flush(self) -> np.ndarray:
         self.closed = True
-        T = self.n_in // self.hop
-        if T < 1 or self.n_in <= self.pad:
-            raise ValueError("audio too short")       # shorter than one hop / the STFT reflect padding, like convert
+        check_stream_length(self.n_in, self.hop, self.pad)
         self._extend_spec(final=True)
-        outs = []
-        while self.emitted < T:
-            e1 = min(T, self.emitted + self.W)
-            outs.append(self._convert_window(self.emitted, e1, T))
+        T = self.n_in // self.hop
+        outs = [self._convert_window(*w) for w in stream_windows(self.emitted, T, self.W, self.H, final=True)]
         return np.concatenate(outs) if outs else np.zeros(0, dtype=np.float32)
+
+
+# Padded frames (windows x Tmax) of one voice-conversion launch of ``StreamingSessions``: a step whose windows exceed it
+# runs several launches.  64 sessions' 256-frame windows with both 128-frame halos (64 x 512) fill one launch, about the
+# converter workspace of ``convert_batch``'s 64-item batches of 10 s clips.
+SESSION_BATCH_FRAMES = 32768
+
+
+class _Session:
+    __slots__ = ("row", "seed", "tau", "n_in", "emitted")
+
+    def __init__(self, row: int, seed: int, tau: float):
+        self.row, self.seed, self.tau = row, seed, tau
+        self.n_in = 0                                     # samples received
+        self.emitted = 0                                  # frames whose samples have been returned
+
+
+class StreamingSessions:
+    """Many live streams through one converter, advanced together.
+
+    ``open`` starts a session and returns its id; ``push({id: samples, ...})`` feeds any number of sessions and returns
+    ``{id: float32 samples that became final}``; ``close(ids)`` ends sessions and returns the rest of their audio.  Each
+    session's output equals ``StreamingConverter(converter, src_se, tgt_se, tau, window_frames, request_seed=seed)`` fed
+    the same chunks, bit for bit, whatever else runs beside it: the windows follow ``stream_windows``, the spectrogram
+    frames are those of the whole clip, and each window draws its noise at its own seed and absolute frames.
+
+    Every ``push`` / ``close`` is one step: one packed upload (the pushed samples and every per-window value), one
+    scatter of the samples into the sessions' device audio rings, one ``ovc_spectrogram_ring`` over every ready window of
+    every session in the call, one gather of their embeddings from a device table, ragged voice conversions of up to
+    ``SESSION_BATCH_FRAMES`` padded frames each (one for a typical step), one gather of the emitted frames, one download
+    and one synchronisation.  Buffers are grow-only and the padded window length is rounded up to 16 frames, so a steady
+    lockstep step replays its CUDA graph.  A session keeps the audio of its next window and both halos, plus the STFT
+    support and its largest push, on the device.
+
+    Noise is drawn in-kernel from each session's seed (no ``noise_fn``); audio is at the model's rate (use
+    ``StreamingConverter`` with ``input_sr`` / ``output_sr`` to resample a single stream)."""
+
+    def __init__(self, converter, window_frames: int = 256):
+        W = int(window_frames)
+        if W < 1:
+            raise ValueError(f"window_frames must be >= 1, got {window_frames!r}")
+        hp = converter.hps
+        self.native = converter.model.native
+        self.sr = int(hp.data.sampling_rate)
+        self.hop = hp.data.hop_length
+        self.nfft = hp.data.filter_length
+        self.pad = (self.nfft - self.hop) // 2
+        self.S = self.nfft // 2 + 1
+        self.gin = int(getattr(hp.model, "gin_channels", 256))
+        self.H = converter.HALO_FRAMES
+        self.W = W
+        self.dev = torch.device(converter.device)
+        self.cuda = self.dev.type == "cuda"
+        self.sessions: Dict[int, _Session] = {}
+        self.free_rows: List[int] = []
+        self.rows = 0
+        self.cap = self.hop * (W + 2 * self.H + 8) + 4096   # samples per ring row; grows for larger pushes
+        self.rings = torch.zeros(0, self.cap, device=self.dev)
+        self.se = torch.zeros(2, 0, self.gin, device=self.dev)   # [src | tgt, row, gin]
+        self.next_id = 0
+        self._bufs: dict = {}
+        self._h2d_done = None
+
+    # ------------------------------------------------------------------ sessions
+    def open(self, src_se, tgt_se, tau: float = 0.3, seed: Optional[int] = None, input_sr: Optional[int] = None,
+             output_sr: Optional[int] = None) -> int:
+        """Start a session converting from ``src_se`` to ``tgt_se`` (tone-colour embeddings of ``gin`` values each) and
+        return its id.  ``seed``: the session's Philox key in [0, 2^64) (default: drawn from torch's generator).
+        ``input_sr`` / ``output_sr`` other than the model's rate are refused."""
+        from .api import check_seeds
+        for name, rate in (("input_sr", input_sr), ("output_sr", output_sr)):
+            if rate is not None and int(rate) != self.sr:
+                raise ValueError(f"{name}={rate}: StreamingSessions takes and returns audio at the model's rate "
+                                 f"({self.sr} Hz); StreamingConverter resamples a single stream")
+        tau = float(tau)
+        if not math.isfinite(tau):
+            raise ValueError(f"tau = {tau!r} is not a finite number")
+        seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None else check_seeds([seed], 1, "seed")[0]
+        ses = []
+        for name, se in (("src_se", src_se), ("tgt_se", tgt_se)):
+            se = torch.as_tensor(se, dtype=torch.float32).reshape(-1)
+            if se.numel() != self.gin:
+                raise ValueError(f"{name} has {se.numel()} values, the model's embeddings have {self.gin}")
+            ses.append(se)
+        if not self.free_rows:
+            rows = self.rows + max(1, self.rows // 2)
+            self.free_rows += range(self.rows, rows)
+            self._grow(rows, self.cap, [])
+        row = min(self.free_rows)
+        self.free_rows.remove(row)
+        self.se[:, row] = torch.stack(ses).to(self.dev)
+        sid = self.next_id
+        self.next_id += 1
+        self.sessions[sid] = _Session(row, seed, tau)
+        return sid
+
+    @property
+    def rows_in_use(self) -> int:
+        return len(self.sessions)
+
+    def state_samples(self, sid: int) -> int:
+        """Samples of session ``sid`` still held in its ring row (the ones its next windows read)."""
+        s = self.sessions[sid]
+        return s.n_in - self._keep_from(s)
+
+    def _keep_from(self, s: _Session) -> int:
+        """First sample of the session's next window: frame max(0, emitted - H) reads from (that frame) * hop - pad."""
+        return max(0, (s.emitted - self.H) * self.hop - self.pad)
+
+    def _check_ids(self, ids) -> List[int]:
+        ids = list(ids)
+        for sid in ids:
+            if sid not in self.sessions:
+                raise ValueError(f"unknown or closed session {sid!r}")
+        if len(set(ids)) != len(ids):
+            raise ValueError("a session is named twice")
+        return ids
+
+    # ------------------------------------------------------------------ public steps
+    @torch.no_grad()
+    def push(self, chunks: Dict[int, object]) -> Dict[int, np.ndarray]:
+        """Append ``chunks[id]`` (float32 samples at the model's rate) to each named session; returns, per named session,
+        the converted samples that became final (possibly none)."""
+        ids = self._check_ids(chunks.keys())
+        xs = {sid: np.asarray(chunks[sid], dtype=np.float32).reshape(-1) for sid in ids}
+        return self._step(xs, final=False)
+
+    @torch.no_grad()
+    def close(self, ids: Iterable[int]) -> Dict[int, np.ndarray]:
+        """End the named sessions: converts what is left of each (right reflect padding at its end, like the whole-clip
+        spectrogram) and frees their rows.  A session shorter than one hop or than the STFT padding raises ValueError,
+        like ``StreamingConverter.flush``; nothing is changed then."""
+        ids = self._check_ids(ids)
+        for sid in ids:
+            check_stream_length(self.sessions[sid].n_in, self.hop, self.pad)
+        out = self._step({sid: np.zeros(0, dtype=np.float32) for sid in ids}, final=True)
+        for sid in ids:
+            self.free_rows.append(self.sessions.pop(sid).row)
+        return out
+
+    # ------------------------------------------------------------------ device buffers
+    def _buf(self, name: str, numel: int, dtype, pinned: bool = False):
+        """Grow-only buffers: stable addresses, so repeated step shapes replay their CUDA graphs."""
+        b = self._bufs.get(name)
+        if b is None or b.numel() < numel:
+            b = torch.empty(int(numel * 1.25) + 64, dtype=dtype, device="cpu" if pinned else self.dev)
+            b = b.pin_memory() if pinned and self.cuda else b
+            self._bufs[name] = b
+        return b[:numel]
+
+    def _grow(self, rows: int, cap: int, live: List[Tuple[int, int, int]]):
+        """Reallocate the rings as [rows, cap] (and the embedding table as [2, rows, gin]), moving each live session's
+        samples [a, b) of row r (``live``: (r, a, b)) to their places under the new capacity."""
+        rings = torch.zeros(rows, cap, device=self.dev)
+        if live:
+            src = np.concatenate([r * self.cap + np.arange(a, b) % self.cap for r, a, b in live])
+            dst = np.concatenate([r * cap + np.arange(a, b) % cap for r, a, b in live])
+            rings.view(-1)[torch.from_numpy(dst).to(self.dev)] = self.rings.reshape(-1)[torch.from_numpy(src).to(self.dev)]
+        else:
+            rings[: self.rows] = self.rings
+        se = torch.zeros(2, rows, self.gin, device=self.dev)
+        se[:, : self.rows] = self.se
+        self.rings, self.se, self.rows, self.cap = rings, se, rows, cap
+
+    # ------------------------------------------------------------------ one step
+    def _step(self, xs: Dict[int, np.ndarray], final: bool) -> Dict[int, np.ndarray]:
+        hop, H = self.hop, self.H
+        ses = [(sid, self.sessions[sid], xs[sid]) for sid in xs]
+        need = max([s.n_in + len(x) - self._keep_from(s) for _, s, x in ses], default=0)
+        if need > self.cap:
+            cap = -(-int(need * 1.25) // hop) * hop
+            self._grow(self.rows, cap, [(s.row, self._keep_from(s), s.n_in) for s in self.sessions.values()])
+        # windows of every named session: (session index, lo, hi, e0, e1)
+        wins = []
+        for i, (_, s, x) in enumerate(ses):
+            n = s.n_in + len(x)
+            have = ready_frames(n, hop, self.nfft, final)
+            wins += [(i,) + w for w in stream_windows(s.emitted, have, self.W, H, final)]
+        B, Ns = len(wins), sum(len(x) for _, _, x in ses)
+        Tmax = -(-max([hi - lo for _, lo, hi, _, _ in wins], default=1) // 16) * 16
+        Nf = sum(e1 - e0 for _, _, _, e0, e1 in wins)
+        # packed upload (int64 words): row, lo, frames, stream length, seed, stream (0), embedding rows (2B), tau (float32),
+        # then the emitted frames' rows of the output, the ring positions of the pushed samples and the samples (float32)
+        nt = (B + 1) // 2
+        n_words = 8 * B + nt + Nf + Ns + (Ns + 1) // 2
+        if self._h2d_done is not None:
+            self._h2d_done.synchronize()                  # the previous step's upload has left the pinned buffer
+        pin = self._buf("pin", n_words, torch.int64, pinned=True)
+        w = pin.numpy()
+        if B:
+            ii = np.asarray([i for i, _, _, _, _ in wins])
+            rows = np.asarray([s.row for _, s, _ in ses], dtype=np.int64)[ii]
+            lo = np.asarray([v[1] for v in wins], dtype=np.int64)
+            w[0:B], w[B:2 * B], w[2 * B:3 * B] = rows, lo, [hi - l for _, l, hi, _, _ in wins]
+            w[3 * B:4 * B] = [ses[i][1].n_in + len(ses[i][2]) if final else STREAM_OPEN for i in ii]
+            from .api import seed_array
+            w[4 * B:5 * B] = seed_array([ses[i][1].seed for i in ii])
+            w[5 * B:6 * B] = 0
+            w[6 * B:7 * B], w[7 * B:8 * B] = rows, rows + self.rows
+            w[8 * B:8 * B + nt].view(np.float32)[:B] = [ses[i][1].tau for i in ii]
+            o = 8 * B + nt
+            w[o:o + Nf] = np.concatenate([b * Tmax + np.arange(e0 - l, e1 - l) for b, (_, l, _, e0, e1) in enumerate(wins)])
+        o = 8 * B + nt + Nf
+        if Ns:
+            w[o:o + Ns] = np.concatenate([s.row * self.cap + np.arange(s.n_in, s.n_in + len(x)) % self.cap
+                                          for _, s, x in ses if len(x)])
+            w[o + Ns:].view(np.float32)[:Ns] = np.concatenate([x for _, _, x in ses])
+        d = self._buf("up", n_words, torch.int64)
+        d.copy_(pin, non_blocking=True)
+        if self.cuda:
+            self._h2d_done = torch.cuda.Event()
+            self._h2d_done.record(torch.cuda.current_stream(self.dev))
+        if Ns:
+            self.rings.view(-1).index_copy_(0, d[o:o + Ns], d[o + Ns:].view(torch.float32)[:Ns])
+        res = {sid: np.zeros(0, dtype=np.float32) for sid, _, _ in ses}
+        if B:
+            spec = self._buf("spec", B * self.S * Tmax, torch.float32).view(B, self.S, Tmax)
+            self.native.spectrogram_ring(self.rings, d[0:B], d[B:2 * B], d[2 * B:3 * B], d[3 * B:4 * B], Tmax, out=spec)
+            g = torch.index_select(self.se.view(-1, self.gin), 0, d[6 * B:8 * B],
+                                   out=self._buf("g", 2 * B * self.gin, torch.float32).view(2 * B, self.gin))
+            obuf = self._buf("o", B * Tmax * hop, torch.float32)
+            per = max(1, SESSION_BATCH_FRAMES // Tmax)
+            taus = d[8 * B:8 * B + nt].view(torch.float32)[:B]
+            for b0 in range(0, B, per):
+                b1 = min(B, b0 + per)
+                items = {"seed": d[4 * B + b0:4 * B + b1], "stream": d[5 * B + b0:5 * B + b1],
+                         "frame0": d[B + b0:B + b1], "tau": taus[b0:b1]}
+                self.native.voice_conversion(spec[b0:b1], d[2 * B + b0:2 * B + b1], g[b0:b1], g[B + b0:B + b1],
+                                             ragged=True, latents=False, items=items,
+                                             out=obuf[b0 * Tmax * hop:b1 * Tmax * hop])
+            fo = 8 * B + nt
+            y = torch.index_select(obuf.view(B * Tmax, hop), 0, d[fo:fo + Nf],
+                                   out=self._buf("y", Nf * hop, torch.float32).view(Nf, hop))
+            host = self._buf("host", Nf * hop, torch.float32, pinned=True)
+            host.copy_(y.view(-1), non_blocking=True)
+            if self.cuda:
+                torch.cuda.current_stream(self.dev).synchronize()
+            y = host.numpy()
+            at, per_ses = 0, {}
+            for i, _, _, e0, e1 in wins:
+                per_ses.setdefault(i, []).append(y[at * hop:(at + e1 - e0) * hop])
+                at += e1 - e0
+            for i, parts in per_ses.items():
+                res[ses[i][0]] = np.concatenate(parts)
+        for i, (_, s, x) in enumerate(ses):
+            s.n_in += len(x)
+            s.emitted = max([e1 for j, _, _, _, e1 in wins if j == i], default=s.emitted)
+        return res
