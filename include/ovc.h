@@ -25,11 +25,11 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 8  /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 9  /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
-                               * 8: ovc_spectrogram_ring */
+                               * 8: ovc_spectrogram_ring; 9: OVC_OPT_PAIR_OCC */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -336,6 +336,9 @@ OVC_API int ovc_set_precision(ovc_ctx* ctx, int mode);
                               * MRF stage concurrently (three streams, a third of the SMs per kernel); results are bit-identical */
 #define OVC_OPT_PAIR 8       /* 1 (default): the HBM-bound ResBlock conv pairs (C <= 64, k = 3) run as ONE kernel each
                               * (tcconv_kernel<C, true>): the intermediate activation stays in shared memory */
+#define OVC_OPT_PAIR_OCC 9   /* 1 (default): the conv pairs of the C = 32 / 64 stages run two CTAs per SM where that is
+                              * measured faster (tc_pair_occ), so one tile's MMAs overlap another's epilogue; 0: one CTA
+                              * per SM everywhere.  Results are bit-identical */
 OVC_API int ovc_set_option(ovc_ctx* ctx, int key, int value);
 
 /* Number of kernels the last ovc_voice_conversion / ovc_convert_waveform call launched. */

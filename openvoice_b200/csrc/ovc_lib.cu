@@ -188,6 +188,8 @@ struct ovc_ctx {
   bool use_branches = true;
   int par_frames = 512;
   bool use_pair = true;        // OVC_OPT_PAIR: the ResBlock conv pairs of the C <= 128 stages as ONE kernel (tcconv_kernel<C, true>, tc_pair_fuses)
+  bool use_pair_occ = true;    // OVC_OPT_PAIR_OCC: pairs run two CTAs per SM where tc_pair_occ picks it
+  bool pair_occ2_ok[TCN_N_OCC2] = {};   // the device fits two CTAs per SM of kTcPairOcc2[i] (occupancy query at load)
   cudaStream_t br_stream[2] = {nullptr, nullptr};
   cudaEvent_t br_ev[4] = {nullptr, nullptr, nullptr, nullptr};
   size_t post_w_off = 0;
@@ -640,6 +642,18 @@ static int finalize(ovc_ctx* c) {
   CK(cudaFuncSetAttribute(tcconv_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<128, true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tcconv_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<64, true>::SMEM_BYTES));
   CK(cudaFuncSetAttribute(tcconv_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<32, true>::SMEM_BYTES));
+  for (int i = 0; i < TCN_N_OCC2; ++i) {
+    // a config runs two CTAs per SM only where the device confirms they fit: otherwise its pairs keep one CTA per SM
+    // (and a grid of one CTA per SM), never a doubled grid on one
+    const TcPairKernel k = tc_pair_kernel(kTcPairOcc2[i].C, kTcPairOcc2[i].o);
+    CK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem));
+    int blocks = 0;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, k.fn, TCN_THREADS, k.smem));
+    c->pair_occ2_ok[i] = blocks >= 2;
+    if (blocks < 2)
+      fprintf(stderr, "ovc: the C = %d conv-pair kernel with %d operand buffer(s) fits %d CTA(s) per SM, not 2; its pairs run "
+              "one CTA per SM\n", kTcPairOcc2[i].C, kTcPairOcc2[i].o.nabuf, blocks);
+  }
   if (c->d_cond_wrow) cudaFree(c->d_cond_wrow);
   if (c->d_cond_sel) cudaFree(c->d_cond_sel);
   CK(cudaMalloc(&c->d_cond_wrow, wrow.size() * sizeof(int)));
@@ -892,13 +906,16 @@ static int launch_pair(Run& r, const TcLayer& T1, const TcLayer& T2, const float
   a.Cin = C; a.Ntot = C; a.K = T1.K; a.DIL = T1.DIL;
   a.slope = slope; a.scale = scale; a.accumulate = accumulate;
   a.passes = r.c->precision == 2 ? 1 : 3;
-  const TcGrid g = tc_pair_grid(t_len, r.B, T1.K, r.c->sm_count);
+  TcPairOcc o = r.c->use_pair_occ ? tc_pair_occ(T1, T2) : TcPairOcc();
+  for (int i = 0; i < TCN_N_OCC2; ++i)
+    if (o.occ == 2 && kTcPairOcc2[i].C == C && kTcPairOcc2[i].o.nabuf == o.nabuf && !r.c->pair_occ2_ok[i]) o = TcPairOcc();
+  const TcPairKernel k = tc_pair_kernel(C, o);
+  if (!k.fn) return fail(OVC_ERR_INVALID, "no conv-pair kernel for C = %d at %d CTA(s) per SM, %d operand buffer(s)", C, o.occ, o.nabuf);
+  const TcGrid g = tc_pair_grid(t_len, r.B, T1.K, r.c->sm_count, o.occ);
   const int n_tt = g.n_tt, total = g.total;
   TRY(prof_begin(r));
   dim3 pg((unsigned)g.grid_x, 1, 1);
-  if (C == 128) CK(launch_ex(tcconv_kernel<128, true>, pg, TCN_THREADS, TcnCfg<128, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
-  else if (C == 64) CK(launch_ex(tcconv_kernel<64, true>, pg, TCN_THREADS, TcnCfg<64, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
-  else CK(launch_ex(tcconv_kernel<32, true>, pg, TCN_THREADS, TcnCfg<32, true>::SMEM_BYTES, r.st, false, a, n_tt, total));
+  CK(launch_ex(k.fn, pg, TCN_THREADS, k.smem, r.st, false, a, n_tt, total));
   CK(cudaGetLastError());
   r.c->launches++;
   const double units = (double)r.B * t_len;
@@ -1091,7 +1108,8 @@ static int set_call_params(ovc_ctx* c, uint64_t seed, float tau, const ItemParam
   return OVC_OK;
 }
 static uintptr_t option_bits(const ovc_ctx* c) {
-  return (uintptr_t)c->precision | ((uintptr_t)c->use_pdl << 15) | ((uintptr_t)c->use_branches << 14) | ((uintptr_t)c->use_pair << 17);
+  return (uintptr_t)c->precision | ((uintptr_t)c->use_pdl << 15) | ((uintptr_t)c->use_branches << 14) | ((uintptr_t)c->use_pair << 17) |
+         ((uintptr_t)c->use_pair_occ << 18);
 }
 
 static int ensure_ws(ovc_ctx* c, const WsLayout& W, int B, int Tmax, cudaStream_t st) {
@@ -1833,6 +1851,7 @@ int ovc_set_option(ovc_ctx* c, int key, int value) {
       return OVC_OK;
     case OVC_OPT_BRANCHES: c->use_branches = value != 0; return OVC_OK;
     case OVC_OPT_PAIR: c->use_pair = value != 0; return OVC_OK;
+    case OVC_OPT_PAIR_OCC: c->use_pair_occ = value != 0; return OVC_OK;
     default: return fail(OVC_ERR_INVALID, "unknown option %d", key);
   }
 }

@@ -18,7 +18,9 @@
 // K-major, no-swizzle operand tiles (see ovc_tc.cuh): a convolution tap is a 16-byte-per-row shift of the A
 // descriptor's start address, so all taps (any dilation) read ONE staged halo tile.
 //
-// tcconv_kernel<TN, PAIR>: persistent, one CTA (three warpgroups) per SM walks the (utterance, 128-step tile) list.
+// tcconv_kernel<TN, PAIR, OCC, NAB>: persistent, OCC CTAs (three warpgroups each) per SM walk the (utterance, 128-step
+// tile) list; OCC = 2 only for conv pairs of the C = 32 / 64 stages (tc_pair_occ), where a second CTA's MMAs run while
+// the first sits in an epilogue or at a named barrier.
 //   warp 0       weights by TMA bulk copies: resident in shared memory for the whole launch when they fit, else a ring
 //                streams them per tile
 //   warps 1-3    converters: global fp32 rows -> lrelu -> fp16 hi/lo split -> A operand layout, running ahead across
@@ -166,28 +168,31 @@ __device__ __forceinline__ void tc_mma_step(float (&d)[TN], uint64_t a_hi, uint6
 constexpr int TCN_THREADS = 384;   // warpgroup 0: producers; warpgroups 1, 2: MMAs + epilogue
 constexpr int TCN_NCT = 96;        // converter threads (warps 1-3)
 
-template <int TN, bool PAIR>
+// OCC: CTAs per SM (2: pairs of the C = 32 / 64 stages only, ovc_tcpack.h tc_pair_occ); NAB: conv-1 operand buffers
+template <int TN, bool PAIR, int OCC = 1, int NAB = 2>
 struct TcnCfg {
   static_assert(!PAIR || TN == 32 || TN == 64 || TN == 128, "conv pairs: C = 32, 64 or 128");
+  static_assert(OCC == 1 || (PAIR && TN <= 64), "two CTAs per SM: C = 32 / 64 pairs");
   static constexpr int KCH = 32, NKC = KCH / 8;                   // channels per converted A chunk
   static constexpr int ROWS = 194;                                // A pitch in rows: >= 128 + 2 * TCN_HMAX, = 2 (mod 8)
   static constexpr int ROWS2 = TCN_ROWS2;                         // PAIR: conv-2 A pitch: 128 + 2 * H2 rows, H2 <= 9
-  static constexpr int NABUF = 2;
-  static constexpr int RING = tc_ring_slots(TN, PAIR);            // weight slots (ovc_tcpack.h)
+  static constexpr int NABUF = NAB;
+  static constexpr int RING = PAIR ? tc_pair_ring(TN, OCC, NAB) : tc_ring_slots(TN, PAIR);   // weight slots (ovc_tcpack.h)
   static constexpr int SLOT_BYTES = 2 * 2 * TN * 16;
   static constexpr int A_BUF_BYTES = 2 * NKC * ROWS * 16;         // [hi|lo][column block][row][8 halfs]
   static constexpr int A2_BYTES = PAIR ? 2 * (TN / 8) * ROWS2 * 16 : 0;
   static constexpr size_t SMEM_BYTES = 1024 + NABUF * A_BUF_BYTES + A2_BYTES + RING * SLOT_BYTES;
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+  static_assert(!PAIR || SMEM_BYTES == tc_pair_smem(TN, NABUF, RING), "tc_pair_smem");
+  static_assert(SMEM_BYTES <= (OCC == 1 ? 232448 : TCN_SMEM_OCC2), "shared memory budget");
   static_assert((2 * NABUF + 2 * RING) * 8 <= 1024, "barrier area");
+  // registers per thread after the producers hand theirs to the MMA warpgroups: 128 x 56 + 256 x 224 = 64 K at one CTA
+  // per SM, 128 x 32 + 256 x 104 = 30 K (of the 32 K the launch bounds give a CTA) at two
+  static constexpr int PROD_REGS = OCC == 1 ? 56 : 32, MMA_REGS = OCC == 1 ? 224 : 104;
 };
 
-// registers per thread after the producers hand theirs to the MMA warpgroups (128 x 56 + 256 x 224 = 64 K)
-constexpr int TCN_PROD_REGS = 56, TCN_MMA_REGS = 224;
-
-template <int TN, bool PAIR>
-__global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs a, int n_tt, int total) {
-  using Cfg = TcnCfg<TN, PAIR>;
+template <int TN, bool PAIR, int OCC = 1, int NAB = 2>
+__global__ void __launch_bounds__(TCN_THREADS, OCC) tcconv_kernel(const TcConvArgs a, int n_tt, int total) {
+  using Cfg = TcnCfg<TN, PAIR, OCC, NAB>;
   constexpr int ROWS = Cfg::ROWS, ROWS2 = Cfg::ROWS2, NABUF = Cfg::NABUF, RING = Cfg::RING, NKC = Cfg::NKC;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
@@ -233,7 +238,7 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
     if (t0 >= lim) continue;
 
   if (warp < 4) {
-    tc::regs_dealloc<TCN_PROD_REGS>();
+    tc::regs_dealloc<Cfg::PROD_REGS>();
     if (warp == 0) {
       // ------------------------------------------------------------ weights
       if (lane == 0) {
@@ -313,7 +318,7 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
     }
   } else {
     // ------------------------------------------------------------ MMA warpgroups: rows [64 wg, +64) of every tile
-    tc::regs_alloc<TCN_MMA_REGS>();
+    tc::regs_alloc<Cfg::MMA_REGS>();
     const int wg = (warp >> 2) - 1;
     const bool leader = (tid & 127) == 0;
     const int row_a = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // this thread's first accumulator row
@@ -433,6 +438,27 @@ __global__ void __launch_bounds__(TCN_THREADS, 1) tcconv_kernel(const TcConvArgs
   }
 #undef TCN_FOR_TILES
 }
+
+// the pair-kernel instantiation of a (C, tc_pair_occ) config and its dynamic shared memory; fn = nullptr when none is built
+struct TcPairKernel {
+  void (*fn)(TcConvArgs, int, int) = nullptr;
+  size_t smem = 0;
+};
+inline TcPairKernel tc_pair_kernel(int C, TcPairOcc o) {
+  if (o.occ == 1 && o.nabuf == 2) {
+    if (C == 128) return {tcconv_kernel<128, true>, TcnCfg<128, true>::SMEM_BYTES};
+    if (C == 64) return {tcconv_kernel<64, true>, TcnCfg<64, true>::SMEM_BYTES};
+    if (C == 32) return {tcconv_kernel<32, true>, TcnCfg<32, true>::SMEM_BYTES};
+  } else if (o.occ == 2) {
+    if (C == 32 && o.nabuf == 2) return {tcconv_kernel<32, true, 2, 2>, TcnCfg<32, true, 2, 2>::SMEM_BYTES};
+    if (C == 32 && o.nabuf == 1) return {tcconv_kernel<32, true, 2, 1>, TcnCfg<32, true, 2, 1>::SMEM_BYTES};
+    if (C == 64 && o.nabuf == 1) return {tcconv_kernel<64, true, 2, 1>, TcnCfg<64, true, 2, 1>::SMEM_BYTES};
+  }
+  return {};
+}
+// the two-CTA-per-SM configs tc_pair_occ can pick
+constexpr int TCN_N_OCC2 = 3;
+constexpr struct { int C; TcPairOcc o; } kTcPairOcc2[TCN_N_OCC2] = {{32, {2, 2}}, {32, {2, 1}}, {64, {2, 1}}};
 
 // conv_post on channels-last input: y[b, t] = tanh(sum_{k<7, ci<C} w[ci, k] * lrelu_0.01(x[b, t+k-3, ci]))
 // (models.py:287-289).  HBM-bound (132 B per sample): a CTA stages 256+6 rows with coalesced 16-byte loads into a

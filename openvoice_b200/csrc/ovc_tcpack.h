@@ -119,15 +119,47 @@ inline TcGrid tc_grid(int t_len, int B, int Ntot, int TN, int sm_count, int grid
   g.grid_x = std::min(g.total, per_col);
   return g;
 }
-// conv pair: a tile is 128 conv-1 steps and yields R = 128 - (k - 1) output steps; one CTA per SM
-inline TcGrid tc_pair_grid(int t_len, int B, int K, int sm_count) {
+// conv pair: a tile is 128 conv-1 steps and yields R = 128 - (k - 1) output steps; occ CTAs per SM
+inline TcGrid tc_pair_grid(int t_len, int B, int K, int sm_count, int occ = 1) {
   TcGrid g;
   const int R = 128 - (K - 1);
   g.n_tt = (t_len + R - 1) / R;
   g.total = g.n_tt * B;
   g.ncol = 1;
-  g.grid_x = std::min(g.total, sm_count);
+  g.grid_x = std::min(g.total, occ * sm_count);
   return g;
+}
+
+// shared memory of one pair-kernel CTA (TcnCfg<TN, true, ...>): barriers, nabuf conv-1 operand buffers of 194 rows x 32
+// channels, the conv-2 operand, ring weight slots
+constexpr size_t tc_pair_smem(int TN, int nabuf, int ring) {
+  return 1024 + (size_t)nabuf * 2 * 4 * 194 * 16 + (size_t)2 * (TN / 8) * TCN_ROWS2 * 16 + (size_t)ring * 2 * 2 * TN * 16;
+}
+// two CTAs per SM: 228 KB of shared memory per SM, less 1 KB the hardware reserves per CTA
+constexpr size_t TCN_SMEM_OCC2 = (233472 - 2 * 1024) / 2;
+// weight slots of a pair config: today's ring at one CTA per SM (two operand buffers); at two, as many as fit
+constexpr int tc_pair_ring(int TN, int occ, int nabuf) {
+  return occ == 1 ? tc_ring_slots(TN, true) : (int)((TCN_SMEM_OCC2 - tc_pair_smem(TN, nabuf, 0)) / (2 * 2 * TN * 16));
+}
+
+// CTAs per SM and conv-1 operand buffers of a fused pair (tc_pair_fuses).  Two CTAs per SM let one tile's MMAs run while
+// the other CTA sits in an epilogue or at a named barrier; they halve the shared memory, so the ring and the operand
+// buffers shrink.  A pair whose weights are resident at one CTA per SM only runs two per SM where they stay resident
+// (a streamed slot costs L2 bandwidth on every tile).  Measured per (C, k) on an H100 (DESIGN.md, two pair CTAs per SM):
+//   C = 32, k = 3: two buffers, ring 22 (12 slots resident);  k = 7: one buffer, ring 34 (28 slots resident)
+//   C = 64, k = 7 / 11 (streamed either way): one buffer, ring 12
+//   C = 32, k = 11 and C = 64, k = 3 (resident only at one CTA per SM) and C = 128: one CTA per SM
+struct TcPairOcc {
+  int occ = 1, nabuf = 2;
+};
+inline TcPairOcc tc_pair_occ(const TcGeom& T1, const TcGeom& T2) {
+  TcPairOcc o;
+  if (!tc_pair_fuses(T1, T2)) return o;
+  const int n_w = 2 * (T1.Cin / 16) * T1.K;   // both convs' weight slots
+  if (T1.TN == 32 && n_w <= tc_pair_ring(32, 2, 2)) o = {2, 2};
+  else if (T1.TN == 32 && n_w <= tc_pair_ring(32, 2, 1)) o = {2, 1};
+  else if (T1.TN == 64 && n_w > tc_pair_ring(64, 1, 2)) o = {2, 1};
+  return o;
 }
 
 }  // namespace ovc

@@ -23,6 +23,7 @@ def main():
     ap.add_argument("--precision", default="fp32", choices=["fp32", "f16x3", "f16"])
     ap.add_argument("--pdl", type=int, default=None)
     ap.add_argument("--pair", type=int, default=None)
+    ap.add_argument("--pair-occ", type=int, default=None, help="0: every conv pair one CTA per SM; 1: tc_pair_occ")
     ap.add_argument("--reps", type=int, default=1, help="profiled calls (per-variant times are averaged)")
     args = ap.parse_args()
     import numpy as np
@@ -45,6 +46,8 @@ def main():
         nat.set_option("pdl", args.pdl)
     if args.pair is not None:
         nat.set_option("pair", args.pair)
+    if args.pair_occ is not None:
+        nat.set_option("pair_occ", args.pair_occ)
     nat.set_option("graph", 0)
     for _ in range(2):
         nat.convert_waveform(wav, wlen, g, g, tau=0.3, seed=1)
