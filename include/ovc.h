@@ -25,11 +25,11 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 9  /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 10 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
-                               * 8: ovc_spectrogram_ring; 9: OVC_OPT_PAIR_OCC */
+                               * 8: ovc_spectrogram_ring; 9: OVC_OPT_PAIR_OCC; 10: ovc_splice */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -162,6 +162,27 @@ OVC_API int ovc_voice_conversion_items(ovc_ctx* ctx, const float* spec, const in
  * for callers that must hand a kernel the noise a request would have drawn. */
 OVC_API int ovc_philox_normals(uint64_t seed, int64_t stream, int64_t c0, int C, int64_t frame0, int T, float* out,
                                void* cuda_stream);
+
+/* Copy many sample runs between device buffers in one launch: the join of the TTS decode's sentence rows, their
+ * silences and the converter's input rows (an utterance buffer, or the audio rings of live streams).  No context; the
+ * caller's current device; only enqueues on `stream` and takes stable pointers, so it can sit inside a captured graph.
+ *   src   [src_rows, src_pitch] fp32 (device); may be NULL with src_rows = 0 (every segment a gap)
+ *   dst   [dst_rows, dst_cap] fp32 (device)
+ *   seg   [S][5] int64 (device): rows (src_row, src_off, count, dst_row, dst_off).  Segment s writes, for i < count,
+ *           dst[dst_row * dst_cap + (dst_off + i) mod dst_cap] = src[src_row * src_pitch + src_off + i], or 0 when
+ *           src_row < 0 (a silence gap).
+ *         dst_cap is the ring wrap of a stream's audio ring; a buffer of whole utterances passes its row pitch and no
+ *         write wraps.  Descriptor values are clamped on the device, so nothing is read or written outside src and dst
+ *         whatever seg holds: dst_row into [0, dst_rows), dst_off mod dst_cap, count into [0, dst_cap], a source row
+ *         into [0, src_rows), src_off into [0, src_pitch] and count to the samples left in the source row.  Segments
+ *         whose destinations overlap leave an unspecified one of their values.
+ *   flags OVC_SPLICE_PCM16: every copied value x becomes q / 32768.0f, q = rint_even(fl32(x * 32767.0f)) saturated to
+ *         [-32768, 32767] (NaN: 0).  This is the project's specification of a float waveform written as a 16-bit PCM
+ *         wav and read back as float: libsndfile's default float -> PCM_16 write (scale by 32767, round to nearest)
+ *         and its PCM_16 -> float read (divide by 32768), which is what librosa.load returns for such a file. */
+#define OVC_SPLICE_PCM16 1
+OVC_API int ovc_splice(const float* src, int64_t src_rows, int64_t src_pitch, float* dst, int64_t dst_rows, int64_t dst_cap,
+                       const int64_t* seg, int S, int flags, void* stream);
 
 /* Front end of convert (row a2): linear magnitude spectrogram, replaces spectrogram_torch
  * (openvoice/mel_processing.py:40-75; call sites api.py:126-128,150-152) for n_fft = win = 1024,

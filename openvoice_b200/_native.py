@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -22,10 +22,11 @@ EXPORTS = (
     "ovc_tts_info", "ovc_tts_encode", "ovc_tts_decode", "ovc_set_option", "ovc_graph_replays",
     "ovc_reference_encoder_ragged", "ovc_resample", "ovc_resample_span", "ovc_voice_conversion_items",
     "ovc_convert_waveform_items", "ovc_tts_encode_items", "ovc_tts_decode_items", "ovc_philox_normals",
-    "ovc_tts_encode_state", "ovc_tts_decode_windows", "ovc_spectrogram_ring",
+    "ovc_tts_encode_state", "ovc_tts_decode_windows", "ovc_spectrogram_ring", "ovc_splice",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample / ovc_spectrogram_ring length of a stream that has not ended
+SPLICE_PCM16 = 1            # ovc_splice flag: the 16-bit PCM round trip of every copied value
 
 
 class OvcHParams(C.Structure):
@@ -151,6 +152,8 @@ def load_library(path: Optional[str] = None):
     lib.ovc_tts_encode_state.argtypes = [C.c_void_p] * 5
     lib.ovc_tts_decode_windows.argtypes = ([C.c_void_p] * 5 + [C.c_int, C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int]
                                            + [C.c_void_p] * 6)
+    lib.ovc_splice.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int,
+                               C.c_int, C.c_void_p]
     if lib.ovc_abi_version() != ABI_VERSION:
         raise OvcError(f"ABI mismatch: library {lib.ovc_abi_version()} vs binding {ABI_VERSION}")
     _lib = lib
@@ -449,6 +452,30 @@ class NativeConverter:
                                    int(out_pitch), int(out_start), C.c_void_p(st.cuda_stream))
         _check(self.lib, rc, "ovc_resample")
         return out
+
+    def splice(self, src, seg, dst, pcm16: bool = False, stream=None):
+        """Copy sample runs between device buffers in one launch (include/ovc.h: ovc_splice).  src [rows, pitch] f32
+        cuda, or None when every segment is a gap; seg [S, 5] int64 cuda, rows (src_row, src_off, count, dst_row,
+        dst_off); dst [rows, cap] f32 cuda, written in place: segment s puts src[src_row, src_off + i] (0 when src_row
+        < 0) at dst[dst_row, (dst_off + i) % cap], i < count.  ``pcm16``: every copied value takes the 16-bit PCM round
+        trip (``SPLICE_PCM16``).  Asynchronous on `stream`; returns ``dst``."""
+        import torch
+        assert dst.is_cuda and dst.dtype == torch.float32 and dst.is_contiguous() and dst.dim() == 2
+        assert seg.is_cuda and seg.dtype == torch.int64 and seg.is_contiguous()
+        if seg.dim() != 2 or seg.shape[1] != 5:
+            raise ValueError(f"splice: seg needs shape (S, 5), got {tuple(seg.shape)}")
+        if src is not None:
+            assert src.is_cuda and src.dtype == torch.float32 and src.is_contiguous() and src.dim() == 2
+            assert src.device == dst.device
+        rows, pitch = (0, 0) if src is None else (int(src.shape[0]), int(src.shape[1]))
+        st = stream if stream is not None else torch.cuda.current_stream(dst.device)
+        with torch.cuda.device(dst.device):
+            rc = self.lib.ovc_splice(None if src is None else C.c_void_p(src.data_ptr()), rows, pitch,
+                                     C.c_void_p(dst.data_ptr()), int(dst.shape[0]), int(dst.shape[1]),
+                                     C.c_void_p(seg.data_ptr()), int(seg.shape[0]), SPLICE_PCM16 if pcm16 else 0,
+                                     C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_splice")
+        return dst
 
     # ---- V1 TTS front half (SynthesizerTrn.infer, openvoice/models.py:467-490) ----------------
     def tts_info(self) -> dict:

@@ -4,7 +4,8 @@ Same classes, method names, arguments and return types as ``OpenVoiceBaseClass``
 ``ToneColorConverter`` (openvoice/api.py:14-39, :101-201); ``self.model`` is a
 ``NativeSynthesizer`` whose ``voice_conversion`` (the seam at openvoice/api.py:154) runs in
 libovc_b200.so.  Supersets of the reference: ``convert`` also accepts a NumPy waveform,
-``convert_batch`` converts a list of utterances in one launch sequence,
+``convert_batch`` converts a list of utterances in one launch sequence, ``clone_batch`` /
+``clone_stream_batch`` take text to cloned voice with the TTS audio joined on the device,
 ``enable_watermark=False`` works (it raises TypeError in the reference, SURVEY.md section 3.2).
 CUDA only: there is no CPU path.
 """
@@ -146,6 +147,33 @@ def plan_tts_windows(frames: int, first_window: int, window: int, halo: int) -> 
         out.append((max(0, e0 - halo), min(frames, e1 + halo), e0, e1))
         e0 = e1
     return out
+
+
+def plan_clone(frames: Sequence[int], owner: Sequence[int], speeds: Sequence[float], hop: int,
+               sr: int) -> Tuple[List[List[Tuple[int, int, int]]], List[int]]:
+    """Layout of each request's utterance as ``BaseSpeakerTTS.tts_batch`` joins it (``audio_numpy_concat``): sentence
+    i (a row of the TTS decode, owned by request ``owner[i]``) contributes its ``hop * frames[i]`` samples, then
+    ``int(sr * 0.05 / speed)`` zeros.  Returns per request the runs (src_row, src_off, count) in order (src_row -1: zeros)
+    and its length in samples."""
+    runs: List[List[Tuple[int, int, int]]] = [[] for _ in speeds]
+    for i, r in enumerate(owner):
+        runs[r] += [(i, 0, int(hop) * int(frames[i])), (-1, 0, int((sr * 0.05) / speeds[r]))]
+    return runs, [sum(n for _, _, n in rr) for rr in runs]
+
+
+def splice_table(runs: Sequence[Sequence[Tuple[int, int, int]]], pitch: int) -> np.ndarray:
+    """``ovc_splice`` segments [S, 5] that write item b's runs back to back into row b of a [len(runs), pitch] buffer,
+    and zeros from its end to the row's end."""
+    segs = []
+    for b, rr in enumerate(runs):
+        at = 0
+        for row, off, n in rr:
+            if n:
+                segs.append((row, off, n, b, at))
+                at += n
+        if at < pitch:
+            segs.append((-1, 0, pitch - at, b, at))
+    return np.asarray(segs, dtype=np.int64).reshape(-1, 5)
 
 
 class TtsState(NamedTuple):
@@ -344,6 +372,22 @@ class NativeSynthesizer:
         attn = (path.to(torch.float32) * y_mask.transpose(1, 2)).unsqueeze(1)      # [B,1,Ty,T]
         z, z_p = lat if lat else (None, None)
         return o, attn, y_mask, (z, z_p, None, None)
+
+    @torch.no_grad()
+    def infer_ragged(self, x, x_lengths, sid=None, noise_scale=1, length_scale=1, noise_scale_w=1.0, sdp_ratio=0.2,
+                     seed: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
+                     streams: Optional[Sequence[int]] = None) -> Tuple[torch.Tensor, List[int]]:
+        """The audio of ``infer(..., ragged=True, latents=False)`` (same arguments and draws) left on the device, with
+        each row's decoded frames on the host: (o [B, hop * max(frames)], frames).  Row b's samples are
+        o[b, : hop * frames[b]], zeros after.  One host sync (y_lengths), as in ``infer``."""
+        a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams)
+        y_lengths, _, _ = self.native.tts_encode(a["x"], a["x_lengths"], a["sid"], seed=a["seed"], items=a["enc_items"],
+                                                 **a["enc_scalars"])
+        frames = [int(v) for v in y_lengths.cpu()]             # the sync
+        o, _ = self.native.tts_decode(a["B"], max(frames), self.device, seed=a["seed"] + 1,
+                                      noise_scale=float(a["noise_scale"]), ragged=True, latents=False,
+                                      items=a["dec_items"])
+        return o[:, 0], frames
 
     def _tts_args(self, x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams):
         """The checks and device inputs ``infer`` and ``tts_encode`` share: validated tokens, lengths and speakers on the
@@ -628,14 +672,11 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
 
     def _infer_sentences(self, sequences, sid, **kw) -> List[np.ndarray]:
         """One ragged infer over token-id lists with per-sentence speaker ids; each sentence's samples."""
-        n = len(sequences)
         x, lens = self._pad_ids(sequences)
-        o, _, y_mask, _ = self.model.infer(x, lens, sid=torch.as_tensor(sid, dtype=torch.int64), ragged=True,
-                                           latents=False, **kw)
-        frames = y_mask[:, 0].sum(1).long().cpu()
-        o = o[:, 0].float().cpu().numpy()
+        o, frames = self.model.infer_ragged(x, lens, sid=torch.as_tensor(sid, dtype=torch.int64), **kw)
+        o = o.cpu().numpy()
         hop = self.hps.data.hop_length
-        return [o[i, : int(frames[i]) * hop].copy() for i in range(n)]
+        return [o[i, : frames[i] * hop].copy() for i in range(len(sequences))]
 
     @torch.no_grad()
     def tts_from_ids(self, sequences, speaker, speed=1.0, noise_scale=0.667, noise_scale_w=0.6, sdp_ratio=0.2,
@@ -827,6 +868,167 @@ class ToneColorConverter(OpenVoiceBaseClass):
                 out[i] = self.add_watermark(a, msg)
         return out  # type: ignore[return-value]
 
+    # ------------------------------------------------------------------ text to cloned voice
+    def _clone_requests(self, tts, requests):
+        """Validated ``clone_batch`` / ``clone_stream_batch`` requests, before anything is launched: the TTS sentences
+        (``BaseSpeakerTTS._request_sentences``) and per request its embeddings (stacked [n, gin]), tau, conversion key
+        and watermark message; the embeddings stay on the host.  ValueError for a request without sentences, a missing or mis-sized embedding, a tau
+        that is not finite, a bad seed, or models on different devices."""
+        reqs = list(requests)
+        if torch.device(tts.model.device) != torch.device(self.model.device):
+            raise ValueError(f"the TTS model is on {tts.model.device} and the converter on {self.model.device}")
+        seqs, sid, owner, speeds, kw = tts._request_sentences(reqs)
+        gin = int(getattr(self.hps.model, "gin_channels", 256))
+        ses = {"src_se": [], "tgt_se": []}
+        taus, seeds, messages = [], [], []
+        for r, q in enumerate(reqs):
+            if r not in owner:
+                raise ValueError(f"request {r} has no sentences")
+            for name in ses:
+                if q.get(name) is None:
+                    raise ValueError(f"request {r} has no {name}")
+                se = torch.as_tensor(q[name], dtype=torch.float32).reshape(1, -1)
+                if se.shape[1] != gin:
+                    raise ValueError(f"request {r}: {name} has {se.shape[1]} values, the converter's embeddings have {gin}")
+                ses[name].append(se)
+            tau = float(q.get("tau", 0.3))
+            if not math.isfinite(tau):
+                raise ValueError(f"request {r}: tau = {tau!r} is not a finite number")
+            taus.append(tau)
+            seed = q.get("convert_seed")
+            seeds.append(int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None
+                         else check_seeds([seed], 1, f"request {r}: convert_seed")[0])
+            messages.append(q.get("message", "default"))
+        stack = {k: torch.cat(v, 0) if v else None for k, v in ses.items()}
+        return (seqs, sid, owner, speeds, kw), stack["src_se"], stack["tgt_se"], taus, seeds, messages
+
+    def _check_clone_lengths(self, lengths, rate):
+        """ValueError for an utterance ``convert`` would refuse: shorter than one hop or not past the STFT padding
+        (after resampling from ``rate`` when it is given)."""
+        hop = self.hps.data.hop_length
+        pad = (self.hps.data.filter_length - hop) // 2
+        for r, n in enumerate(lengths):
+            m = self._resampled_len(n, rate)
+            if m < hop or m <= pad:
+                raise ValueError(f"request {r}: its utterance has {m} samples{'' if rate is None else ' after resampling'}: "
+                                 f"needs at least one hop ({hop}) and more than the STFT reflect padding ({pad})")
+
+    @torch.no_grad()
+    def clone_batch(self, tts: "BaseSpeakerTTS", requests: Sequence[dict], pcm16: bool = False,
+                    max_batch: int = 64) -> List[np.ndarray]:
+        """Text to cloned voice for many requests, joined on the device: what ``tts.tts(...)`` followed by
+        ``convert(...)`` gives, without the audio leaving the GPU in between.  A request is a ``tts.tts_batch`` request
+        dict plus ``src_se`` and ``tgt_se`` (required; [1, gin, 1] embeddings), ``tau`` (0.3), ``convert_seed`` (the
+        conversion's key; default: drawn from torch's generator, as ``seed`` is) and ``message`` (watermark payload,
+        applied on the host as ``convert_batch`` applies it).
+
+        One ragged TTS encode + decode of every sentence (one host sync, for the frame counts), then per chunk of
+        ``max_batch`` requests (sorted by length, as ``convert_batch`` chunks) one ``ovc_splice`` that builds the
+        utterances in the converter's input rows -- each sentence followed by int(sr * 0.05 / speed) zeros, as
+        ``audio_numpy_concat`` joins them -- one ragged conversion with each request's embeddings, tau and key, and one
+        download.  If the TTS model's rate is not the converter's, the joined rows are resampled on the device.
+
+        Request r's array equals ``convert(tts.tts_batch([q])[0], q["src_se"], q["tgt_se"], tau=q["tau"],
+        seed=q["convert_seed"], sr=tts_rate)`` bit for bit, whatever else is in the batch.  ``pcm16``: each TTS sample
+        first takes the 16-bit PCM round trip of a wav file (include/ovc.h: OVC_SPLICE_PCM16), as when the TTS output is
+        written to a 16-bit wav and converted from that file.  Malformed requests raise ValueError before any launch;
+        an utterance too short to convert (a very high speed) raises it after the encode, before the conversion."""
+        reqs = list(requests)
+        (seqs, sid, owner, speeds, kw), src, tgt, taus, seeds, messages = self._clone_requests(tts, reqs)
+        if not reqs:
+            return []
+        rate = self._input_rate([], int(tts.hps.data.sampling_rate))
+        x, lens = tts._pad_ids(seqs)
+        o, frames = tts.model.infer_ragged(x, lens, sid=torch.as_tensor(sid, dtype=torch.int64), **kw)
+        runs, lengths = plan_clone(frames, owner, speeds, tts.hps.data.hop_length, int(tts.hps.data.sampling_rate))
+        self._check_clone_lengths(lengths, rate)
+        src, tgt = src.to(self.device), tgt.to(self.device)
+        out: List[Optional[np.ndarray]] = [None] * len(reqs)
+        order = sorted(range(len(reqs)), key=lambda i: -lengths[i])
+        for lo in range(0, len(reqs), max_batch):
+            idx = order[lo: lo + max_batch]
+
+            def fill(rows, idx=idx):
+                table = splice_table([runs[i] for i in idx], rows.shape[1])
+                pin = self._pinned_i64("splice", table.size)
+                pin.copy_(torch.from_numpy(table.reshape(-1)))
+                seg = self._dev("splice", table.size, torch.int64)
+                seg.copy_(pin, non_blocking=True)
+                self.model.native.splice(o, seg.view(-1, 5), rows, pcm16=pcm16)
+            res = self._convert_chunk([lengths[i] for i in idx], src[idx], tgt[idx], [taus[i] for i in idx], None,
+                                      sr=rate, seeds=[seeds[i] for i in idx], fill=fill)
+            for i, a in zip(idx, res):
+                out[i] = self.add_watermark(a, messages[i])
+        return out  # type: ignore[return-value]
+
+    def clone_stream_batch(self, tts: "BaseSpeakerTTS", requests: Sequence[dict], window_frames: int = 256,
+                           first_window_frames: int = 32) -> Iterator[Tuple[int, np.ndarray]]:
+        """Streaming ``clone_batch`` (``pcm16=False``): yields ``(request_index, chunk)`` of cloned audio while the
+        requests are still being synthesised.  Requests as in ``clone_batch``; the TTS encode of all their sentences
+        runs here, so malformed requests and too-short utterances raise ValueError before the first step.
+
+        Each request is a ``streaming.StreamingSessions`` session (``window_frames``-frame converter windows, the
+        request's embeddings, tau and ``convert_seed``).  A step is one batched launch sequence over every unfinished
+        request: ONE ``tts_decode_windows`` call decodes, per request, the next TTS windows (``plan_tts_windows``:
+        ``first_window_frames`` then ``window_frames`` frames) until its converter can emit a window or its text is
+        done; ONE ``ovc_splice`` writes the windows' interiors and the sentences' 50 ms / speed gaps into the sessions'
+        rings; then one ring spectrogram and ragged conversion of every ready window, and one download.  A request is
+        closed in the step that writes its last gap.  Every step yields one non-empty chunk per unfinished request, in
+        request order; a request's chunks concatenate to its ``clone_batch`` array (same length; the TTS windows equal
+        the whole decode to fp32 reordering).  The models must share a sampling rate (ValueError otherwise)."""
+        window_frames, first_window_frames = int(window_frames), int(first_window_frames)
+        if window_frames < 1 or first_window_frames < 1:
+            raise ValueError(f"window_frames ({window_frames}) and first_window_frames ({first_window_frames}) must be >= 1")
+        sr = int(self.hps.data.sampling_rate)
+        if int(tts.hps.data.sampling_rate) != sr:
+            raise ValueError(f"the TTS model runs at {tts.hps.data.sampling_rate} Hz and the converter at {sr} Hz: "
+                             f"clone_stream_batch needs one rate (clone_batch resamples)")
+        reqs = list(requests)
+        (seqs, sid, owner, speeds, kw), src, tgt, taus, seeds, _ = self._clone_requests(tts, reqs)
+        if not reqs:
+            return iter(())
+        x, lens = tts._pad_ids(seqs)
+        state = tts.model.tts_encode(x, lens, sid=torch.as_tensor(sid, dtype=torch.int64), **kw)
+        self._check_clone_lengths(plan_clone(state.frames, owner, speeds, tts.hps.data.hop_length, sr)[1], None)
+        # per request: its TTS windows in order, (state row, lo, hi, e0, e1, zeros after the window)
+        plans: List[List[Tuple[int, int, int, int, int, int]]] = [[] for _ in reqs]
+        for i, r in enumerate(owner):
+            wins = plan_tts_windows(state.frames[i], first_window_frames if not plans[r] else window_frames,
+                                    window_frames, TTS_HALO_FRAMES)
+            gap = int((sr * 0.05) / speeds[r])
+            plans[r] += [(i, lo, hi, e0, e1, gap if k == len(wins) - 1 else 0) for k, (lo, hi, e0, e1) in enumerate(wins)]
+        return self._clone_stream(tts, state, plans, src, tgt, taus, seeds, window_frames)
+
+    @torch.no_grad()
+    def _clone_stream(self, tts, state, plans, src, tgt, taus, seeds, window_frames):
+        from .streaming import StreamingSessions, ready_frames
+        hop, nfft = self.hps.data.hop_length, self.hps.data.filter_length
+        ss = StreamingSessions(self, window_frames=window_frames)
+        ids = [ss.open(src[r], tgt[r], tau=taus[r], seed=seeds[r]) for r in range(len(plans))]
+        done = [0] * len(plans)                          # TTS windows of each request already pushed
+        live = list(range(len(plans)))
+        while live:
+            wins, runs, closing = [], {}, []
+            for r in live:
+                s = ss.sessions[ids[r]]
+                n_in, runs[ids[r]] = s.n_in, []
+                while done[r] < len(plans[r]):
+                    i, lo, hi, e0, e1, gap = plans[r][done[r]]
+                    runs[ids[r]] += [(len(wins), (e0 - lo) * hop, (e1 - e0) * hop)] + ([(-1, 0, gap)] if gap else [])
+                    wins.append((i, lo, hi - lo))
+                    n_in += (e1 - e0) * hop + gap
+                    done[r] += 1
+                    if ready_frames(n_in, hop, nfft, False) >= s.emitted + ss.W + ss.H:
+                        break
+                if done[r] == len(plans[r]):
+                    closing.append(ids[r])
+            o, _ = tts.model.tts_decode_windows(state, wins)
+            out = ss.push_device(runs, o, close=closing)
+            for r in live:
+                if len(out[ids[r]]):
+                    yield r, out[ids[r]]
+            live = [r for r in live if ids[r] not in closing]
+
     # ------------------------------------------------------------------ one utterance per stream
     @torch.no_grad()
     def convert_concurrent(self, audios: Sequence[AudioLike], src_se, tgt_se, tau: Union[float, Sequence[float]] = 0.3,
@@ -989,15 +1191,18 @@ class ToneColorConverter(OpenVoiceBaseClass):
         assert se.shape[0] == n, "one speaker embedding per utterance (or a single one for all)"
         return se
 
-    def _enqueue_chunk(self, waves, src, tgt, tau, noise, slot=0, sr=None, seeds=None):
+    def _enqueue_chunk(self, waves, src, tgt, tau, noise, slot=0, sr=None, seeds=None, fill=None):
         """Stage, upload and launch one ragged batch on the current stream WITHOUT synchronising the host.
         Returns (o [B, 256 * Tmax] on the device, frames per item).  ``sr``: the waves' rate when it is not the
         model's (``_input_rate``): the raw samples are uploaded and resampled on the device into the slot's buffer.
-        ``tau``: a float or one per item; ``seeds``: None or one key per item (validated by the caller)."""
+        ``tau``: a float or one per item; ``seeds``: None or one key per item (validated by the caller).
+        ``fill``: the items are already on the device.  ``waves`` then holds each item's sample count, and
+        ``fill(rows)`` enqueues the writes of the items' samples, zero padded, into the [B, pitch] device rows the
+        upload would have filled."""
         hps = self.hps
         hop = hps.data.hop_length
         B = len(waves)
-        lens_in = [len(w) for w in waves]
+        lens_in = [len(w) for w in waves] if fill is None else [int(n) for n in waves]
         lens = [self._resampled_len(n, sr) for n in lens_in]
         after = "" if sr is None else " after resampling"
         frames = [n // hop for n in lens]
@@ -1016,24 +1221,25 @@ class ToneColorConverter(OpenVoiceBaseClass):
         ev = self.__dict__.setdefault("_h2d_done", {}).get(slot)
         if ev is not None:
             ev.synchronize()
-        stage = self._pinned(f"in{slot}", B * Lin).view(B, Lin)
-        stage_np = stage.numpy()
+        if fill is None:
+            stage = self._pinned(f"in{slot}", B * Lin).view(B, Lin)
+            stage_np = stage.numpy()
 
-        def put(b):
-            w = waves[b]
-            stage_np[b, : len(w)] = w
-            if len(w) < Lin:
-                stage_np[b, len(w):] = 0.0
-        _parallel(put, B)
+            def put(b):
+                w = waves[b]
+                stage_np[b, : len(w)] = w
+                if len(w) < Lin:
+                    stage_np[b, len(w):] = 0.0
+            _parallel(put, B)
         # device-side buffers are cached per slot too: with every address stable, a repeated (batch, length) call is
         # replayed from a CUDA graph by the native library (include/ovc.h: OVC_OPT_GRAPH); the resampler writes into
         # the same per-slot buffer the spectrogram reads
         wav = self._dev(f"wav{slot}", B * Lmax, torch.float32).view(B, Lmax)
         if sr is None:
-            wav.copy_(stage, non_blocking=True)
+            wav.copy_(stage, non_blocking=True) if fill is None else fill(wav)
         else:
             raw = self._dev(f"raw{slot}", B * Lin, torch.float32).view(B, Lin)
-            raw.copy_(stage, non_blocking=True)
+            raw.copy_(stage, non_blocking=True) if fill is None else fill(raw)
             rlen_pin = self._pinned_i64(f"rlen{slot}", B)
             rlen_pin.copy_(torch.tensor(lens_in, dtype=torch.int64))
             rlen = self._dev(f"rlen{slot}", B, torch.int64)
@@ -1088,9 +1294,9 @@ class ToneColorConverter(OpenVoiceBaseClass):
             items["tau"] = d
         return items
 
-    def _convert_chunk(self, waves, src, tgt, tau, noise, sr=None, seeds=None):
+    def _convert_chunk(self, waves, src, tgt, tau, noise, sr=None, seeds=None, fill=None):
         hop = self.hps.data.hop_length
-        o, frames = self._enqueue_chunk(waves, src, tgt, tau, noise, sr=sr, seeds=seeds)
+        o, frames = self._enqueue_chunk(waves, src, tgt, tau, noise, sr=sr, seeds=seeds, fill=fill)
         host = self._pinned("out", o.numel()).view(o.shape)
         host.copy_(o, non_blocking=True)
         torch.cuda.current_stream(self.device).synchronize()

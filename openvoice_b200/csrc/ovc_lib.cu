@@ -20,6 +20,7 @@
 #include "ovc_tts.cuh"
 #include "ovc_refenc.cuh"
 #include "ovc_resample.cuh"
+#include "ovc_splice.h"
 #include "ovc_variants.h"
 
 namespace ovc {
@@ -1829,6 +1830,25 @@ int ovc_philox_normals(uint64_t seed, int64_t stream, int64_t c0, int C, int64_t
   if (!out || C < 1 || T < 1 || C > 65535) return fail(OVC_ERR_INVALID, "bad argument to ovc_philox_normals (C=%d, T=%d)", C, T);
   philox_normals_kernel<<<dim3((T + 127) / 128, C), 128, 0, (cudaStream_t)cuda_stream>>>(
       seed, (uint32_t)stream, (uint32_t)c0, (uint32_t)frame0, T, out);
+  CK(cudaGetLastError());
+  return OVC_OK;
+}
+
+static_assert(OVC_SPLICE_PCM16 == ovc_sp::PCM16, "ovc_splice flag");
+
+int ovc_splice(const float* src, int64_t src_rows, int64_t src_pitch, float* dst, int64_t dst_rows, int64_t dst_cap,
+               const int64_t* seg, int S, int flags, void* stream) {
+  if (S < 0 || (S > 0 && !seg)) return fail(OVC_ERR_INVALID, "ovc_splice: bad segment table (S=%d)", S);
+  if (!dst || dst_rows < 1 || dst_cap < 1)
+    return fail(OVC_ERR_INVALID, "ovc_splice: bad destination (rows %lld, cap %lld)", (long long)dst_rows, (long long)dst_cap);
+  if (src_rows < 0 || (src_rows > 0 && (!src || src_pitch < 1)))
+    return fail(OVC_ERR_INVALID, "ovc_splice: bad source (rows %lld, pitch %lld)", (long long)src_rows, (long long)src_pitch);
+  if (flags & ~OVC_SPLICE_PCM16) return fail(OVC_ERR_INVALID, "ovc_splice: unknown flags %d", flags);
+  if (S == 0) return OVC_OK;
+  const int gy = S < 65535 ? S : 65535;
+  const int gx = std::max(1, std::min(1024, 2048 / gy));
+  ovc_sp::splice_kernel<<<dim3(gx, gy), 256, 0, (cudaStream_t)stream>>>(src, src_rows, src_pitch, seg, S, dst, dst_rows,
+                                                                         dst_cap, flags);
   CK(cudaGetLastError());
   return OVC_OK;
 }

@@ -33,7 +33,7 @@ window's spectrogram in one launch, and one ragged voice conversion converts the
 ``stream_windows`` are the readiness and window rules both classes follow.
 """
 import math
-from typing import Callable, Dict, Iterable, List, Optional, Tuple
+from typing import Callable, Dict, Iterable, List, Optional, Sequence, Set, Tuple
 
 import numpy as np
 import torch
@@ -308,8 +308,8 @@ class StreamingSessions:
     frames are those of the whole clip, and each window draws its noise at its own seed and absolute frames.
 
     Every ``push`` / ``close`` is one step: one packed upload (the pushed samples and every per-window value), one
-    scatter of the samples into the sessions' device audio rings, one ``ovc_spectrogram_ring`` over every ready window of
-    every session in the call, one gather of their embeddings from a device table, ragged voice conversions of up to
+    ``ovc_splice`` of the samples into the sessions' device audio rings, one ``ovc_spectrogram_ring`` over every ready
+    window of every session in the call, one gather of their embeddings from a device table, ragged voice conversions of up to
     ``SESSION_BATCH_FRAMES`` padded frames each (one for a typical step), one gather of the emitted frames, one download
     and one synchronisation.  Buffers are grow-only and the padded window length is rounded up to 16 frames, so a steady
     lockstep step replays its CUDA graph.  A session keeps the audio of its next window and both halos, plus the STFT
@@ -406,7 +406,35 @@ class StreamingSessions:
         the converted samples that became final (possibly none)."""
         ids = self._check_ids(chunks.keys())
         xs = {sid: np.asarray(chunks[sid], dtype=np.float32).reshape(-1) for sid in ids}
-        return self._step(xs, final=False)
+        return self._step(xs, final=set())
+
+    @torch.no_grad()
+    def push_device(self, runs: Dict[int, Sequence[Tuple[int, int, int]]], src: torch.Tensor,
+                    close: Iterable[int] = ()) -> Dict[int, np.ndarray]:
+        """``push`` of audio already on the device: appends to each named session, in order, the runs
+        ``(src_row, src_off, count)`` of ``src`` ([rows, pitch] float32 on the converter's device): samples
+        src[src_row, src_off : src_off + count], or ``count`` zeros when src_row < 0.  The runs of every session go into
+        the rings in ONE ``ovc_splice``; nothing is uploaded but the step's small tables.  The sessions named in
+        ``close`` (each also in ``runs``) then end as ``close`` ends them, in the same step.  Returns what ``push`` and
+        ``close`` return.  A run outside ``src`` or a session too short to end raises ValueError before any launch."""
+        ids = self._check_ids(runs.keys())
+        close = set(close)
+        if not close <= set(ids):
+            raise ValueError("close names a session that has no runs in this call")
+        assert src.is_cuda and src.dtype == torch.float32 and src.is_contiguous() and src.dim() == 2
+        rows, pitch = src.shape
+        xs = {}
+        for sid in ids:
+            xs[sid] = [tuple(int(v) for v in r) for r in runs[sid]]
+            for r, o, n in xs[sid]:
+                if n < 0 or (r >= 0 and (r >= rows or o < 0 or o + n > pitch)):
+                    raise ValueError(f"session {sid}: run {(r, o, n)} is not inside src {tuple(src.shape)}")
+        for sid in close:
+            check_stream_length(self.sessions[sid].n_in + sum(n for _, _, n in xs[sid]), self.hop, self.pad)
+        out = self._step(xs, final=close, src=src)
+        for sid in close:
+            self.free_rows.append(self.sessions.pop(sid).row)
+        return out
 
     @torch.no_grad()
     def close(self, ids: Iterable[int]) -> Dict[int, np.ndarray]:
@@ -416,7 +444,7 @@ class StreamingSessions:
         ids = self._check_ids(ids)
         for sid in ids:
             check_stream_length(self.sessions[sid].n_in, self.hop, self.pad)
-        out = self._step({sid: np.zeros(0, dtype=np.float32) for sid in ids}, final=True)
+        out = self._step({sid: np.zeros(0, dtype=np.float32) for sid in ids}, final=set(ids))
         for sid in ids:
             self.free_rows.append(self.sessions.pop(sid).row)
         return out
@@ -446,26 +474,42 @@ class StreamingSessions:
         self.rings, self.se, self.rows, self.cap = rings, se, rows, cap
 
     # ------------------------------------------------------------------ one step
-    def _step(self, xs: Dict[int, np.ndarray], final: bool) -> Dict[int, np.ndarray]:
+    def _step(self, xs: Dict[int, object], final: Set[int], src: Optional[torch.Tensor] = None) -> Dict[int, np.ndarray]:
+        """One step over the sessions of ``xs``: xs[sid] is the session's new host samples, or with ``src`` its runs
+        (src_row, src_off, count) of that device array; the sessions in ``final`` end after them."""
         hop, H = self.hop, self.H
         ses = [(sid, self.sessions[sid], xs[sid]) for sid in xs]
-        need = max([s.n_in + len(x) - self._keep_from(s) for _, s, x in ses], default=0)
+        if src is None:                                   # host samples: the upload's sample block is the one source row
+            counts = [len(x) for _, _, x in ses]
+            starts = np.cumsum([0] + counts)
+            runs = [[(0, int(a), n)] for a, n in zip(starts, counts)]
+        else:
+            runs = [x for _, _, x in ses]
+            counts = [sum(n for _, _, n in r) for r in runs]
+        need = max([s.n_in + n - self._keep_from(s) for (_, s, _), n in zip(ses, counts)], default=0)
         if need > self.cap:
             cap = -(-int(need * 1.25) // hop) * hop
             self._grow(self.rows, cap, [(s.row, self._keep_from(s), s.n_in) for s in self.sessions.values()])
         # windows of every named session: (session index, lo, hi, e0, e1)
         wins = []
-        for i, (_, s, x) in enumerate(ses):
-            n = s.n_in + len(x)
-            have = ready_frames(n, hop, self.nfft, final)
-            wins += [(i,) + w for w in stream_windows(s.emitted, have, self.W, H, final)]
-        B, Ns = len(wins), sum(len(x) for _, _, x in ses)
+        for i, ((sid, s, _), n) in enumerate(zip(ses, counts)):
+            have = ready_frames(s.n_in + n, hop, self.nfft, sid in final)
+            wins += [(i,) + w for w in stream_windows(s.emitted, have, self.W, H, sid in final)]
+        # splice segments: each run to the ring row of its session, at the session's next sample positions
+        segs = []
+        for (_, s, _), r in zip(ses, runs):
+            at = s.n_in
+            for row, off, n in r:
+                if n:
+                    segs.append((row, off, n, s.row, at))
+                    at += n
+        B, nS, Ns = len(wins), len(segs), (sum(counts) if src is None else 0)
         Tmax = -(-max([hi - lo for _, lo, hi, _, _ in wins], default=1) // 16) * 16
         Nf = sum(e1 - e0 for _, _, _, e0, e1 in wins)
         # packed upload (int64 words): row, lo, frames, stream length, seed, stream (0), embedding rows (2B), tau (float32),
-        # then the emitted frames' rows of the output, the ring positions of the pushed samples and the samples (float32)
+        # then the emitted frames' rows of the output, the splice segments (5 words each) and the pushed samples (float32)
         nt = (B + 1) // 2
-        n_words = 8 * B + nt + Nf + Ns + (Ns + 1) // 2
+        n_words = 8 * B + nt + Nf + 5 * nS + (Ns + 1) // 2
         if self._h2d_done is not None:
             self._h2d_done.synchronize()                  # the previous step's upload has left the pinned buffer
         pin = self._buf("pin", n_words, torch.int64, pinned=True)
@@ -475,7 +519,7 @@ class StreamingSessions:
             rows = np.asarray([s.row for _, s, _ in ses], dtype=np.int64)[ii]
             lo = np.asarray([v[1] for v in wins], dtype=np.int64)
             w[0:B], w[B:2 * B], w[2 * B:3 * B] = rows, lo, [hi - l for _, l, hi, _, _ in wins]
-            w[3 * B:4 * B] = [ses[i][1].n_in + len(ses[i][2]) if final else STREAM_OPEN for i in ii]
+            w[3 * B:4 * B] = [ses[i][1].n_in + counts[i] if ses[i][0] in final else STREAM_OPEN for i in ii]
             from .api import seed_array
             w[4 * B:5 * B] = seed_array([ses[i][1].seed for i in ii])
             w[5 * B:6 * B] = 0
@@ -484,17 +528,23 @@ class StreamingSessions:
             o = 8 * B + nt
             w[o:o + Nf] = np.concatenate([b * Tmax + np.arange(e0 - l, e1 - l) for b, (_, l, _, e0, e1) in enumerate(wins)])
         o = 8 * B + nt + Nf
+        if nS:
+            w[o:o + 5 * nS] = np.asarray(segs, dtype=np.int64).reshape(-1)
         if Ns:
-            w[o:o + Ns] = np.concatenate([s.row * self.cap + np.arange(s.n_in, s.n_in + len(x)) % self.cap
-                                          for _, s, x in ses if len(x)])
-            w[o + Ns:].view(np.float32)[:Ns] = np.concatenate([x for _, _, x in ses])
+            w[o + 5 * nS:].view(np.float32)[:Ns] = np.concatenate([x for _, _, x in ses])
         d = self._buf("up", n_words, torch.int64)
         d.copy_(pin, non_blocking=True)
         if self.cuda:
             self._h2d_done = torch.cuda.Event()
             self._h2d_done.record(torch.cuda.current_stream(self.dev))
-        if Ns:
-            self.rings.view(-1).index_copy_(0, d[o:o + Ns], d[o + Ns:].view(torch.float32)[:Ns])
+        if nS:
+            source = d[o + 5 * nS:].view(torch.float32)[:Ns].view(1, Ns) if src is None else src
+            if self.cuda:
+                self.native.splice(source, d[o:o + 5 * nS].view(nS, 5), self.rings)
+            else:   # only the CPU stand-in converters of the host tests get here: the same writes as one index_copy_
+                at = np.concatenate([r * self.cap + np.arange(a, a + n) % self.cap for _, _, n, r, a in segs])
+                val = torch.cat([source[row, off:off + n] if row >= 0 else torch.zeros(n) for row, off, n, _, _ in segs])
+                self.rings.view(-1).index_copy_(0, torch.from_numpy(at), val)
         res = {sid: np.zeros(0, dtype=np.float32) for sid, _, _ in ses}
         if B:
             spec = self._buf("spec", B * self.S * Tmax, torch.float32).view(B, self.S, Tmax)
@@ -525,7 +575,7 @@ class StreamingSessions:
                 at += e1 - e0
             for i, parts in per_ses.items():
                 res[ses[i][0]] = np.concatenate(parts)
-        for i, (_, s, x) in enumerate(ses):
-            s.n_in += len(x)
+        for i, (_, s, _) in enumerate(ses):
+            s.n_in += counts[i]
             s.emitted = max([e1 for j, _, _, _, e1 in wins if j == i], default=s.emitted)
         return res
