@@ -25,11 +25,12 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 10 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 11 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
-                               * 8: ovc_spectrogram_ring; 9: OVC_OPT_PAIR_OCC; 10: ovc_splice */
+                               * 8: ovc_spectrogram_ring; 9: OVC_OPT_PAIR_OCC; 10: ovc_splice;
+                               * 11: ovc_tts_encode_state_rows, ovc_tts_state_rows */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -328,6 +329,34 @@ OVC_API int ovc_tts_decode_items(ovc_ctx* ctx, const float* noise, uint64_t seed
  * that repeats its (W, Wmax, buffers, options) is replayed from a CUDA graph (OVC_OPT_GRAPH) and follows the arrays'
  * new contents.  Null buffers or non-positive sizes are OVC_ERR_INVALID. */
 OVC_API int ovc_tts_encode_state(ovc_ctx* ctx, float* stats, int32_t* cum, float* g, void* stream);
+
+/* Encode state written straight into rows of a pool: a grow-only set of N rows at token pitch Tp that holds the
+ * sentences of many encodes (live streams whose text arrives over time), decoded together by ovc_tts_decode_windows with
+ * (N, Tp) in place of (N, T).
+ *
+ * ovc_tts_encode_state_rows writes row b of the pending ovc_tts_encode (B rows of T tokens) into pool row dst_row[b]:
+ * stats [N][Tp][2 inter], cum [N][Tp] int32, g [N][gin] and y_lengths [N] int64 (the encode's y_length of the row).
+ * ovc_tts_state_rows does the same from caller-owned state (stats [B][T][2 inter], cum [B][T], g [B][gin],
+ * y_lengths [B]), e.g. to re-pitch a pool into a larger one with dst_row = 0 .. B - 1.
+ *
+ * Padding rule.  Tokens T <= t < Tp of a pool row are filled as an encode fills the tokens of a short row inside its
+ * batch: cum[t] = cum[T - 1] (the durations past a row's x_length are 0, so the cumulative sum stays put), and stats[t]
+ * = 0 (an encode does not write a row's stats past its x_length; what lies there is never read for a row with frames).
+ * ovc_tts_decode_windows finds frame f's token as the first t with cum[t] > f, so for every f < y_length the token, and
+ * the samples, are those of the encode's own state bit for bit.  (A row whose durations all round to 0 has y_length 1
+ * and expands its one frame from the last token of the pitch, padding included: with a larger pitch that token moves.)
+ * Tokens t < T are copied as they are, including whatever the encode left past x_length.
+ *
+ *   dst_row  [B] int64 (device); clamped into [0, N) on the device, so nothing is written outside the pool whatever it
+ *            holds.  Rows named twice get an unspecified one of their sources.
+ * Tp < T, N < 1 or a null pointer is OVC_ERR_INVALID.  One grid-strided kernel; only enqueues on `stream` and takes
+ * stable pointers, so it can sit inside a captured graph. */
+OVC_API int ovc_tts_encode_state_rows(ovc_ctx* ctx, const int64_t* dst_row, int N, int Tp, float* stats, int32_t* cum,
+                                      float* g, int64_t* y_lengths, void* stream);
+OVC_API int ovc_tts_state_rows(ovc_ctx* ctx, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths,
+                               int B, int T, const int64_t* dst_row, int N, int Tp, float* d_stats, int32_t* d_cum,
+                               float* d_g, int64_t* d_y_lengths, void* stream);
+
 OVC_API int ovc_tts_decode_windows(ovc_ctx* ctx, const float* stats, const int32_t* cum, const float* g,
                                    const int64_t* y_lengths, int N, int T, const int64_t* row, const int64_t* frame0,
                                    const int64_t* len, int W, int Wmax, const uint64_t* seed, const int64_t* stream,

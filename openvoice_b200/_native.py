@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -23,6 +23,7 @@ EXPORTS = (
     "ovc_reference_encoder_ragged", "ovc_resample", "ovc_resample_span", "ovc_voice_conversion_items",
     "ovc_convert_waveform_items", "ovc_tts_encode_items", "ovc_tts_decode_items", "ovc_philox_normals",
     "ovc_tts_encode_state", "ovc_tts_decode_windows", "ovc_spectrogram_ring", "ovc_splice",
+    "ovc_tts_encode_state_rows", "ovc_tts_state_rows",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample / ovc_spectrogram_ring length of a stream that has not ended
@@ -154,6 +155,9 @@ def load_library(path: Optional[str] = None):
                                            + [C.c_void_p] * 6)
     lib.ovc_splice.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int,
                                C.c_int, C.c_void_p]
+    lib.ovc_tts_encode_state_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 5
+    lib.ovc_tts_state_rows.argtypes = ([C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
+                                       + [C.c_void_p] * 5)
     if lib.ovc_abi_version() != ABI_VERSION:
         raise OvcError(f"ABI mismatch: library {lib.ovc_abi_version()} vs binding {ABI_VERSION}")
     _lib = lib
@@ -544,6 +548,51 @@ class NativeConverter:
                                            C.c_void_p(g.data_ptr()), C.c_void_p(st.cuda_stream))
         _check(self.lib, rc, "ovc_tts_encode_state")
         return stats, cum, g
+
+    def tts_state_rows(self, dst_row, stats, cum, g, y_lengths, src=None, stream=None):
+        """Write encoded rows into rows ``dst_row`` (host ints) of a state pool (include/ovc.h: ovc_tts_encode_state_rows,
+        ovc_tts_state_rows): stats [N,Tp,2*inter] f32, cum [N,Tp] int32, g [N,gin] f32, y_lengths [N] int64 on the device,
+        written in place.  ``src``: None for the rows of the last ``tts_encode``, or caller-owned state (stats, cum, g,
+        y_lengths) of B rows.  Tokens past the source's pitch get the library's padding.  Asynchronous on `stream`."""
+        import torch
+        N, Tp = cum.shape
+        dev = cum.device
+        for t, dt, shape in ((stats, torch.float32, (N, Tp, 2 * self.hp.inter_channels)), (cum, torch.int32, (N, Tp)),
+                             (g, torch.float32, (N, self.hp.gin_channels)), (y_lengths, torch.int64, (N,))):
+            assert t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, t.shape)
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        # the row table goes up through a pinned buffer, reused once its previous upload has left it: no host sync
+        dst_row = [int(r) for r in dst_row]
+        cache = self.__dict__.setdefault("_rows_bufs", {})
+        if cache.get("ev") is not None:
+            cache["ev"].synchronize()
+        n = max(1, len(dst_row))
+        if cache.get("pin") is None or cache["pin"].numel() < n or cache["dev"].device != dev:
+            cache["pin"] = torch.empty(int(n * 1.25) + 64, dtype=torch.int64).pin_memory()
+            cache["dev"] = torch.empty(cache["pin"].numel(), dtype=torch.int64, device=dev)
+        cache["pin"][:len(dst_row)].copy_(torch.tensor(dst_row, dtype=torch.int64))
+        rows = cache["dev"][:n]
+        with torch.cuda.stream(st):
+            rows.copy_(cache["pin"][:n], non_blocking=True)
+            cache["ev"] = torch.cuda.Event()
+            cache["ev"].record(st)
+        p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+        if src is None:
+            rc = self.lib.ovc_tts_encode_state_rows(self.handle, p(rows), N, Tp, p(stats), p(cum), p(g), p(y_lengths),
+                                                    C.c_void_p(st.cuda_stream))
+        else:
+            s_stats, s_cum, s_g, s_len = src
+            B, T = s_cum.shape
+            if len(dst_row) != B:
+                raise ValueError(f"tts_state_rows: {len(dst_row)} destination rows for {B} source rows")
+            for t, dt, shape in ((s_stats, torch.float32, (B, T, 2 * self.hp.inter_channels)),
+                                 (s_cum, torch.int32, (B, T)), (s_g, torch.float32, (B, self.hp.gin_channels)),
+                                 (s_len, torch.int64, (B,))):
+                assert t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, t.shape)
+            rc = self.lib.ovc_tts_state_rows(self.handle, p(s_stats), p(s_cum), p(s_g), p(s_len), B, T, p(rows), N, Tp,
+                                             p(stats), p(cum), p(g), p(y_lengths), C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_tts_state_rows")
+        return stats, cum, g, y_lengths
 
     def tts_decode_windows(self, stats, cum, g, y_lengths, row, frame0, length, seed, streams, noise_scale, w_max: int,
                            latents: bool = False, slot: int = 0, stream=None):

@@ -190,6 +190,34 @@ class TtsState(NamedTuple):
     dec_noise_scale: List[float]
 
 
+class TtsPool:
+    """Encode state shared by the sentences of many live requests: device tensors stats [N,Tp,2*inter], cum [N,Tp] int32,
+    g [N,gin] and y_lengths [N], grown on demand and never shrunk.  ``NativeSynthesizer.tts_encode(..., pool=, rows=)``
+    writes an encode's rows into any rows of it (include/ovc.h: ovc_tts_encode_state_rows); a larger token pitch
+    re-pitches the rows already there once, with the library's padding.  The owner tracks which rows are live."""
+
+    def __init__(self, native, device):
+        self.native, self.device = native, torch.device(device)
+        self.N = self.Tp = 0
+        self.stats = self.cum = self.g = self.y_lengths = None
+
+    def fit(self, N: int, T: int) -> None:
+        """At least ``N`` rows at a pitch of at least ``T`` tokens; the rows already held keep their contents."""
+        if N <= self.N and T <= self.Tp:
+            return
+        N2 = max(int(N), self.N + self.N // 2) if N > self.N else self.N
+        Tp2 = -(-max(int(T), self.Tp) // 16) * 16
+        hp, dev = self.native.hp, self.device
+        stats = torch.zeros(N2, Tp2, 2 * hp.inter_channels, device=dev)
+        cum = torch.zeros(N2, Tp2, dtype=torch.int32, device=dev)
+        g = torch.zeros(N2, hp.gin_channels, device=dev)
+        y_lengths = torch.zeros(N2, dtype=torch.int64, device=dev)
+        if self.N:
+            self.native.tts_state_rows(range(self.N), stats, cum, g, y_lengths,
+                                       src=(self.stats, self.cum, self.g, self.y_lengths))
+        self.stats, self.cum, self.g, self.y_lengths, self.N, self.Tp = stats, cum, g, y_lengths, N2, Tp2
+
+
 _POOL = None
 
 
@@ -389,24 +417,32 @@ class NativeSynthesizer:
                                       items=a["dec_items"])
         return o[:, 0], frames
 
-    def _tts_args(self, x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams):
-        """The checks and device inputs ``infer`` and ``tts_encode`` share: validated tokens, lengths and speakers on the
-        device, the call's key, the per-item parameter arrays of both halves, and each row's decode key, stream and
-        noise scale as host lists (what the whole decode draws row b with)."""
+    def check_tts_input(self, x, sid):
+        """The token and speaker checks of ``infer`` / ``tts_encode``, before anything is launched: RuntimeError for a
+        checkpoint without the TTS half, ValueError for a token id outside [0, n_vocab), a missing ``sid`` or a speaker id
+        outside [0, n_speakers).  ``x``: int64 token ids (any shape, at least one); returns ``sid`` as a flat int64
+        tensor."""
         info = self.native.tts_info()
         if not info["has_tts"]:
             raise RuntimeError("this checkpoint has no enc_p / dp / sdp / emb_g: infer() needs a V1 base speaker")
-        x = x.to(torch.int64)
         if int(x.min()) < 0 or int(x.max()) >= info["n_vocab"]:
             raise ValueError(f"token ids must lie in [0, {info['n_vocab']})")
-        x = x.to(self.device).contiguous()
-        B, T = x.shape
-        x_lengths = x_lengths.to(self.device, torch.int64).contiguous()
         if sid is None:
             raise ValueError("sid is required (n_speakers > 0)")
         sid = sid.to(torch.int64).reshape(-1)
         if int(sid.min()) < 0 or int(sid.max()) >= info["n_speakers"]:
             raise ValueError(f"speaker ids must lie in [0, {info['n_speakers']})")
+        return sid
+
+    def _tts_args(self, x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams):
+        """The checks and device inputs ``infer`` and ``tts_encode`` share: validated tokens, lengths and speakers on the
+        device, the call's key, the per-item parameter arrays of both halves, and each row's decode key, stream and
+        noise scale as host lists (what the whole decode draws row b with)."""
+        x = x.to(torch.int64)
+        sid = self.check_tts_input(x, sid)
+        x = x.to(self.device).contiguous()
+        B, T = x.shape
+        x_lengths = x_lengths.to(self.device, torch.int64).contiguous()
         sid = sid.to(self.device).contiguous()
         seeds = check_seeds(seeds, B)
         if streams is not None:
@@ -440,18 +476,33 @@ class NativeSynthesizer:
     @torch.no_grad()
     def tts_encode(self, x, x_lengths, sid=None, noise_scale=1, length_scale=1, noise_scale_w=1.0, sdp_ratio=0.2,
                    seed: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
-                   streams: Optional[Sequence[int]] = None) -> "TtsState":
+                   streams: Optional[Sequence[int]] = None, pool: Optional["TtsPool"] = None,
+                   rows: Optional[Sequence[int]] = None) -> "TtsState":
         """The encode half of ``infer`` (same arguments and draws), returning state the caller owns: a later
         ``tts_encode`` or ``infer`` does not change it.  ``tts_decode_windows`` decodes any frames of its rows, each
         row with the decode key, stream and noise scale ``infer`` would give it.  One host sync (y_lengths), as in
-        ``infer``."""
+        ``infer``.
+
+        ``pool`` / ``rows``: encoded row b is written into row ``rows[b]`` of ``pool`` instead (one
+        ``ovc_tts_encode_state_rows``; the pool grows to fit first).  The returned state then holds the pool's tensors,
+        and its host lists (frames, decode keys, streams, noise scales) describe the encoded rows in order."""
         a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams)
         x = a["x"]
+        B, T = x.shape
+        if pool is not None:
+            rows = [int(r) for r in rows]
+            if len(rows) != B or min(rows) < 0:
+                raise ValueError(f"tts_encode: {len(rows)} pool rows for {B} encoded rows (each >= 0)")
+            pool.fit(max(rows) + 1, T)
         y_lengths, _, _ = self.native.tts_encode(x, a["x_lengths"], a["sid"], seed=a["seed"], items=a["enc_items"],
                                                  **a["enc_scalars"])
-        stats, cum, g = self.native.tts_encode_state(x.shape[0], x.shape[1], self.device)
+        if pool is None:
+            stats, cum, g = self.native.tts_encode_state(B, T, self.device)
+        else:
+            stats, cum, g, _ = self.native.tts_state_rows(rows, pool.stats, pool.cum, pool.g, pool.y_lengths)
         frames = [int(v) for v in y_lengths.cpu()]             # the sync
-        return TtsState(stats, cum, g, y_lengths, frames, a["dec_keys"], a["dec_streams"], a["dec_noise_scale"])
+        return TtsState(stats, cum, g, y_lengths if pool is None else pool.y_lengths, frames, a["dec_keys"],
+                        a["dec_streams"], a["dec_noise_scale"])
 
     @torch.no_grad()
     def tts_decode_windows(self, state: "TtsState", windows: Sequence[Tuple[int, int, int]], w_max: Optional[int] = None,
@@ -585,25 +636,37 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
         speeds = []
         for r, q in enumerate(reqs):
             ids = q["ids"] if "ids" in q else self._sentences(q["text"], q.get("language", "English"))
-            spk = q["speaker"]
-            spk = self.hps.speakers[spk] if isinstance(spk, str) else int(spk)
-            speed = float(q.get("speed", 1.0))
-            if not (math.isfinite(speed) and speed > 0):
-                raise ValueError(f"request {r}: speed {speed!r} must be a positive number")
-            seed = q.get("seed")
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None else check_seeds([seed], 1, "seed")[0]
-            speeds.append(speed)
+            k = self._request_keys(q, f"request {r}")
+            speeds.append(k["speed"])
             for j, q_ids in enumerate(ids):
                 seqs.append(list(q_ids))
-                sid.append(spk)
-                seeds.append(seed)
+                sid.append(k["speaker"])
+                seeds.append(k["seed"])
                 streams.append(j)
                 owner.append(r)
-                par["noise_scale"].append(float(q.get("noise_scale", 0.667)))
-                par["noise_scale_w"].append(float(q.get("noise_scale_w", 0.6)))
-                par["length_scale"].append(1.0 / speed)
-                par["sdp_ratio"].append(float(q.get("sdp_ratio", 0.2)))
+                self._sentence_params(k, par)
         return seqs, sid, owner, speeds, dict(seeds=seeds, streams=streams, **par)
+
+    def _request_keys(self, q, who: str) -> dict:
+        """The TTS keys of one request (all but its text), validated: speaker id, speed, seed (drawn from torch's
+        generator when absent) and the noise parameters.  ValueError names the request as ``who``."""
+        spk = q["speaker"]
+        spk = self.hps.speakers[spk] if isinstance(spk, str) else int(spk)
+        speed = float(q.get("speed", 1.0))
+        if not (math.isfinite(speed) and speed > 0):
+            raise ValueError(f"{who}: speed {speed!r} must be a positive number")
+        seed = q.get("seed")
+        seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None else check_seeds([seed], 1, "seed")[0]
+        return dict(speaker=spk, speed=speed, seed=seed, noise_scale=float(q.get("noise_scale", 0.667)),
+                    noise_scale_w=float(q.get("noise_scale_w", 0.6)), sdp_ratio=float(q.get("sdp_ratio", 0.2)))
+
+    @staticmethod
+    def _sentence_params(k: dict, par: dict) -> None:
+        """Append one sentence's ``infer`` parameters, for a request with keys ``k`` (``_request_keys``), to ``par``."""
+        par["noise_scale"].append(k["noise_scale"])
+        par["noise_scale_w"].append(k["noise_scale_w"])
+        par["length_scale"].append(1.0 / k["speed"])
+        par["sdp_ratio"].append(k["sdp_ratio"])
 
     @staticmethod
     def _pad_ids(sequences):
@@ -875,42 +938,58 @@ class ToneColorConverter(OpenVoiceBaseClass):
         and watermark message; the embeddings stay on the host.  ValueError for a request without sentences, a missing or mis-sized embedding, a tau
         that is not finite, a bad seed, or models on different devices."""
         reqs = list(requests)
-        if torch.device(tts.model.device) != torch.device(self.model.device):
-            raise ValueError(f"the TTS model is on {tts.model.device} and the converter on {self.model.device}")
+        self._check_same_device(tts)
         seqs, sid, owner, speeds, kw = tts._request_sentences(reqs)
-        gin = int(getattr(self.hps.model, "gin_channels", 256))
         ses = {"src_se": [], "tgt_se": []}
         taus, seeds, messages = [], [], []
         for r, q in enumerate(reqs):
             if r not in owner:
                 raise ValueError(f"request {r} has no sentences")
+            k = self._clone_keys(q, f"request {r}")
             for name in ses:
-                if q.get(name) is None:
-                    raise ValueError(f"request {r} has no {name}")
-                se = torch.as_tensor(q[name], dtype=torch.float32).reshape(1, -1)
-                if se.shape[1] != gin:
-                    raise ValueError(f"request {r}: {name} has {se.shape[1]} values, the converter's embeddings have {gin}")
-                ses[name].append(se)
-            tau = float(q.get("tau", 0.3))
-            if not math.isfinite(tau):
-                raise ValueError(f"request {r}: tau = {tau!r} is not a finite number")
-            taus.append(tau)
-            seed = q.get("convert_seed")
-            seeds.append(int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None
-                         else check_seeds([seed], 1, f"request {r}: convert_seed")[0])
-            messages.append(q.get("message", "default"))
+                ses[name].append(k[name])
+            taus.append(k["tau"])
+            seeds.append(k["convert_seed"])
+            messages.append(k["message"])
         stack = {k: torch.cat(v, 0) if v else None for k, v in ses.items()}
         return (seqs, sid, owner, speeds, kw), stack["src_se"], stack["tgt_se"], taus, seeds, messages
 
-    def _check_clone_lengths(self, lengths, rate):
+    def _check_same_device(self, tts):
+        if torch.device(tts.model.device) != torch.device(self.model.device):
+            raise ValueError(f"the TTS model is on {tts.model.device} and the converter on {self.model.device}")
+
+    def _clone_keys(self, q, who: str) -> dict:
+        """The conversion keys of one clone request, validated: ``src_se`` / ``tgt_se`` ([1, gin] on the host), ``tau``,
+        ``convert_seed`` (drawn from torch's generator when absent) and ``message``.  ValueError names it as ``who``."""
+        gin = int(getattr(self.hps.model, "gin_channels", 256))
+        out = {}
+        for name in ("src_se", "tgt_se"):
+            if q.get(name) is None:
+                raise ValueError(f"{who} has no {name}")
+            se = torch.as_tensor(q[name], dtype=torch.float32).reshape(1, -1)
+            if se.shape[1] != gin:
+                raise ValueError(f"{who}: {name} has {se.shape[1]} values, the converter's embeddings have {gin}")
+            out[name] = se
+        tau = float(q.get("tau", 0.3))
+        if not math.isfinite(tau):
+            raise ValueError(f"{who}: tau = {tau!r} is not a finite number")
+        seed = q.get("convert_seed")
+        out["tau"] = tau
+        out["convert_seed"] = (int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None
+                               else check_seeds([seed], 1, f"{who}: convert_seed")[0])
+        out["message"] = q.get("message", "default")
+        return out
+
+    def _check_clone_lengths(self, lengths, rate, names: Optional[Sequence[str]] = None):
         """ValueError for an utterance ``convert`` would refuse: shorter than one hop or not past the STFT padding
-        (after resampling from ``rate`` when it is given)."""
+        (after resampling from ``rate`` when it is given).  ``names[r]`` names utterance r (default "request r")."""
         hop = self.hps.data.hop_length
         pad = (self.hps.data.filter_length - hop) // 2
         for r, n in enumerate(lengths):
             m = self._resampled_len(n, rate)
             if m < hop or m <= pad:
-                raise ValueError(f"request {r}: its utterance has {m} samples{'' if rate is None else ' after resampling'}: "
+                who = f"request {r}" if names is None else names[r]
+                raise ValueError(f"{who}: its utterance has {m} samples{'' if rate is None else ' after resampling'}: "
                                  f"needs at least one hop ({hop}) and more than the STFT reflect padding ({pad})")
 
     @torch.no_grad()
@@ -967,67 +1046,39 @@ class ToneColorConverter(OpenVoiceBaseClass):
         requests are still being synthesised.  Requests as in ``clone_batch``; the TTS encode of all their sentences
         runs here, so malformed requests and too-short utterances raise ValueError before the first step.
 
-        Each request is a ``streaming.StreamingSessions`` session (``window_frames``-frame converter windows, the
-        request's embeddings, tau and ``convert_seed``).  A step is one batched launch sequence over every unfinished
-        request: ONE ``tts_decode_windows`` call decodes, per request, the next TTS windows (``plan_tts_windows``:
-        ``first_window_frames`` then ``window_frames`` frames) until its converter can emit a window or its text is
-        done; ONE ``ovc_splice`` writes the windows' interiors and the sentences' 50 ms / speed gaps into the sessions'
-        rings; then one ring spectrogram and ragged conversion of every ready window, and one download.  A request is
-        closed in the step that writes its last gap.  Every step yields one non-empty chunk per unfinished request, in
+        Each request is a ``streaming.CloneSessions`` session that says all its sentences at once and ends: its
+        ``window_frames``-frame converter windows use the request's embeddings, tau and ``convert_seed``.  A step is
+        ``CloneSessions.step``, one batched launch sequence over every unfinished request: ONE ``tts_decode_windows``
+        call decodes, per request, the next TTS windows (``plan_tts_windows``: ``first_window_frames`` then
+        ``window_frames`` frames) until its converter can emit a window or its text is done; ONE ``ovc_splice`` writes
+        the windows' interiors and the sentences' 50 ms / speed gaps into the converter's rings; then one ring
+        spectrogram and ragged conversion of every ready window, and one download.  A request is closed in the step
+        that writes its last gap.  Every step yields one non-empty chunk per unfinished request, in
         request order; a request's chunks concatenate to its ``clone_batch`` array (same length; the TTS windows equal
         the whole decode to fp32 reordering).  The models must share a sampling rate (ValueError otherwise)."""
-        window_frames, first_window_frames = int(window_frames), int(first_window_frames)
-        if window_frames < 1 or first_window_frames < 1:
-            raise ValueError(f"window_frames ({window_frames}) and first_window_frames ({first_window_frames}) must be >= 1")
-        sr = int(self.hps.data.sampling_rate)
-        if int(tts.hps.data.sampling_rate) != sr:
-            raise ValueError(f"the TTS model runs at {tts.hps.data.sampling_rate} Hz and the converter at {sr} Hz: "
-                             f"clone_stream_batch needs one rate (clone_batch resamples)")
+        from .streaming import CloneSessions
         reqs = list(requests)
-        (seqs, sid, owner, speeds, kw), src, tgt, taus, seeds, _ = self._clone_requests(tts, reqs)
+        cs = CloneSessions(self, tts, window_frames=window_frames, first_window_frames=first_window_frames,
+                           label="request")
+        (seqs, _, owner, speeds, kw), _, _, taus, seeds, _ = self._clone_requests(tts, reqs)
         if not reqs:
             return iter(())
-        x, lens = tts._pad_ids(seqs)
-        state = tts.model.tts_encode(x, lens, sid=torch.as_tensor(sid, dtype=torch.int64), **kw)
-        self._check_clone_lengths(plan_clone(state.frames, owner, speeds, tts.hps.data.hop_length, sr)[1], None)
-        # per request: its TTS windows in order, (state row, lo, hi, e0, e1, zeros after the window)
-        plans: List[List[Tuple[int, int, int, int, int, int]]] = [[] for _ in reqs]
-        for i, r in enumerate(owner):
-            wins = plan_tts_windows(state.frames[i], first_window_frames if not plans[r] else window_frames,
-                                    window_frames, TTS_HALO_FRAMES)
-            gap = int((sr * 0.05) / speeds[r])
-            plans[r] += [(i, lo, hi, e0, e1, gap if k == len(wins) - 1 else 0) for k, (lo, hi, e0, e1) in enumerate(wins)]
-        return self._clone_stream(tts, state, plans, src, tgt, taus, seeds, window_frames)
+        for r, q in enumerate(reqs):                     # session r is request r, with the keys drawn above
+            mine = [i for i, o in enumerate(owner) if o == r]
+            keys = {k: q[k] for k in CloneSessions.OPEN_KEYS if k in q}
+            keys.update(seed=kw["seeds"][mine[0]], convert_seed=seeds[r], tau=taus[r], speed=speeds[r])
+            sid = cs.open(**keys)
+            cs._queue(sid, [seqs[i] for i in mine])       # checked by the encode below, for the whole call
+            cs.end(sid)
+        cs.encode_pending()
+        return self._clone_stream(cs)
 
-    @torch.no_grad()
-    def _clone_stream(self, tts, state, plans, src, tgt, taus, seeds, window_frames):
-        from .streaming import StreamingSessions, ready_frames
-        hop, nfft = self.hps.data.hop_length, self.hps.data.filter_length
-        ss = StreamingSessions(self, window_frames=window_frames)
-        ids = [ss.open(src[r], tgt[r], tau=taus[r], seed=seeds[r]) for r in range(len(plans))]
-        done = [0] * len(plans)                          # TTS windows of each request already pushed
-        live = list(range(len(plans)))
-        while live:
-            wins, runs, closing = [], {}, []
-            for r in live:
-                s = ss.sessions[ids[r]]
-                n_in, runs[ids[r]] = s.n_in, []
-                while done[r] < len(plans[r]):
-                    i, lo, hi, e0, e1, gap = plans[r][done[r]]
-                    runs[ids[r]] += [(len(wins), (e0 - lo) * hop, (e1 - e0) * hop)] + ([(-1, 0, gap)] if gap else [])
-                    wins.append((i, lo, hi - lo))
-                    n_in += (e1 - e0) * hop + gap
-                    done[r] += 1
-                    if ready_frames(n_in, hop, nfft, False) >= s.emitted + ss.W + ss.H:
-                        break
-                if done[r] == len(plans[r]):
-                    closing.append(ids[r])
-            o, _ = tts.model.tts_decode_windows(state, wins)
-            out = ss.push_device(runs, o, close=closing)
-            for r in live:
-                if len(out[ids[r]]):
-                    yield r, out[ids[r]]
-            live = [r for r in live if ids[r] not in closing]
+    @staticmethod
+    def _clone_stream(cs):
+        while cs.sessions:
+            out = cs.step()
+            for r in sorted(out):
+                yield r, out[r]
 
     # ------------------------------------------------------------------ one utterance per stream
     @torch.no_grad()

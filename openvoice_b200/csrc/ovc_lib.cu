@@ -1798,6 +1798,45 @@ int ovc_tts_encode_state(ovc_ctx* c, float* stats, int32_t* cum, float* g, void*
   return OVC_OK;
 }
 
+static int tts_state_rows(ovc_ctx* c, const float* stats, const int* cum, const float* g, const long long* y_len, int B, int T,
+                          const int64_t* dst_row, int N, int Tp, float* d_stats, int32_t* d_cum, float* d_g, int64_t* d_ylen,
+                          cudaStream_t st) {
+  if (!dst_row || !d_stats || !d_cum || !d_g || !d_ylen) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (N < 1 || Tp < T) return fail(OVC_ERR_INVALID, "pool of %d rows at pitch %d cannot take rows of %d tokens", N, Tp, T);
+  const long long per_row = (long long)Tp * 2 * c->tts.C + Tp + c->hp.gin_channels + 1;
+  const int gx = (int)std::max(1LL, std::min((per_row + 255) / 256, std::max(1LL, 4LL * c->sm_count / B)));
+  tts_state_rows_kernel<<<dim3(gx, std::min(B, 65535)), 256, 0, st>>>(stats, cum, g, y_len, B, T, 2 * c->tts.C, c->hp.gin_channels,
+                                                     (const long long*)dst_row, N, Tp, d_stats, d_cum, d_g,
+                                                     (long long*)d_ylen);
+  CK(cudaGetLastError());
+  return OVC_OK;
+}
+
+int ovc_tts_encode_state_rows(ovc_ctx* c, const int64_t* dst_row, int N, int Tp, float* stats, int32_t* cum, float* g,
+                              int64_t* y_lengths, void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
+  if (c->tts_B < 1) return fail(OVC_ERR_STATE, "ovc_tts_encode_state_rows needs a preceding ovc_tts_encode");
+  ON_DEVICE(c);
+  const int B = c->tts_B, T = c->tts_T;
+  const TtsWs TW = tts_ws_layout(c, B, T);
+  return tts_state_rows(c, c->d_tts + TW.STATS, reinterpret_cast<const int*>(c->d_tts + TW.cum),
+                        c->d_tts + TW.g, reinterpret_cast<const long long*>(c->d_tts + TW.ylen), B, T, dst_row, N, Tp,
+                        stats, cum, g, y_lengths, (cudaStream_t)stream);
+}
+
+int ovc_tts_state_rows(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths, int B,
+                       int T, const int64_t* dst_row, int N, int Tp, float* d_stats, int32_t* d_cum, float* d_g,
+                       int64_t* d_y_lengths, void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
+  if (!stats || !cum || !g || !y_lengths) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (B < 1 || T < 1) return fail(OVC_ERR_INVALID, "B and T must be positive (got %d, %d)", B, T);
+  ON_DEVICE(c);
+  return tts_state_rows(c, stats, cum, g, (const long long*)y_lengths, B, T, dst_row, N, Tp, d_stats, d_cum, d_g, d_y_lengths,
+                        (cudaStream_t)stream);
+}
+
 int ovc_tts_decode_windows(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths,
                            int N, int T, const int64_t* row, const int64_t* frame0, const int64_t* len, int W, int Wmax,
                            const uint64_t* seed, const int64_t* stream, const float* noise_scale, float* o, float* z_p,

@@ -372,6 +372,35 @@ __global__ void tts_window_rows_kernel(const float* g, const long long* y_len, i
   }
 }
 
+// Encoded rows -> rows of a state pool (ovc_tts_encode_state_rows / ovc_tts_state_rows): source row b (B rows of T tokens)
+// goes to pool row dst_row[b], clamped into [0, N), at token pitch Tp >= T.  Tokens T <= t < Tp get the padding a short
+// row gets inside an encode: cum keeps its last value (durations_row), stats are 0.  One item per element of the
+// destination row: Tp * C2 stats, Tp cum, gin g, one y_length.  grid (x: element blocks, y: rows), both strided.
+__global__ void __launch_bounds__(256) tts_state_rows_kernel(const float* __restrict__ stats, const int* __restrict__ cum,
+                                                             const float* __restrict__ g, const long long* __restrict__ y_len,
+                                                             int B, int T, int C2, int gin, const long long* __restrict__ dst_row,
+                                                             int N, int Tp, float* __restrict__ d_stats, int* __restrict__ d_cum,
+                                                             float* __restrict__ d_g, long long* __restrict__ d_ylen) {
+  const long long n_stats = (long long)Tp * C2, per_row = n_stats + Tp + gin + 1;
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const long long r = min(max(dst_row[b], 0LL), (long long)N - 1);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_row; i += (long long)gridDim.x * blockDim.x) {
+      if (i < n_stats) {
+        const int t = (int)(i / C2), c = (int)(i - (long long)t * C2);
+        d_stats[r * n_stats + i] = t < T ? stats[((size_t)b * T + t) * C2 + c] : 0.f;
+      } else if (i < n_stats + Tp) {
+        const int t = (int)(i - n_stats);
+        d_cum[r * Tp + t] = cum[(size_t)b * T + min(t, T - 1)];
+      } else if (i < n_stats + Tp + gin) {
+        const int k = (int)(i - n_stats - Tp);
+        d_g[r * gin + k] = g[(size_t)b * gin + k];
+      } else {
+        d_ylen[r] = y_len[b];
+      }
+    }
+  }
+}
+
 // out[c][t] = philox_normal(seed, stream, c0 + c, frame0 + t): the draws the kernels above make, as a tensor
 // (ovc_philox_normals).  grid (ceil(T/128), C)
 __global__ void philox_normals_kernel(unsigned long long seed, uint32_t stream, uint32_t c0, uint32_t frame0, int T,

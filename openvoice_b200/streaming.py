@@ -33,6 +33,7 @@ window's spectrogram in one launch, and one ragged voice conversion converts the
 ``stream_windows`` are the readiness and window rules both classes follow.
 """
 import math
+from collections import deque
 from typing import Callable, Dict, Iterable, List, Optional, Sequence, Set, Tuple
 
 import numpy as np
@@ -421,7 +422,7 @@ class StreamingSessions:
         close = set(close)
         if not close <= set(ids):
             raise ValueError("close names a session that has no runs in this call")
-        assert src.is_cuda and src.dtype == torch.float32 and src.is_contiguous() and src.dim() == 2
+        assert src.device.type == self.dev.type and src.dtype == torch.float32 and src.is_contiguous() and src.dim() == 2
         rows, pitch = src.shape
         xs = {}
         for sid in ids:
@@ -448,6 +449,12 @@ class StreamingSessions:
         for sid in ids:
             self.free_rows.append(self.sessions.pop(sid).row)
         return out
+
+    def discard(self, ids: Iterable[int]) -> None:
+        """Drop the named sessions without converting what is left of them (a caller that has gone away) and free their
+        rows for the next ``open``.  Nothing is launched."""
+        for sid in self._check_ids(ids):
+            self.free_rows.append(self.sessions.pop(sid).row)
 
     # ------------------------------------------------------------------ device buffers
     def _buf(self, name: str, numel: int, dtype, pinned: bool = False):
@@ -579,3 +586,273 @@ class StreamingSessions:
             s.n_in += counts[i]
             s.emitted = max([e1 for j, _, _, _, e1 in wins if j == i], default=s.emitted)
         return res
+
+
+class _CloneSession:
+    __slots__ = ("tts_keys", "conv_keys", "said", "unencoded", "plans", "length", "ended", "checked", "ss_id")
+
+    def __init__(self, tts_keys: dict, conv_keys: dict):
+        self.tts_keys, self.conv_keys = tts_keys, conv_keys
+        self.said = 0                                     # sentences said so far: the next one is sentence `said`
+        self.unencoded = 0                                # said sentences still waiting for the encode
+        self.plans: deque = deque()                       # TTS windows to decode: (pool row, lo, hi, e0, e1, gap, last)
+        self.length = 0                                   # samples of the encoded sentences and their gaps
+        self.ended = False
+        self.checked = False                              # ended, fully encoded and long enough to convert
+        self.ss_id: Optional[int] = None                  # its StreamingSessions session, from its first audio on
+
+
+class CloneSessions:
+    """Live text-to-cloned-voice sessions: requests open, receive text one sentence at a time and end while the others run,
+    and every ``step`` advances all of them with one batched launch sequence.
+
+    ``open`` takes the keys of a ``ToneColorConverter.clone_batch`` request other than its text and returns the session's
+    id; ``say(sid, text=... | ids=...)`` queues sentences through the text front end ``tts_batch`` uses; ``end`` marks
+    that no more text follows; ``cancel`` drops a session at once.  Sentence j of a session (counted across ``say``
+    calls) draws at (seed, stream j) with the session's parameters, as sentence j of the one-shot request does, so a
+    session's chunks concatenate to those of ``clone_stream_batch(tts, [request])`` for the request holding the same
+    sentences and keys, bit for bit, whenever its text arrives and whatever runs beside it.
+
+    A ``step`` is at most:
+      1. ONE ragged ``tts_encode`` of every sentence said since the last step (one host sync, for the frame counts),
+         written by ONE ``ovc_tts_encode_state_rows`` into free rows of a ``TtsPool`` shared by all sessions.  The pool
+         is grow-only (a larger token pitch re-pitches it once, one more copy) and a sentence's row is freed once its
+         last window is decoded.
+      2. ONE ``tts_decode_windows`` over the pool: per session, the next TTS windows (``plan_tts_windows``;
+         ``first_window_frames`` for its first sentence only) until its converter can emit a window or its encoded text
+         runs out.
+      3. ONE ``StreamingSessions.push_device`` of every session's window interiors and 50 ms / speed gaps, closing the
+         sessions that have ended and whose last gap is written (``close`` alone when a session ended after that).
+    A session waiting for text costs nothing; a step in which nothing can advance returns {} and launches nothing.
+
+    Bad input is refused where its session can be named: keys in ``open``, token and speaker ids in ``say`` (the session
+    keeps what it had said), so the shared encode of a step only sees checked text.  An encode that still fails takes no
+    pool rows and keeps the text for the next step.  A session whose whole utterance turns out too short to convert
+    raises ValueError naming it in the step where its length becomes known, before that step's decode; it is cancelled
+    and the others continue on the next ``step``.  Both
+    models must be on one device and at one sampling rate (ValueError here)."""
+
+    OPEN_KEYS = ("speaker", "src_se", "tgt_se", "tau", "seed", "convert_seed", "speed", "noise_scale", "noise_scale_w",
+                 "sdp_ratio")
+
+    def __init__(self, converter, tts, window_frames: int = 256, first_window_frames: int = 32, label: str = "session"):
+        """``label``: how errors name a session ("session 3"); ``clone_stream_batch`` passes "request"."""
+        W, W1 = int(window_frames), int(first_window_frames)
+        if W < 1 or W1 < 1:
+            raise ValueError(f"window_frames ({W}) and first_window_frames ({W1}) must be >= 1")
+        sr = int(converter.hps.data.sampling_rate)
+        if int(tts.hps.data.sampling_rate) != sr:
+            raise ValueError(f"the TTS model runs at {tts.hps.data.sampling_rate} Hz and the converter at {sr} Hz: "
+                             f"streaming text to cloned voice needs one rate (clone_batch resamples)")
+        converter._check_same_device(tts)
+        self.conv, self.tts, self.W, self.W1, self.sr, self.label = converter, tts, W, W1, sr, label
+        self.hop, self.nfft = converter.hps.data.hop_length, converter.hps.data.filter_length
+        self.H = converter.HALO_FRAMES
+        self.sessions: Dict[int, _CloneSession] = {}
+        self.next_id = 0
+        self.pending: List[Tuple[int, List[int]]] = []   # (session, token ids) said since the last encode, in order
+        self.ss: Optional[StreamingSessions] = None       # the converter side, made with the first audio
+        self.pool = None                                  # api.TtsPool, made with the first encode
+        self.free_rows: List[int] = []
+        self.rows = 0                                     # pool rows handed out so far
+        # host side of each pool row: decoded frames, decode key, stream and noise scale of its sentence
+        self.row_frames: List[int] = []
+        self.row_keys: List[int] = []
+        self.row_streams: List[int] = []
+        self.row_noise: List[float] = []
+        self._fresh: List[Tuple[object, List[Tuple[int, int]]]] = []   # (encode state, [(its row i, pool row)]) whose
+                                                                          # decode keys are not in the row lists yet
+
+    # ------------------------------------------------------------------ sessions
+    def open(self, speaker, src_se=None, tgt_se=None, tau: float = 0.3, seed: Optional[int] = None,
+             convert_seed: Optional[int] = None, speed: float = 1.0, noise_scale: float = 0.667,
+             noise_scale_w: float = 0.6, sdp_ratio: float = 0.2) -> int:
+        """Start a session and return its id.  The keys are those of a ``clone_batch`` request, validated as it
+        validates them, and the noise parameters as the encode checks them (ValueError naming the session); ``seed`` /
+        ``convert_seed`` default to draws from torch's generator.  The speaker id is checked against the checkpoint
+        with the session's first ``say``."""
+        from .api import check_per_item
+        q = dict(speaker=speaker, src_se=src_se, tgt_se=tgt_se, tau=tau, seed=seed, convert_seed=convert_seed,
+                 speed=speed, noise_scale=noise_scale, noise_scale_w=noise_scale_w, sdp_ratio=sdp_ratio)
+        who = f"{self.label} {self.next_id}"
+        tts_keys = self.tts._request_keys(q, who)
+        for name in ("noise_scale", "noise_scale_w", "sdp_ratio"):
+            check_per_item([tts_keys[name]], 1, f"{who}: {name}")
+        conv_keys = self.conv._clone_keys(q, who)
+        sid = self.next_id
+        self.next_id += 1
+        self.sessions[sid] = _CloneSession(tts_keys, conv_keys)
+        return sid
+
+    def _session(self, sid) -> _CloneSession:
+        s = self.sessions.get(sid)
+        if s is None:
+            raise ValueError(f"unknown or closed {self.label} {sid!r}")
+        return s
+
+    def say(self, sid: int, text: Optional[str] = None, ids: Optional[Sequence[Sequence[int]]] = None,
+            language: str = "English") -> None:
+        """Queue sentences for session ``sid``: ``ids`` (token-id lists, one per sentence) or ``text`` through the TTS
+        model's front end.  They are encoded in the next ``step``.  ValueError for an unknown or ended session, no
+        sentences, a token id outside the vocabulary or a session speaker outside the checkpoint's speakers
+        (``NativeSynthesizer.check_tts_input``, the encode's own check); the session keeps what it had said before."""
+        ids = self._sentences(sid, text, ids, language)
+        flat = [t for q in ids for t in q]
+        try:
+            self.tts.model.check_tts_input(torch.as_tensor(flat or [0], dtype=torch.int64),
+                                           torch.as_tensor([self.sessions[sid].tts_keys["speaker"]], dtype=torch.int64))
+        except ValueError as e:
+            raise ValueError(f"{self.label} {sid}: {e}") from None
+        self._queue(sid, ids)
+
+    def _sentences(self, sid, text, ids, language) -> List[List[int]]:
+        s = self._session(sid)
+        if s.ended:
+            raise ValueError(f"{self.label} {sid} has ended: it takes no more text")
+        if ids is None:
+            if text is None:
+                raise ValueError("say needs text or ids")
+            ids = self.tts._sentences(text, language)
+        ids = [list(q) for q in ids]
+        if not ids:
+            raise ValueError(f"{self.label} {sid}: no sentences to say")
+        return ids
+
+    def _queue(self, sid: int, ids: List[List[int]]) -> None:
+        """``say`` after its checks.  ``clone_stream_batch`` queues here: its eager encode checks every sentence of the
+        call before the generator is returned, so a bad request fails the whole call and no step ever runs."""
+        s = self.sessions[sid]
+        self.pending += [(sid, q) for q in ids]
+        s.said += len(ids)
+        s.unencoded += len(ids)
+
+    def end(self, sid: int) -> None:
+        """No more text for session ``sid``: it closes once its audio is out."""
+        s = self._session(sid)
+        if s.ended:
+            raise ValueError(f"{self.label} {sid} has already ended")
+        s.ended = True
+
+    def cancel(self, sid: int) -> None:
+        """Drop session ``sid`` now: its queued text, pool rows and converter row are freed; it returns nothing more."""
+        s = self._session(sid)
+        self.pending = [(o, q) for o, q in self.pending if o != sid]
+        self.free_rows += sorted({p[0] for p in s.plans})
+        if s.ss_id is not None:
+            self.ss.discard([s.ss_id])
+        del self.sessions[sid]
+
+    @property
+    def pool_rows_in_use(self) -> int:
+        return self.rows - len(self.free_rows)
+
+    # ------------------------------------------------------------------ one step
+    def encode_pending(self) -> None:
+        """The encode half of ``step``: one ragged encode of every sentence said since the last step into free pool rows,
+        then the length check of every session whose utterance is now complete (ValueError naming the first one too
+        short, after cancelling each such session)."""
+        if self.pending:
+            self._encode()
+        bad = []
+        for sid, s in self.sessions.items():
+            if s.ended and not s.unencoded and not s.checked:
+                try:
+                    self.conv._check_clone_lengths([s.length], None, names=[f"{self.label} {sid}"])
+                    s.checked = True
+                except ValueError as e:
+                    bad.append((sid, e))
+        for sid, _ in bad:
+            self.cancel(sid)
+        if bad:
+            raise bad[0][1]
+
+    def _encode(self) -> None:
+        from .api import TTS_HALO_FRAMES, TtsPool, plan_tts_windows
+        tts = self.tts
+        seqs, spk = [q for _, q in self.pending], []
+        kw = {"seeds": [], "streams": [], "noise_scale": [], "noise_scale_w": [], "length_scale": [], "sdp_ratio": []}
+        nth: Dict[int, int] = {}
+        for sid, _ in self.pending:
+            s = self.sessions[sid]
+            j = s.said - s.unencoded + nth.get(sid, 0)    # the sentence's number in its session
+            nth[sid] = nth.get(sid, 0) + 1
+            spk.append(s.tts_keys["speaker"])
+            kw["seeds"].append(s.tts_keys["seed"])
+            kw["streams"].append(j)
+            tts._sentence_params(s.tts_keys, kw)
+        # free rows first, then new ones; they are taken only once the encode has gone through
+        take = self.free_rows[:len(seqs)]
+        new = list(range(self.rows, self.rows + len(seqs) - len(take)))
+        rows = take + new
+        if self.pool is None:
+            self.pool = TtsPool(tts.model.native, tts.model.device)
+        x, lens = tts._pad_ids(seqs)
+        state = tts.model.tts_encode(x, lens, sid=torch.as_tensor(spk, dtype=torch.int64), pool=self.pool, rows=rows, **kw)
+        del self.free_rows[:len(take)]
+        self.rows += len(new)
+        for lst, v in ((self.row_frames, 0), (self.row_keys, 0), (self.row_streams, 0), (self.row_noise, 0.0)):
+            lst += [v] * len(new)
+        self._fresh.append((state, list(enumerate(rows))))
+        for i, ((sid, _), row) in enumerate(zip(self.pending, rows)):
+            s = self.sessions[sid]
+            frames = state.frames[i]
+            self.row_frames[row] = frames
+            wins = plan_tts_windows(frames, self.W1 if kw["streams"][i] == 0 else self.W, self.W, TTS_HALO_FRAMES)
+            gap = int((self.sr * 0.05) / s.tts_keys["speed"])
+            s.plans += [(row, lo, hi, e0, e1, gap if k == len(wins) - 1 else 0, k == len(wins) - 1)
+                        for k, (lo, hi, e0, e1) in enumerate(wins)]
+            s.length += self.hop * frames + gap
+            s.unencoded -= 1
+        self.pending = []
+
+    @torch.no_grad()
+    def step(self) -> Dict[int, np.ndarray]:
+        """Advance every session that can advance; returns {sid: float32 chunk} for each session that produced audio.
+        Sessions that have ended and whose audio is all out are closed (and forgotten) here."""
+        from .api import TtsState
+        self.encode_pending()
+        hop, ss = self.hop, self.ss
+        wins, runs, closing, done_rows = [], {}, [], []
+        for sid, s in self.sessions.items():
+            if s.plans:
+                st = None if s.ss_id is None else ss.sessions[s.ss_id]
+                n_in, emitted = (0, 0) if st is None else (st.n_in, st.emitted)
+                r = runs[sid] = []
+                while s.plans:
+                    row, lo, hi, e0, e1, gap, last = s.plans.popleft()
+                    r += [(len(wins), (e0 - lo) * hop, (e1 - e0) * hop)] + ([(-1, 0, gap)] if gap else [])
+                    wins.append((row, lo, hi - lo))
+                    if last:
+                        done_rows.append(row)
+                    n_in += (e1 - e0) * hop + gap
+                    if ready_frames(n_in, hop, self.nfft, False) >= emitted + self.W + self.H:
+                        break
+            if s.checked and not s.plans:
+                closing.append(sid)
+                runs.setdefault(sid, [])
+        if not runs:
+            return {}
+        if self.ss is None:
+            self.ss = ss = StreamingSessions(self.conv, window_frames=self.W)
+        for sid in runs:
+            s = self.sessions[sid]
+            if s.ss_id is None:
+                c = s.conv_keys
+                s.ss_id = ss.open(c["src_se"], c["tgt_se"], tau=c["tau"], seed=c["convert_seed"])
+        sids = {sid: self.sessions[sid].ss_id for sid in runs}
+        if wins:
+            for enc, pairs in self._fresh:               # each row's decode key, stream and noise scale, as encoded
+                for i, row in pairs:
+                    self.row_keys[row], self.row_streams[row] = enc.dec_keys[i], enc.dec_streams[i]
+                    self.row_noise[row] = enc.dec_noise_scale[i]
+            self._fresh = []
+            state = TtsState(self.pool.stats, self.pool.cum, self.pool.g, self.pool.y_lengths, self.row_frames,
+                             self.row_keys, self.row_streams, self.row_noise)
+            o, _ = self.tts.model.tts_decode_windows(state, wins)
+            out = ss.push_device({sids[sid]: r for sid, r in runs.items()}, o, close=[sids[sid] for sid in closing])
+        else:
+            out = ss.close([sids[sid] for sid in closing])
+        self.free_rows += done_rows                       # reused by a later encode, which the stream orders after
+        for sid in closing:
+            del self.sessions[sid]
+        return {sid: out[sids[sid]] for sid in runs if len(out[sids[sid]])}
