@@ -25,12 +25,12 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 11 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 12 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
                                * 8: ovc_spectrogram_ring; 9: OVC_OPT_PAIR_OCC; 10: ovc_splice;
-                               * 11: ovc_tts_encode_state_rows, ovc_tts_state_rows */
+                               * 11: ovc_tts_encode_state_rows, ovc_tts_state_rows; 12: OVC_OPT_STAGED_EPI */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -389,6 +389,11 @@ OVC_API int ovc_set_precision(ovc_ctx* ctx, int mode);
 #define OVC_OPT_PAIR_OCC 9   /* 1 (default): the conv pairs of the C = 32 / 64 stages run two CTAs per SM where that is
                               * measured faster (tc_pair_occ), so one tile's MMAs overlap another's epilogue; 0: one CTA
                               * per SM everywhere.  Results are bit-identical */
+#define OVC_OPT_STAGED_EPI 10 /* 1 (default): the tensor-core convs of column tile 128 and the C = 128 conv pairs stage each
+                               * tile's conv result in shared memory and a fourth warpgroup runs its epilogue (bias, residual,
+                               * MRF accumulate, scale, stores) while the MMA warpgroups compute the next tile; 0: the MMA
+                               * warpgroups run it themselves.  Applied where it is measured faster (split precision,
+                               * k >= 5: tc_stage_pays).  Results are bit-identical */
 OVC_API int ovc_set_option(ovc_ctx* ctx, int key, int value);
 
 /* Number of kernels the last ovc_voice_conversion / ovc_convert_waveform call launched. */

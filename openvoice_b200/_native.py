@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -285,8 +285,8 @@ class NativeConverter:
         self.precision = mode
 
     def set_option(self, key: str, value: int):
-        """Tuning switches of include/ovc.h: 'tts_simple', 'graph', 'pdl' (0/1/2), 'branches', 'pair', 'pair_occ' (0/1)."""
-        k = {"tts_simple": 2, "graph": 3, "pdl": 5, "branches": 7, "pair": 8, "pair_occ": 9}[key]
+        """Tuning switches of include/ovc.h: 'tts_simple', 'graph', 'pdl' (0/1/2), 'branches', 'pair', 'pair_occ', 'staged_epi' (0/1)."""
+        k = {"tts_simple": 2, "graph": 3, "pdl": 5, "branches": 7, "pair": 8, "pair_occ": 9, "staged_epi": 10}[key]
         _check(self.lib, self.lib.ovc_set_option(self.handle, k, int(value)), "ovc_set_option")
 
     # ---- hot path --------------------------------------------------------------------------

@@ -190,6 +190,7 @@ struct ovc_ctx {
   int par_frames = 512;
   bool use_pair = true;        // OVC_OPT_PAIR: the ResBlock conv pairs of the C <= 128 stages as ONE kernel (tcconv_kernel<C, true>, tc_pair_fuses)
   bool use_pair_occ = true;    // OVC_OPT_PAIR_OCC: pairs run two CTAs per SM where tc_pair_occ picks it
+  bool use_staged_epi = true;  // OVC_OPT_STAGED_EPI: the TN = 128 convs and C = 128 pairs hand their epilogue to a store warpgroup
   bool pair_occ2_ok[TCN_N_OCC2] = {};   // the device fits two CTAs per SM of kTcPairOcc2[i] (occupancy query at load)
   cudaStream_t br_stream[2] = {nullptr, nullptr};
   cudaEvent_t br_ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -637,19 +638,19 @@ static int finalize(ovc_ctx* c) {
   CK(cudaMemcpy(c->d_tcw, c->h_tcw.data(), c->h_tcw.size() * sizeof(float), cudaMemcpyHostToDevice));
   c->h_tcw.clear();
   c->h_tcw.shrink_to_fit();
-  CK(cudaFuncSetAttribute(tcconv_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<128, false>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcconv_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<64, false>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcconv_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<32, false>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcconv_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<128, true>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcconv_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<64, true>::SMEM_BYTES));
-  CK(cudaFuncSetAttribute(tcconv_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcnCfg<32, true>::SMEM_BYTES));
+  for (int TN : {128, 64, 32})
+    for (bool staged : {false, true}) {
+      const TcKernel k = tc_conv_kernel(TN, staged), p = tc_pair_kernel(TN, TcPairOcc(), staged);
+      CK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem));
+      CK(cudaFuncSetAttribute(p.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p.smem));
+    }
   for (int i = 0; i < TCN_N_OCC2; ++i) {
     // a config runs two CTAs per SM only where the device confirms they fit: otherwise its pairs keep one CTA per SM
     // (and a grid of one CTA per SM), never a doubled grid on one
-    const TcPairKernel k = tc_pair_kernel(kTcPairOcc2[i].C, kTcPairOcc2[i].o);
+    const TcKernel k = tc_pair_kernel(kTcPairOcc2[i].C, kTcPairOcc2[i].o);
     CK(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem));
     int blocks = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, k.fn, TCN_THREADS, k.smem));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, k.fn, k.threads, k.smem));
     c->pair_occ2_ok[i] = blocks >= 2;
     if (blocks < 2)
       fprintf(stderr, "ovc: the C = %d conv-pair kernel with %d operand buffer(s) fits %d CTA(s) per SM, not 2; its pairs run "
@@ -880,9 +881,8 @@ static int launch_tc(Run& r, const TcLayer& T, const float* x, float* y, const f
   const int n_tt = g.n_tt, total = g.total;
   dim3 pg((unsigned)g.grid_x, g.ncol, 1);
   const bool pdl = r.c->use_pdl == 1 || (r.c->use_pdl == 2 && ex.epi != 0);
-  if (T.TN == 128) CK(launch_ex(tcconv_kernel<128, false>, pg, TCN_THREADS, TcnCfg<128, false>::SMEM_BYTES, r.st, pdl, a, n_tt, total));
-  else if (T.TN == 64) CK(launch_ex(tcconv_kernel<64, false>, pg, TCN_THREADS, TcnCfg<64, false>::SMEM_BYTES, r.st, pdl, a, n_tt, total));
-  else CK(launch_ex(tcconv_kernel<32, false>, pg, TCN_THREADS, TcnCfg<32, false>::SMEM_BYTES, r.st, pdl, a, n_tt, total));
+  const TcKernel k = tc_conv_kernel(T.TN, r.c->use_staged_epi && tc_stage_pays(T.K, a.passes));
+  CK(launch_ex(k.fn, pg, k.threads, k.smem, r.st, pdl, a, n_tt, total));
   CK(cudaGetLastError());
   r.c->launches++;
   const double units = (double)r.B * t_len;
@@ -910,13 +910,13 @@ static int launch_pair(Run& r, const TcLayer& T1, const TcLayer& T2, const float
   TcPairOcc o = r.c->use_pair_occ ? tc_pair_occ(T1, T2) : TcPairOcc();
   for (int i = 0; i < TCN_N_OCC2; ++i)
     if (o.occ == 2 && kTcPairOcc2[i].C == C && kTcPairOcc2[i].o.nabuf == o.nabuf && !r.c->pair_occ2_ok[i]) o = TcPairOcc();
-  const TcPairKernel k = tc_pair_kernel(C, o);
+  const TcKernel k = tc_pair_kernel(C, o, r.c->use_staged_epi && tc_stage_pays(T1.K, a.passes));
   if (!k.fn) return fail(OVC_ERR_INVALID, "no conv-pair kernel for C = %d at %d CTA(s) per SM, %d operand buffer(s)", C, o.occ, o.nabuf);
   const TcGrid g = tc_pair_grid(t_len, r.B, T1.K, r.c->sm_count, o.occ);
   const int n_tt = g.n_tt, total = g.total;
   TRY(prof_begin(r));
   dim3 pg((unsigned)g.grid_x, 1, 1);
-  CK(launch_ex(k.fn, pg, TCN_THREADS, k.smem, r.st, false, a, n_tt, total));
+  CK(launch_ex(k.fn, pg, k.threads, k.smem, r.st, false, a, n_tt, total));
   CK(cudaGetLastError());
   r.c->launches++;
   const double units = (double)r.B * t_len;
@@ -1110,7 +1110,7 @@ static int set_call_params(ovc_ctx* c, uint64_t seed, float tau, const ItemParam
 }
 static uintptr_t option_bits(const ovc_ctx* c) {
   return (uintptr_t)c->precision | ((uintptr_t)c->use_pdl << 15) | ((uintptr_t)c->use_branches << 14) | ((uintptr_t)c->use_pair << 17) |
-         ((uintptr_t)c->use_pair_occ << 18);
+         ((uintptr_t)c->use_pair_occ << 18) | ((uintptr_t)c->use_staged_epi << 19);
 }
 
 static int ensure_ws(ovc_ctx* c, const WsLayout& W, int B, int Tmax, cudaStream_t st) {
@@ -1911,6 +1911,7 @@ int ovc_set_option(ovc_ctx* c, int key, int value) {
     case OVC_OPT_BRANCHES: c->use_branches = value != 0; return OVC_OK;
     case OVC_OPT_PAIR: c->use_pair = value != 0; return OVC_OK;
     case OVC_OPT_PAIR_OCC: c->use_pair_occ = value != 0; return OVC_OK;
+    case OVC_OPT_STAGED_EPI: c->use_staged_epi = value != 0; return OVC_OK;
     default: return fail(OVC_ERR_INVALID, "unknown option %d", key);
   }
 }

@@ -27,6 +27,8 @@
 //                tiles (two operand buffers); rows outside the utterance become zeros here (zero padding, x_mask and
 //                the ragged batch in one rule)
 //   warpgroups 1, 2  MMAs of 64 tile rows each (accumulators in registers), then the fused epilogue from registers
+//   warpgroup 3  STAGED only (TN = 128, tc_stage_pays): the MMA warpgroups stage each tile's results in shared memory and
+//                this warpgroup runs the epilogue from there while they compute the next tile
 // PAIR = true runs one ResBlock conv PAIR of the narrow generator stages in the same kernel:
 //   t = c1(lrelu(x)) (k taps, dilation d);  y = (c2(lrelu(t)) + x [+ y_old]) * scale (k taps, dilation 1)
 // The epilogue of conv 1 writes lrelu(t), split into hi/lo, straight into a shared-memory A operand of conv 2, so t
@@ -69,25 +71,37 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
-// Epilogue of one thread's two rows (tile rows row_a and row_a + 8, output steps t0 + row) x TN columns, straight from
-// the accumulator fragment d (ovc_tc.cuh: columns [0, TN) main accumulator, [TN, 2 TN) low-order accumulator).  Four
-// consecutive threads cover 32 contiguous bytes of an output row, so every global access of a warp is whole sectors.
+// The conv result of accumulator-fragment element j (j < TN / 2) of a thread: v = lo / 2^11 + hi (ovc_tc.cuh: fragment
+// columns [0, TN) main accumulator, [TN, 2 TN) low-order accumulator), or hi alone for the single pass.
 template <int TN>
-__device__ __forceinline__ void tc_epilogue(const TcConvArgs& a, const float (&d)[TN], int b, int t0, int n0, int lim, int row_a) {
+__device__ __forceinline__ float tc_result(const float (&d)[TN], bool two, int j) {
+  return two ? fmaf(d[TN / 2 + j], tc::kLoInv, d[j]) : d[j];
+}
+
+// Epilogue of one thread's two rows (tile rows row_a and row_a + 8, output steps t0 + row) x TN columns of an
+// accumulator fragment whose element j holds the conv result v_at(j) (tc_result).  The MMA warpgroups run it on their
+// registers; the store warpgroup of the staged kernels (TcnCfg::STAGED) on the same values read back from shared memory,
+// with the fragment layout of the MMA thread it stands in for, so both paths perform the same operations on the same
+// fp32 values.  Four consecutive threads cover 32 contiguous bytes of an output row, so every global access of a warp is
+// whole sectors.
+template <int TN, class V>
+__device__ __forceinline__ void tc_epilogue_v(const TcConvArgs& a, V v_at, int b, int t0, int n0, int lim, int row_a) {
   const int csub = (threadIdx.x & 3) * 2;
   float* yb = a.y + (size_t)b * a.y_bs;
   const float* rb = a.r ? a.r + (size_t)b * a.y_bs : nullptr;
   float* sb = a.s ? a.s + (size_t)b * a.s_bs : nullptr;
   const float* bias = a.bias + (size_t)b * a.bias_bs;
-  const bool two = a.passes == 3;
   const int ta = t0 + row_a, tb = ta + 8;
   const bool oka = ta < lim, okb = tb < lim;
 #pragma unroll
   for (int c0 = 0; c0 < TN; c0 += 32) {
     float v[16];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = two ? fmaf(d[TN / 2 + c0 / 2 + i], tc::kLoInv, d[c0 / 2 + i]) : d[c0 / 2 + i];
+    for (int i = 0; i < 16; ++i) v[i] = v_at(c0 / 2 + i);
 #pragma unroll
     for (int g = 0; g < 4; ++g) {
       const float2 bq = __ldg(reinterpret_cast<const float2*>(bias + n0 + c0 + 8 * g + csub));
@@ -152,6 +166,18 @@ __device__ __forceinline__ void tc_epilogue(const TcConvArgs& a, const float (&d
     }
   }
 }
+template <int TN>
+__device__ __forceinline__ void tc_epilogue(const TcConvArgs& a, const float (&d)[TN], int b, int t0, int n0, int lim, int row_a) {
+  const bool two = a.passes == 3;
+  tc_epilogue_v<TN>(a, [&](int j) { return tc_result<TN>(d, two, j); }, b, t0, n0, lim, row_a);
+}
+// the linear epilogue of a conv pair's conv 2: bias2, the pair's input as the residual, y_old, scale; rows past
+// t0 + R are the discarded output steps of the tile
+__device__ __forceinline__ TcConvArgs tc_pair_epilogue_args(const TcConvArgs& a, int TN) {
+  TcConvArgs e = a;
+  e.y_ld = TN; e.r = a.x; e.bias = a.bias2; e.bias_bs = 0; e.epi = 0;
+  return e;
+}
 
 // one k-step x tap of a warpgroup's 64 rows: main (+)= a_hi * b_hi^T, low (+)= a_hi * b_lo^T + a_lo * b_hi^T
 template <int TN>
@@ -165,14 +191,19 @@ __device__ __forceinline__ void tc_mma_step(float (&d)[TN], uint64_t a_hi, uint6
   }
 }
 
-constexpr int TCN_THREADS = 384;   // warpgroup 0: producers; warpgroups 1, 2: MMAs + epilogue
+constexpr int TCN_THREADS = 384;   // warpgroup 0: producers; warpgroups 1, 2: MMAs + epilogue (TcnCfg::THREADS unless STAGED)
 constexpr int TCN_NCT = 96;        // converter threads (warps 1-3)
 
-// OCC: CTAs per SM (2: pairs of the C = 32 / 64 stages only, ovc_tcpack.h tc_pair_occ); NAB: conv-1 operand buffers
-template <int TN, bool PAIR, int OCC = 1, int NAB = 2>
+// OCC: CTAs per SM (2: pairs of the C = 32 / 64 stages only, ovc_tcpack.h tc_pair_occ); NAB: conv-1 operand buffers;
+// STAGED (TN = 128, one CTA per SM): a fourth warpgroup runs the global epilogue of each tile from a staging tile in
+// shared memory while the MMA warpgroups go on with the next tile
+template <int TN, bool PAIR, int OCC = 1, int NAB = 2, bool STAGED = false>
 struct TcnCfg {
   static_assert(!PAIR || TN == 32 || TN == 64 || TN == 128, "conv pairs: C = 32, 64 or 128");
   static_assert(OCC == 1 || (PAIR && TN <= 64), "two CTAs per SM: C = 32 / 64 pairs");
+  static_assert(!STAGED || (TN == 128 && OCC == 1), "staged epilogue: TN = 128, one CTA per SM");
+  // warpgroup 0: producers; warpgroups 1, 2: MMAs (+ the epilogue unless STAGED); warpgroup 3 (STAGED): the epilogue
+  static constexpr int THREADS = STAGED ? TCN_THREADS + 128 : TCN_THREADS;
   static constexpr int KCH = 32, NKC = KCH / 8;                   // channels per converted A chunk
   static constexpr int ROWS = 194;                                // A pitch in rows: >= 128 + 2 * TCN_HMAX, = 2 (mod 8)
   static constexpr int ROWS2 = TCN_ROWS2;                         // PAIR: conv-2 A pitch: 128 + 2 * H2 rows, H2 <= 9
@@ -181,25 +212,37 @@ struct TcnCfg {
   static constexpr int SLOT_BYTES = 2 * 2 * TN * 16;
   static constexpr int A_BUF_BYTES = 2 * NKC * ROWS * 16;         // [hi|lo][column block][row][8 halfs]
   static constexpr int A2_BYTES = PAIR ? 2 * (TN / 8) * ROWS2 * 16 : 0;
-  static constexpr size_t SMEM_BYTES = 1024 + NABUF * A_BUF_BYTES + A2_BYTES + RING * SLOT_BYTES;
+  // STAGED: the conv results of one tile, fp32, [fragment element j < TN / 2][MMA thread t < 256] (conflict-free: a warp
+  // writes and reads 32 consecutive words).  A pair stages in its conv-2 operand, dead once conv 2's MMAs are done and
+  // not rewritten before the next tile's conv-1 epilogue; a single conv adds a buffer of its own.
+  static constexpr int STAGE_BYTES = STAGED ? (TN / 2) * 256 * 4 : 0;
+  static_assert(!STAGED || !PAIR || STAGE_BYTES <= A2_BYTES, "a pair's staging tile lies in its conv-2 operand");
+  static constexpr int SBUF_BYTES = STAGED && !PAIR ? STAGE_BYTES : 0;
+  static constexpr size_t SMEM_BYTES = 1024 + NABUF * A_BUF_BYTES + A2_BYTES + RING * SLOT_BYTES + SBUF_BYTES;
   static_assert(!PAIR || SMEM_BYTES == tc_pair_smem(TN, NABUF, RING), "tc_pair_smem");
   static_assert(SMEM_BYTES <= (OCC == 1 ? 232448 : TCN_SMEM_OCC2), "shared memory budget");
-  static_assert((2 * NABUF + 2 * RING) * 8 <= 1024, "barrier area");
-  // registers per thread after the producers hand theirs to the MMA warpgroups: 128 x 56 + 256 x 224 = 64 K at one CTA
-  // per SM, 128 x 32 + 256 x 104 = 30 K (of the 32 K the launch bounds give a CTA) at two
-  static constexpr int PROD_REGS = OCC == 1 ? 56 : 32, MMA_REGS = OCC == 1 ? 224 : 104;
+  static_assert((2 * NABUF + 2 * RING + 2) * 8 <= 1024, "barrier area");
+  // registers per thread after the producers hand theirs to the MMA warpgroups: 128 x 56 + 256 x 224 = 63 K at one CTA
+  // per SM, 128 x 32 + 256 x 104 = 30 K (of the 32 K the launch bounds give a CTA) at two.  STAGED: 128 x 32 (producers)
+  // + 256 x 184 (MMAs: the accumulators and, in a pair, the conv-1 epilogue; ptxas allocates 180 there) + 128 x 112 (the
+  // store warpgroup: room for many loads in flight; at 32 it spills) = 64 K
+  static constexpr int PROD_REGS = OCC == 1 && !STAGED ? 56 : 32, MMA_REGS = STAGED ? 184 : OCC == 1 ? 224 : 104;
+  static constexpr int STORE_REGS = 112;
+  static_assert(128 * PROD_REGS + 256 * MMA_REGS + (STAGED ? 128 * STORE_REGS : 0) <= 65536 / OCC, "register budget");
 };
 
-template <int TN, bool PAIR, int OCC = 1, int NAB = 2>
-__global__ void __launch_bounds__(TCN_THREADS, OCC) tcconv_kernel(const TcConvArgs a, int n_tt, int total) {
-  using Cfg = TcnCfg<TN, PAIR, OCC, NAB>;
+template <int TN, bool PAIR, int OCC = 1, int NAB = 2, bool STAGED = false>
+__global__ void __launch_bounds__(TcnCfg<TN, PAIR, OCC, NAB, STAGED>::THREADS, OCC) tcconv_kernel(const TcConvArgs a, int n_tt, int total) {
+  using Cfg = TcnCfg<TN, PAIR, OCC, NAB, STAGED>;
   constexpr int ROWS = Cfg::ROWS, ROWS2 = Cfg::ROWS2, NABUF = Cfg::NABUF, RING = Cfg::RING, NKC = Cfg::NKC;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
   uint64_t *a_full = bars, *a_empty = bars + NABUF, *b_full = a_empty + NABUF, *b_empty = b_full + RING;
+  uint64_t *s_full = b_empty + RING, *s_empty = s_full + 1;   // STAGED: the staging tile holds a tile / is free
   unsigned char* abuf = smem_raw + 1024;
   unsigned char* a2buf = abuf + NABUF * Cfg::A_BUF_BYTES;
   unsigned char* bring = a2buf + Cfg::A2_BYTES;
+  float* stage = reinterpret_cast<float*>(PAIR ? a2buf : bring + RING * Cfg::SLOT_BYTES);
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // provably warp-uniform
@@ -217,11 +260,12 @@ __global__ void __launch_bounds__(TCN_THREADS, OCC) tcconv_kernel(const TcConvAr
   if (tid == 0) {
     for (int i = 0; i < NABUF; ++i) { mbar_init(&a_full[i], TCN_NCT); mbar_init(&a_empty[i], 2); }
     for (int i = 0; i < RING; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 2); }
+    if (STAGED) { mbar_init(s_full, 256); mbar_init(s_empty, 128); }
     fence_mbar_init();
   }
   if (PAIR) {
     // rows of the conv-2 operand that conv 1 never produces (the taps of the discarded last output rows read them)
-    for (int i = tid; i < Cfg::A2_BYTES / 16; i += TCN_THREADS) reinterpret_cast<uint4*>(a2buf)[i] = make_uint4(0u, 0u, 0u, 0u);
+    for (int i = tid; i < Cfg::A2_BYTES / 16; i += Cfg::THREADS) reinterpret_cast<uint4*>(a2buf)[i] = make_uint4(0u, 0u, 0u, 0u);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
@@ -316,6 +360,27 @@ __global__ void __launch_bounds__(TCN_THREADS, OCC) tcconv_kernel(const TcConvAr
         }
       }
     }
+  } else if (STAGED && warp >= 12) {
+    // ------------------------------------------------------------ store warpgroup (STAGED): the global epilogue of each
+    // tile, for both MMA warpgroups' rows, from the staging tile
+    tc::regs_dealloc<Cfg::STORE_REGS>();
+    const int st = tid & 127;
+    uint32_t phase = 0;
+    TCN_FOR_TILES
+      // a pair's conv-1 epilogue rewrites the staging tile (its conv-2 operand): the previous tile has been read
+      if (PAIR) named_bar_arrive(1, 384);
+      mbar_wait(s_full, phase);
+      phase ^= 1;
+#pragma unroll 1
+      for (int h = 0; h < 2; ++h) {
+        const float* sv = stage + h * 128 + st;   // stands in for MMA thread 128 h + st
+        const auto v_at = [&](int j) { return sv[j * 256]; };
+        const int row_a = 64 * h + 16 * (warp & 3) + (lane >> 2);
+        if constexpr (PAIR) tc_epilogue_v<TN>(tc_pair_epilogue_args(a, TN), v_at, b, t0, 0, min(lim, t0 + R), row_a);
+        else tc_epilogue_v<TN>(a, v_at, b, t0, blockIdx.y * TN, lim, row_a);
+      }
+      if (!PAIR) mbar_arrive(s_empty);
+    }
   } else {
     // ------------------------------------------------------------ MMA warpgroups: rows [64 wg, +64) of every tile
     tc::regs_alloc<Cfg::MMA_REGS>();
@@ -330,6 +395,14 @@ __global__ void __launch_bounds__(TCN_THREADS, OCC) tcconv_kernel(const TcConvAr
     float d[TN];
 #pragma unroll
     for (int i = 0; i < TN; ++i) d[i] = 0.f;
+    // STAGED: this thread's conv results -> the staging tile, then on to the next tile (the store warpgroup takes it)
+    const auto stage_tile = [&]() {
+#pragma unroll
+      for (int j = 0; j < TN / 2; ++j) stage[j * 256 + tid - 128] = tc_result<TN>(d, three, j);
+      mbar_arrive(s_full);
+    };
+    uint32_t sphase = 1;   // the first tile finds the staging tile free
+    (void)sphase;
     if (resident)
       for (int it = 0; it < n_w; ++it) mbar_wait(&b_full[it], 0u);   // resident weights: waited on once
     int slot = 0, buf = 0;
@@ -370,10 +443,18 @@ __global__ void __launch_bounds__(TCN_THREADS, OCC) tcconv_kernel(const TcConvAr
         if (++buf == NABUF) { buf = 0; aphase ^= 1; }
       }
       if constexpr (!PAIR) {
-        tc_epilogue<TN>(a, d, b, t0, blockIdx.y * TN, lim, row_a);
+        if constexpr (STAGED) {
+          mbar_wait(s_empty, sphase);
+          sphase ^= 1;
+          stage_tile();
+        } else {
+          tc_epilogue<TN>(a, d, b, t0, blockIdx.y * TN, lim, row_a);
+        }
       } else {
         // ---- conv-1 epilogue: bias, leaky-relu, hi/lo split -> conv-2 A operand (rows = steps t0 - H2 + row)
-        named_bar_sync(1, 256);   // both warpgroups are done reading the conv-2 operand of the previous tile
+        // both warpgroups are done reading the conv-2 operand of the previous tile (and STAGED: the store warpgroup is
+        // done reading the previous tile's results staged there)
+        named_bar_sync(1, STAGED ? 384 : 256);
         unsigned char* a2h = a2buf;
         unsigned char* a2l = a2buf + (TN / 8) * ROWS2 * 16;
         const int ta = t0 - H2 + row_a, tb = ta + 8;
@@ -430,29 +511,55 @@ __global__ void __launch_bounds__(TCN_THREADS, OCC) tcconv_kernel(const TcConvAr
         tc::wgmma_wait<0>();
         tc::fence_regs(d);
         if (leader && prev >= 0) mbar_arrive(&b_empty[prev]);
-        TcConvArgs e = a;
-        e.y_ld = TN; e.r = a.x; e.bias = a.bias2; e.bias_bs = 0; e.epi = 0;
-        tc_epilogue<TN>(e, d, b, t0, 0, min(lim, t0 + R), row_a);
+        if constexpr (STAGED) {
+          // the staging tile overlays the conv-2 operand, and each warpgroup's MMAs read halo rows of the other's
+          named_bar_sync(3, 256);
+          // rows >= 128 of the operand (zero) are overwritten too: only the accumulator rows >= R read them, and
+          // those rows are the discarded output steps of every tile
+          stage_tile();
+        } else {
+          tc_epilogue<TN>(tc_pair_epilogue_args(a, TN), d, b, t0, 0, min(lim, t0 + R), row_a);
+        }
       }
     }
   }
 #undef TCN_FOR_TILES
 }
 
-// the pair-kernel instantiation of a (C, tc_pair_occ) config and its dynamic shared memory; fn = nullptr when none is built
-struct TcPairKernel {
+// a tcconv_kernel instantiation with its dynamic shared memory and block size; fn = nullptr when none is built
+struct TcKernel {
   void (*fn)(TcConvArgs, int, int) = nullptr;
   size_t smem = 0;
+  int threads = 0;
 };
-inline TcPairKernel tc_pair_kernel(int C, TcPairOcc o) {
+using TcPairKernel = TcKernel;   // the unstaged pair kernels: threads = TCN_THREADS
+template <int TN, bool PAIR, int OCC = 1, int NAB = 2, bool STAGED = false>
+inline TcKernel tc_kernel() {
+  using Cfg = TcnCfg<TN, PAIR, OCC, NAB, STAGED>;
+  return {tcconv_kernel<TN, PAIR, OCC, NAB, STAGED>, Cfg::SMEM_BYTES, Cfg::THREADS};
+}
+// whether a TN = 128 conv (or C = 128 pair) of k taps runs the staged epilogue when OVC_OPT_STAGED_EPI is on.  The store
+// warpgroup takes longer over a tile's epilogue than the two MMA warpgroups did, so it only pays where a tile's MMAs
+// outlast it: measured on an H100 (DESIGN.md, staged epilogue), split precision at k >= 5 gains, while k = 1 / 3 and
+// every single-pass shape but k = 11 lose or break even.
+inline bool tc_stage_pays(int K, int passes) { return passes * K >= 15; }
+// the single-conv kernel of column tile TN; staged: TN = 128 runs the staged epilogue (OVC_OPT_STAGED_EPI)
+inline TcKernel tc_conv_kernel(int TN, bool staged) {
+  if (TN == 128) return staged ? tc_kernel<128, false, 1, 2, true>() : tc_kernel<128, false>();
+  if (TN == 64) return tc_kernel<64, false>();
+  if (TN == 32) return tc_kernel<32, false>();
+  return {};
+}
+// the pair kernel of a (C, tc_pair_occ) config; staged: C = 128 runs the staged epilogue
+inline TcKernel tc_pair_kernel(int C, TcPairOcc o, bool staged = false) {
   if (o.occ == 1 && o.nabuf == 2) {
-    if (C == 128) return {tcconv_kernel<128, true>, TcnCfg<128, true>::SMEM_BYTES};
-    if (C == 64) return {tcconv_kernel<64, true>, TcnCfg<64, true>::SMEM_BYTES};
-    if (C == 32) return {tcconv_kernel<32, true>, TcnCfg<32, true>::SMEM_BYTES};
+    if (C == 128) return staged ? tc_kernel<128, true, 1, 2, true>() : tc_kernel<128, true>();
+    if (C == 64) return tc_kernel<64, true>();
+    if (C == 32) return tc_kernel<32, true>();
   } else if (o.occ == 2) {
-    if (C == 32 && o.nabuf == 2) return {tcconv_kernel<32, true, 2, 2>, TcnCfg<32, true, 2, 2>::SMEM_BYTES};
-    if (C == 32 && o.nabuf == 1) return {tcconv_kernel<32, true, 2, 1>, TcnCfg<32, true, 2, 1>::SMEM_BYTES};
-    if (C == 64 && o.nabuf == 1) return {tcconv_kernel<64, true, 2, 1>, TcnCfg<64, true, 2, 1>::SMEM_BYTES};
+    if (C == 32 && o.nabuf == 2) return tc_kernel<32, true, 2, 2>();
+    if (C == 32 && o.nabuf == 1) return tc_kernel<32, true, 2, 1>();
+    if (C == 64 && o.nabuf == 1) return tc_kernel<64, true, 2, 1>();
   }
   return {};
 }

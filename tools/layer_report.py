@@ -24,6 +24,7 @@ def main():
     ap.add_argument("--pdl", type=int, default=None)
     ap.add_argument("--pair", type=int, default=None)
     ap.add_argument("--pair-occ", type=int, default=None, help="0: every conv pair one CTA per SM; 1: tc_pair_occ")
+    ap.add_argument("--staged-epi", type=int, default=None, help="0: TN = 128 epilogues in the MMA warpgroups; 1: staged")
     ap.add_argument("--reps", type=int, default=1, help="profiled calls (per-variant times are averaged)")
     args = ap.parse_args()
     import numpy as np
@@ -48,6 +49,8 @@ def main():
         nat.set_option("pair", args.pair)
     if args.pair_occ is not None:
         nat.set_option("pair_occ", args.pair_occ)
+    if args.staged_epi is not None:
+        nat.set_option("staged_epi", args.staged_epi)
     nat.set_option("graph", 0)
     for _ in range(2):
         nat.convert_waveform(wav, wlen, g, g, tau=0.3, seed=1)
