@@ -25,12 +25,13 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 12 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 13 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
                                * 8: ovc_spectrogram_ring; 9: OVC_OPT_PAIR_OCC; 10: ovc_splice;
-                               * 11: ovc_tts_encode_state_rows, ovc_tts_state_rows; 12: OVC_OPT_STAGED_EPI */
+                               * 11: ovc_tts_encode_state_rows, ovc_tts_state_rows; 12: OVC_OPT_STAGED_EPI;
+                               * 13: ovc_resample_plan, ovc_resample_rings */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -264,6 +265,32 @@ OVC_API int ovc_resample(ovc_ctx* ctx, int sr_in, int sr_out, const float* in, c
  *   out4[1] = outputs whose input support lies inside the first n_in samples (what a stream can emit before it ends)
  *   out4[2], out4[3] = input samples [lo, hi) read by outputs [m0, m1) (m1 > m0; lo may be negative) */
 OVC_API int ovc_resample_span(int sr_in, int sr_out, int64_t n_in, int64_t m0, int64_t m1, int64_t* out4);
+
+/* Build (once per context) the filter bank of sr_in -> sr_out and return its plan id in *id, for ovc_resample_rings.
+ * The banks are those of ovc_resample (one per reduced pair, shared), and asking again for a pair returns the same id.
+ * Uploads and waits for `stream`: call it at set-up, never inside a step.  Refuses the rates ovc_resample refuses
+ * (OVC_ERR_INVALID). */
+OVC_API int ovc_resample_plan(ovc_ctx* ctx, int sr_in, int sr_out, int32_t* id, void* stream);
+
+/* ovc_resample for many live streams in one launch, each with its own plan: input from ring rows, output into ring
+ * rows or a packed buffer.  Item b < B computes outputs [m0[b], m0[b] + count[b]) of plan plan[b] (an id of
+ * ovc_resample_plan); it reads input sample j at in[in_row[b] * in_cap + j mod in_cap], zero outside [0, in_len[b])
+ * (in_len INT64_MAX: a stream that has not ended), and writes output m at
+ * out[out_row[b] * out_cap + (out_off[b] + m - m0[b]) mod out_cap].  out_off = m0 writes a ring row indexed by absolute
+ * sample; an out_cap past every item's end makes `out` a packed buffer.  Outputs at or past n_out(in_len[b]) are
+ * written as 0.
+ *   plan                                          [B] int32 (device)
+ *   in_row, in_len, m0, count, out_row, out_off   [B] int64 (device)
+ *   in [in_rows, in_cap], out [out_rows, out_cap] fp32 (device); max_count bounds every count (the launch's width)
+ * Every descriptor is clamped on the device, so nothing outside `in` and `out` is read or written whatever the arrays
+ * hold: the plan id and rows into range, in_len to >= 0, m0 into [0, 2^63 / 16384], count into [0, max_count], out_off
+ * mod out_cap.  Exactness: an output equals the whole-signal ovc_resample of the same stream bit for bit when its ring
+ * row still holds every input sample that ovc_resample_span says it reads (and no other item writes where it reads).
+ * Only enqueues on `stream` and takes stable pointers, so it can sit inside a captured graph. */
+OVC_API int ovc_resample_rings(ovc_ctx* ctx, const int32_t* plan, const float* in, int in_rows, int64_t in_cap,
+                               const int64_t* in_row, const int64_t* in_len, const int64_t* m0, const int64_t* count,
+                               float* out, int out_rows, int64_t out_cap, const int64_t* out_row, const int64_t* out_off,
+                               int B, int64_t max_count, void* stream);
 
 /* ---- V1 base-speaker TTS front half: SynthesizerTrn.infer (openvoice/models.py:467-490), SURVEY.md section 8 row f3 ----
  * Available when the checkpoint passed through ovc_load_tensor holds enc_p.* / dp.* / sdp.* / emb_g.* (a V1 base

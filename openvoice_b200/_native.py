@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 12
+ABI_VERSION = 13
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -23,7 +23,7 @@ EXPORTS = (
     "ovc_reference_encoder_ragged", "ovc_resample", "ovc_resample_span", "ovc_voice_conversion_items",
     "ovc_convert_waveform_items", "ovc_tts_encode_items", "ovc_tts_decode_items", "ovc_philox_normals",
     "ovc_tts_encode_state", "ovc_tts_decode_windows", "ovc_spectrogram_ring", "ovc_splice",
-    "ovc_tts_encode_state_rows", "ovc_tts_state_rows",
+    "ovc_tts_encode_state_rows", "ovc_tts_state_rows", "ovc_resample_plan", "ovc_resample_rings",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample / ovc_spectrogram_ring length of a stream that has not ended
@@ -158,6 +158,9 @@ def load_library(path: Optional[str] = None):
     lib.ovc_tts_encode_state_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 5
     lib.ovc_tts_state_rows.argtypes = ([C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
                                        + [C.c_void_p] * 5)
+    lib.ovc_resample_plan.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int32), C.c_void_p]
+    lib.ovc_resample_rings.argtypes = ([C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64] + [C.c_void_p] * 5
+                                       + [C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p])
     if lib.ovc_abi_version() != ABI_VERSION:
         raise OvcError(f"ABI mismatch: library {lib.ovc_abi_version()} vs binding {ABI_VERSION}")
     _lib = lib
@@ -455,6 +458,40 @@ class NativeConverter:
                                    C.c_void_p(in_lengths.data_ptr()), B, pitch, int(in_start), C.c_void_p(out.data_ptr()),
                                    int(out_pitch), int(out_start), C.c_void_p(st.cuda_stream))
         _check(self.lib, rc, "ovc_resample")
+        return out
+
+    def resample_plan(self, sr_in: int, sr_out: int, stream=None) -> int:
+        """Plan id of sr_in -> sr_out for ``resample_rings`` (include/ovc.h: ovc_resample_plan).  Builds the pair's filter
+        bank on first use and WAITS for the stream: call it at set-up.  ValueError for a pair the resampler refuses."""
+        import torch
+        dev = torch.device("cuda", self.device_index)
+        st = stream if stream is not None else torch.cuda.current_stream(dev)
+        out = C.c_int32(-1)
+        with torch.cuda.device(dev):
+            rc = self.lib.ovc_resample_plan(self.handle, int(sr_in), int(sr_out), C.byref(out), C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_resample_plan")
+        return int(out.value)
+
+    def resample_rings(self, plan, x, in_row, in_len, m0, count, out, out_row, out_off, max_count: int, stream=None):
+        """Many streams' resampling in one launch (include/ovc.h: ovc_resample_rings): item b computes outputs
+        [m0[b], m0[b] + count[b]) of plan[b], reading x[in_row[b], j % cap] (0 outside [0, in_len[b])) and writing output
+        m to out[out_row[b], (out_off[b] + m - m0[b]) % out_cap].  plan [B] int32, the rest [B] int64, all cuda; x and
+        out 2-D f32 cuda.  Asynchronous on `stream`; returns ``out``."""
+        import torch
+        for t in (x, out):
+            assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 2
+        B = plan.numel()
+        assert plan.is_cuda and plan.dtype == torch.int32 and plan.is_contiguous()
+        for t in (in_row, in_len, m0, count, out_row, out_off):
+            assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()
+            if t.numel() != B:
+                raise ValueError(f"resample_rings: per-item arrays need {B} values, got {t.numel()}")
+        st = stream if stream is not None else torch.cuda.current_stream(out.device)
+        p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+        rc = self.lib.ovc_resample_rings(self.handle, p(plan), p(x), int(x.shape[0]), int(x.shape[1]), p(in_row),
+                                         p(in_len), p(m0), p(count), p(out), int(out.shape[0]), int(out.shape[1]),
+                                         p(out_row), p(out_off), B, int(max_count), C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_resample_rings")
         return out
 
     def splice(self, src, seg, dst, pcm16: bool = False, stream=None):

@@ -218,6 +218,12 @@ struct ovc_ctx {
   // ovc_resample: one fp64 polyphase bank per reduced (up, down) pair, built on first use and kept
   std::map<std::pair<int64_t, int64_t>, double*> rs_banks;
   bool rs_smem_opt_in = false;   // resample_kernel's dynamic shared-memory limit raised (once per context)
+  // ovc_resample_plan: the plan table of ovc_resample_rings (banks shared with rs_banks), and the tile and shared memory
+  // that fit its worst plan
+  std::vector<RsRingPlan> rs_plans;
+  RsRingPlan* d_rs_plans = nullptr;
+  int rs_ring_tile = 256;
+  size_t rs_ring_smem = 0;
 
   // workspace
   float* d_ws = nullptr;
@@ -1443,6 +1449,7 @@ void ovc_destroy(ovc_ctx* c) {
   if (c->d_tcw) cudaFree(c->d_tcw);
   if (c->d_re) cudaFree(c->d_re);
   for (auto& kv : c->rs_banks) cudaFree(kv.second);
+  if (c->d_rs_plans) cudaFree(c->d_rs_plans);
   if (c->d_tw) cudaFree(c->d_tw);
   if (c->d_win) cudaFree(c->d_win);
   drop_graphs(c);
@@ -1681,6 +1688,28 @@ int ovc_resample_span(int sr_in, int sr_out, int64_t n_in, int64_t m0, int64_t m
   return OVC_OK;
 }
 
+static constexpr int64_t RS_SMEM_MAX = 200 * 1024;   // opt-in dynamic shared memory of the resample kernels
+
+// stage a tile of plan p as doubles when one output's span fits shared memory as doubles
+static bool resample_stage_dbl(const ovc_rs::Plan& p) {
+  return resample_stage_len(p, 1) * (int64_t)sizeof(double) <= RS_SMEM_MAX;
+}
+
+// the context's bank of p, built and uploaded on first use (waits for `stream`)
+static int resample_bank(ovc_ctx* c, const ovc_rs::Plan& p, double** out, cudaStream_t stream) {
+  double*& bank = c->rs_banks[{p.up, p.down}];
+  if (!bank) {
+    const std::vector<double> h = ovc_rs::design_bank(p);
+    CK(cudaMalloc(&bank, h.size() * sizeof(double)));
+    // ordered on the call's stream (a non-blocking stream does not wait for the legacy default stream) and finished
+    // before the pageable source goes out of scope
+    CK(cudaMemcpyAsync(bank, h.data(), h.size() * sizeof(double), cudaMemcpyHostToDevice, stream));
+    CK(cudaStreamSynchronize(stream));
+  }
+  *out = bank;
+  return OVC_OK;
+}
+
 int ovc_resample(ovc_ctx* c, int sr_in, int sr_out, const float* in, const int64_t* in_lengths, int B, int64_t in_pitch,
                  int64_t in_start, float* out, int64_t out_pitch, int64_t out_start, void* stream) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
@@ -1692,18 +1721,11 @@ int ovc_resample(ovc_ctx* c, int sr_in, int sr_out, const float* in, const int64
                 (long long)out_pitch, (long long)out_start);
   if (out_pitch == 0) return OVC_OK;
   ON_DEVICE(c);
-  double*& bank = c->rs_banks[{p.up, p.down}];
-  if (!bank) {
-    const std::vector<double> h = ovc_rs::design_bank(p);
-    CK(cudaMalloc(&bank, h.size() * sizeof(double)));
-    // ordered on the call's stream (a non-blocking stream does not wait for the legacy default stream) and finished
-    // before the pageable source goes out of scope
-    CK(cudaMemcpyAsync(bank, h.data(), h.size() * sizeof(double), cudaMemcpyHostToDevice, (cudaStream_t)stream));
-    CK(cudaStreamSynchronize((cudaStream_t)stream));
-  }
+  double* bank = nullptr;
+  TRY(resample_bank(c, p, &bank, (cudaStream_t)stream));
   // tile of up to 256 outputs whose staged span fits the opt-in shared memory; staged as doubles when one output's does
-  const int64_t smem_max = 200 * 1024;
-  const bool dbl = resample_stage_len(p, 1) * (int64_t)sizeof(double) <= smem_max;
+  const int64_t smem_max = RS_SMEM_MAX;
+  const bool dbl = resample_stage_dbl(p);
   const int64_t elem = dbl ? sizeof(double) : sizeof(float);
   int tile = 256;
   while (tile > 1 && resample_stage_len(p, tile) * elem > smem_max) tile /= 2;
@@ -1725,6 +1747,82 @@ int ovc_resample(ovc_ctx* c, int sr_in, int sr_out, const float* in, const int64
     resample_kernel<float><<<grid, threads, smem, st>>>(p, bank, in, in_pitch, in_start, (const int64_t*)in_lengths, out,
                                                         out_pitch, out_start, tile);
   }
+  CK(cudaGetLastError());
+  return OVC_OK;
+}
+
+int ovc_resample_plan(ovc_ctx* c, int sr_in, int sr_out, int32_t* id, void* stream) {
+  if (!c || !id) return fail(OVC_ERR_INVALID, "null argument to ovc_resample_plan");
+  ovc_rs::Plan p;
+  TRY(resample_plan(sr_in, sr_out, &p));
+  for (size_t i = 0; i < c->rs_plans.size(); ++i)
+    if (c->rs_plans[i].p.up == p.up && c->rs_plans[i].p.down == p.down) {
+      *id = (int32_t)i;
+      return OVC_OK;
+    }
+  ON_DEVICE(c);
+  cudaStream_t st = (cudaStream_t)stream;
+  RsRingPlan e;
+  e.p = p;
+  double* bank = nullptr;
+  TRY(resample_bank(c, p, &bank, st));
+  e.bank = bank;
+  e.dbl = resample_stage_dbl(p) ? 1 : 0;
+  std::vector<RsRingPlan> plans = c->rs_plans;
+  plans.push_back(e);
+  // one tile for every plan of the table: the largest (up to 256) whose staged span fits each plan's staging type
+  auto bytes = [](const RsRingPlan& q, int tile) {
+    return resample_stage_len(q.p, tile) * (int64_t)(q.dbl ? sizeof(double) : sizeof(float));
+  };
+  int tile = 256;
+  for (;;) {
+    bool fits = true;
+    for (const RsRingPlan& q : plans) fits = fits && bytes(q, tile) <= RS_SMEM_MAX;
+    if (fits || tile == 1) break;
+    tile /= 2;
+  }
+  int64_t smem = 0;
+  for (const RsRingPlan& q : plans) smem = std::max(smem, bytes(q, tile));
+  RsRingPlan* table = nullptr;
+  CK(cudaMalloc(&table, plans.size() * sizeof(RsRingPlan)));
+  const cudaError_t up = cudaMemcpyAsync(table, plans.data(), plans.size() * sizeof(RsRingPlan), cudaMemcpyHostToDevice, st);
+  const cudaError_t done = up == cudaSuccess ? cudaStreamSynchronize(st) : up;
+  if (done != cudaSuccess) {
+    cudaFree(table);
+    return fail(OVC_ERR_CUDA, "ovc_resample_plan: %s", cudaGetErrorString(done));
+  }
+  CK(cudaFuncSetAttribute(resample_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RS_SMEM_MAX));
+  if (c->d_rs_plans) CK(cudaFree(c->d_rs_plans));   // synchronises the device: no launch still reads the old table
+  c->d_rs_plans = table;
+  c->rs_plans = plans;
+  c->rs_ring_tile = tile;
+  c->rs_ring_smem = (size_t)smem;
+  *id = (int32_t)(plans.size() - 1);
+  return OVC_OK;
+}
+
+int ovc_resample_rings(ovc_ctx* c, const int32_t* plan, const float* in, int in_rows, int64_t in_cap,
+                       const int64_t* in_row, const int64_t* in_len, const int64_t* m0, const int64_t* count, float* out,
+                       int out_rows, int64_t out_cap, const int64_t* out_row, const int64_t* out_off, int B,
+                       int64_t max_count, void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (c->rs_plans.empty()) return fail(OVC_ERR_STATE, "ovc_resample_rings: no plan has been built (ovc_resample_plan)");
+  if (B < 0 || B > 65535 || max_count < 0 || max_count > 0x7fffffffLL)
+    return fail(OVC_ERR_INVALID, "ovc_resample_rings: bad sizes B=%d max_count=%lld", B, (long long)max_count);
+  if (in_rows < 1 || in_cap < 1 || out_rows < 1 || out_cap < 1 || in_cap > (INT64_MAX / 4) / in_rows ||
+      out_cap > (INT64_MAX / 4) / out_rows)
+    return fail(OVC_ERR_INVALID, "ovc_resample_rings: bad rings (in %d x %lld, out %d x %lld)", in_rows,
+                (long long)in_cap, out_rows, (long long)out_cap);
+  if (B == 0 || max_count == 0) return OVC_OK;
+  if (!plan || !in || !in_row || !in_len || !m0 || !count || !out || !out_row || !out_off)
+    return fail(OVC_ERR_INVALID, "null tensor argument");
+  ON_DEVICE(c);
+  const int tile = c->rs_ring_tile;
+  const dim3 grid((unsigned)((max_count + tile - 1) / tile), B);
+  const int threads = std::min(256, (tile + 31) / 32 * 32);
+  resample_ring_kernel<<<grid, threads, c->rs_ring_smem, (cudaStream_t)stream>>>(
+      c->d_rs_plans, (int)c->rs_plans.size(), plan, in, in_rows, in_cap, in_row, in_len, m0, count, out, out_rows,
+      out_cap, out_row, out_off, max_count, tile);
   CK(cudaGetLastError());
   return OVC_OK;
 }

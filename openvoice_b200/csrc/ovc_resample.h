@@ -107,6 +107,57 @@ OVC_HD double output_at(const Plan& p, const double* bank, const T* x, int64_t x
   return acc;
 }
 
+// ---- ovc_resample_rings: many streams, each with its own plan, read from ring rows and written to ring rows or packed
+// buffers.  Every descriptor is clamped here, on the device, so that no index leaves `in` or `out` whatever the arrays
+// hold; the same functions run in tests/hostcheck.
+
+// first output a ring item may start at: keeps t_of(m) and the span arithmetic far from int64 overflow
+constexpr int64_t MAX_POS = OPEN / (8 * MAX_M);
+
+OVC_HD int64_t clamp64(int64_t v, int64_t lo, int64_t hi) { return v < lo ? lo : (v > hi ? hi : v); }
+
+// v mod cap in [0, cap), cap > 0
+OVC_HD int64_t wrap(int64_t v, int64_t cap) {
+  const int64_t r = v % cap;
+  return r < 0 ? r + cap : r;
+}
+
+// flat index of absolute sample s of a ring row: row * cap + s mod cap
+OVC_HD int64_t ring_at(int64_t row, int64_t s, int64_t cap) { return row * cap + wrap(s, cap); }
+
+struct RingItem {
+  int plan;                     // plan id in [0, n_plans)
+  int64_t in_row, in_len;       // input ring row and stream length (OPEN while the stream is open)
+  int64_t m0, count;            // outputs [m0, m0 + count)
+  int64_t out_row, out_off;     // output m goes to out[out_row * out_cap + (out_off + m - m0) mod out_cap]
+};
+
+// the clamped descriptor of one item: plan and rows into range, in_len >= 0, m0 into [0, MAX_POS], count into
+// [0, max_count], out_off reduced mod out_cap (n_plans, in_rows, out_rows, out_cap >= 1; max_count >= 0)
+OVC_HD RingItem ring_item(int64_t plan, int64_t in_row, int64_t in_len, int64_t m0, int64_t count, int64_t out_row,
+                          int64_t out_off, int n_plans, int64_t in_rows, int64_t out_rows, int64_t out_cap,
+                          int64_t max_count) {
+  RingItem it;
+  it.plan = (int)clamp64(plan, 0, n_plans - 1);
+  it.in_row = clamp64(in_row, 0, in_rows - 1);
+  it.in_len = in_len > 0 ? in_len : 0;
+  it.m0 = clamp64(m0, 0, MAX_POS);
+  it.count = clamp64(count, 0, max_count);
+  it.out_row = clamp64(out_row, 0, out_rows - 1);
+  it.out_off = wrap(out_off, out_cap);
+  return it;
+}
+
+// flat index into `in` of input sample j of the item, or -1 when it reads as 0 (outside [0, in_len))
+OVC_HD int64_t ring_in_at(const RingItem& it, int64_t j, int64_t in_cap) {
+  return (j >= 0 && j < it.in_len) ? ring_at(it.in_row, j, in_cap) : -1;
+}
+
+// flat index into `out` of the item's i-th output (m = m0 + i), 0 <= i < count
+OVC_HD int64_t ring_out_at(const RingItem& it, int64_t i, int64_t out_cap) {
+  return ring_at(it.out_row, it.out_off + i, out_cap);
+}
+
 // modified Bessel function I0 by its power series sum (x^2 / 4)^k / (k!)^2
 inline double bessel_i0(double x) {
   const double q = 0.25 * x * x;

@@ -291,12 +291,15 @@ SESSION_BATCH_FRAMES = 32768
 
 
 class _Session:
-    __slots__ = ("row", "seed", "tau", "n_in", "emitted")
+    __slots__ = ("row", "seed", "tau", "n_in", "emitted", "in_sr", "out_sr", "raw_n", "out_n")
 
-    def __init__(self, row: int, seed: int, tau: float):
+    def __init__(self, row: int, seed: int, tau: float, in_sr: Optional[int] = None, out_sr: Optional[int] = None):
         self.row, self.seed, self.tau = row, seed, tau
-        self.n_in = 0                                     # samples received
+        self.n_in = 0                                     # samples received (at the model's rate)
         self.emitted = 0                                  # frames whose samples have been returned
+        self.in_sr, self.out_sr = in_sr, out_sr           # rates of the pushed / returned audio; None: the model's
+        self.raw_n = 0                                    # samples received at in_sr
+        self.out_n = 0                                    # samples returned at out_sr
 
 
 class StreamingSessions:
@@ -316,16 +319,37 @@ class StreamingSessions:
     lockstep step replays its CUDA graph.  A session keeps the audio of its next window and both halos, plus the STFT
     support and its largest push, on the device.
 
-    Noise is drawn in-kernel from each session's seed (no ``noise_fn``); audio is at the model's rate (use
-    ``StreamingConverter`` with ``input_sr`` / ``output_sr`` to resample a single stream)."""
+    Sessions may push and receive audio at other rates than the model's: ``rates`` declares them up front (the
+    constructor builds each rate's two filter banks, which waits for the device), and ``open(input_sr=, output_sr=)``
+    takes any declared rate.  Such a session equals ``StreamingConverter(..., input_sr=, output_sr=)`` bit for bit.  Its
+    pushed samples go into a raw ring row (a second ``ovc_splice``), and ONE ``ovc_resample_rings`` over every such
+    session of the step writes their new model-rate samples into their ring rows; on the way out, the emitted frames are
+    spliced into an output ring row (a third splice) and ONE more ``ovc_resample_rings`` writes every such session's new
+    samples at its rate into the buffer the frames are gathered into, so the step still has one download.  A step that
+    names a resampling session thus has at most four more launches, however many it names; one that names none runs
+    exactly the launches above.  The raw ring keeps the input the next model-rate sample reads plus the largest push,
+    the output ring the model-rate samples the next output sample reads.
 
-    def __init__(self, converter, window_frames: int = 256):
+    Noise is drawn in-kernel from each session's seed (no ``noise_fn``)."""
+
+    def __init__(self, converter, window_frames: int = 256, rates: Iterable[int] = ()):
+        """``rates``: the rates other than the model's that ``open`` will accept for ``input_sr`` / ``output_sr``.
+        ValueError for a rate that is not a positive integer or that the resampler refuses, before anything is built."""
         W = int(window_frames)
         if W < 1:
             raise ValueError(f"window_frames must be >= 1, got {window_frames!r}")
         hp = converter.hps
         self.native = converter.model.native
         self.sr = int(hp.data.sampling_rate)
+        declared = []
+        for r in rates:
+            if isinstance(r, bool) or int(r) != r or int(r) <= 0:
+                raise ValueError(f"rates: {r!r} is not a positive integer rate")
+            r = int(r)
+            resample_span(r, self.sr)                     # ValueError for a pair the resampler refuses
+            resample_span(self.sr, r)
+            declared.append(r)
+        self.rates = tuple(sorted(set(declared)))
         self.hop = hp.data.hop_length
         self.nfft = hp.data.filter_length
         self.pad = (self.nfft - self.hop) // 2
@@ -344,18 +368,36 @@ class StreamingSessions:
         self.next_id = 0
         self._bufs: dict = {}
         self._h2d_done = None
+        # resampling: plan ids of rate -> model and model -> rate, raw input rings and output rings (row = session row)
+        self.plans: Dict[Tuple[int, int], int] = {}
+        for r in self.rates:
+            if r != self.sr:
+                self.plans[(r, self.sr)] = self.native.resample_plan(r, self.sr)
+                self.plans[(self.sr, r)] = self.native.resample_plan(self.sr, r)
+        self.raw = self.orings = None
+        if self.plans:                                    # both grow with the largest push / emitted run
+            span1 = max(resample_span(a, b, 0, 0, 1)[3] - resample_span(a, b, 0, 0, 1)[2] for a, b in self.plans)
+            extra = -(-(span1 + 8192) // 1024) * 1024
+            self.raw = torch.zeros(self.rows, extra, device=self.dev)
+            self.orings = torch.zeros(self.rows, self.hop * (W + 8) + extra, device=self.dev)
 
     # ------------------------------------------------------------------ sessions
     def open(self, src_se, tgt_se, tau: float = 0.3, seed: Optional[int] = None, input_sr: Optional[int] = None,
              output_sr: Optional[int] = None) -> int:
         """Start a session converting from ``src_se`` to ``tgt_se`` (tone-colour embeddings of ``gin`` values each) and
         return its id.  ``seed``: the session's Philox key in [0, 2^64) (default: drawn from torch's generator).
-        ``input_sr`` / ``output_sr`` other than the model's rate are refused."""
+        ``input_sr`` / ``output_sr``: rates of the pushed and of the returned audio, the model's or one declared with
+        ``rates`` (None: the model's); any other rate is refused."""
         from .api import check_seeds
+        sr = {}
         for name, rate in (("input_sr", input_sr), ("output_sr", output_sr)):
-            if rate is not None and int(rate) != self.sr:
-                raise ValueError(f"{name}={rate}: StreamingSessions takes and returns audio at the model's rate "
-                                 f"({self.sr} Hz); StreamingConverter resamples a single stream")
+            ok = rate is None or (not isinstance(rate, bool) and int(rate) == rate
+                                  and (int(rate) == self.sr or int(rate) in self.rates))
+            if not ok:
+                raise ValueError(f"{name}={rate!r}: StreamingSessions takes and returns audio at the model's rate "
+                                 f"({self.sr} Hz) or at a rate declared with rates= (declared: "
+                                 f"{', '.join(map(str, self.rates)) or 'none'})")
+            sr[name] = None if rate is None or int(rate) == self.sr else int(rate)
         tau = float(tau)
         if not math.isfinite(tau):
             raise ValueError(f"tau = {tau!r} is not a finite number")
@@ -375,7 +417,7 @@ class StreamingSessions:
         self.se[:, row] = torch.stack(ses).to(self.dev)
         sid = self.next_id
         self.next_id += 1
-        self.sessions[sid] = _Session(row, seed, tau)
+        self.sessions[sid] = _Session(row, seed, tau, sr["input_sr"], sr["output_sr"])
         return sid
 
     @property
@@ -387,9 +429,31 @@ class StreamingSessions:
         s = self.sessions[sid]
         return s.n_in - self._keep_from(s)
 
+    def raw_state_samples(self, sid: int) -> int:
+        """Samples at its input rate that session ``sid`` holds in its raw ring row (0 without ``input_sr``)."""
+        s = self.sessions[sid]
+        return 0 if s.in_sr is None else s.raw_n - self._raw_keep(s)
+
+    def out_state_samples(self, sid: int) -> int:
+        """Model-rate samples that session ``sid`` holds in its output ring row (0 without ``output_sr``)."""
+        s = self.sessions[sid]
+        return 0 if s.out_sr is None else s.emitted * self.hop - self._out_keep(s)
+
     def _keep_from(self, s: _Session) -> int:
         """First sample of the session's next window: frame max(0, emitted - H) reads from (that frame) * hop - pad."""
         return max(0, (s.emitted - self.H) * self.hop - self.pad)
+
+    def _raw_keep(self, s: _Session) -> int:
+        """First raw sample that the session's next model-rate sample reads."""
+        return max(0, resample_span(s.in_sr, self.sr, 0, s.n_in, s.n_in + 1)[2])
+
+    def _out_keep(self, s: _Session) -> int:
+        """First model-rate sample that the session's next output sample reads."""
+        return max(0, resample_span(self.sr, s.out_sr, 0, s.out_n, s.out_n + 1)[2])
+
+    def _model_len(self, s: _Session, n: int) -> int:
+        """Model-rate length of session ``s`` once ``n`` more samples at its input rate end it."""
+        return s.n_in + n if s.in_sr is None else resample_span(s.in_sr, self.sr, s.raw_n + n)[0]
 
     def _check_ids(self, ids) -> List[int]:
         ids = list(ids)
@@ -403,8 +467,8 @@ class StreamingSessions:
     # ------------------------------------------------------------------ public steps
     @torch.no_grad()
     def push(self, chunks: Dict[int, object]) -> Dict[int, np.ndarray]:
-        """Append ``chunks[id]`` (float32 samples at the model's rate) to each named session; returns, per named session,
-        the converted samples that became final (possibly none)."""
+        """Append ``chunks[id]`` (float32 samples at the session's input rate) to each named session; returns, per named
+        session, the converted samples that became final (possibly none), at its output rate."""
         ids = self._check_ids(chunks.keys())
         xs = {sid: np.asarray(chunks[sid], dtype=np.float32).reshape(-1) for sid in ids}
         return self._step(xs, final=set())
@@ -413,7 +477,8 @@ class StreamingSessions:
     def push_device(self, runs: Dict[int, Sequence[Tuple[int, int, int]]], src: torch.Tensor,
                     close: Iterable[int] = ()) -> Dict[int, np.ndarray]:
         """``push`` of audio already on the device: appends to each named session, in order, the runs
-        ``(src_row, src_off, count)`` of ``src`` ([rows, pitch] float32 on the converter's device): samples
+        ``(src_row, src_off, count)`` of ``src`` ([rows, pitch] float32 on the converter's device, at the session's
+        input rate): samples
         src[src_row, src_off : src_off + count], or ``count`` zeros when src_row < 0.  The runs of every session go into
         the rings in ONE ``ovc_splice``; nothing is uploaded but the step's small tables.  The sessions named in
         ``close`` (each also in ``runs``) then end as ``close`` ends them, in the same step.  Returns what ``push`` and
@@ -431,7 +496,7 @@ class StreamingSessions:
                 if n < 0 or (r >= 0 and (r >= rows or o < 0 or o + n > pitch)):
                     raise ValueError(f"session {sid}: run {(r, o, n)} is not inside src {tuple(src.shape)}")
         for sid in close:
-            check_stream_length(self.sessions[sid].n_in + sum(n for _, _, n in xs[sid]), self.hop, self.pad)
+            check_stream_length(self._model_len(self.sessions[sid], sum(n for _, _, n in xs[sid])), self.hop, self.pad)
         out = self._step(xs, final=close, src=src)
         for sid in close:
             self.free_rows.append(self.sessions.pop(sid).row)
@@ -444,7 +509,7 @@ class StreamingSessions:
         like ``StreamingConverter.flush``; nothing is changed then."""
         ids = self._check_ids(ids)
         for sid in ids:
-            check_stream_length(self.sessions[sid].n_in, self.hop, self.pad)
+            check_stream_length(self._model_len(self.sessions[sid], 0), self.hop, self.pad)
         out = self._step({sid: np.zeros(0, dtype=np.float32) for sid in ids}, final=set(ids))
         for sid in ids:
             self.free_rows.append(self.sessions.pop(sid).row)
@@ -466,25 +531,48 @@ class StreamingSessions:
             self._bufs[name] = b
         return b[:numel]
 
-    def _grow(self, rows: int, cap: int, live: List[Tuple[int, int, int]]):
-        """Reallocate the rings as [rows, cap] (and the embedding table as [2, rows, gin]), moving each live session's
-        samples [a, b) of row r (``live``: (r, a, b)) to their places under the new capacity."""
-        rings = torch.zeros(rows, cap, device=self.dev)
+    def _moved(self, old: torch.Tensor, rows: int, cap: int, live: List[Tuple[int, int, int]]) -> torch.Tensor:
+        """``old`` reallocated as [rows, cap]: each live session's samples [a, b) of row r (``live``: (r, a, b)) moved to
+        their places under the new capacity, or, without ``live``, the old rows copied as they are."""
+        new = torch.zeros(rows, cap, device=self.dev)
         if live:
-            src = np.concatenate([r * self.cap + np.arange(a, b) % self.cap for r, a, b in live])
+            oc = old.shape[1]
+            src = np.concatenate([r * oc + np.arange(a, b) % oc for r, a, b in live])
             dst = np.concatenate([r * cap + np.arange(a, b) % cap for r, a, b in live])
-            rings.view(-1)[torch.from_numpy(dst).to(self.dev)] = self.rings.reshape(-1)[torch.from_numpy(src).to(self.dev)]
+            new.view(-1)[torch.from_numpy(dst).to(self.dev)] = old.reshape(-1)[torch.from_numpy(src).to(self.dev)]
         else:
-            rings[: self.rows] = self.rings
+            new[: old.shape[0]] = old
+        return new
+
+    def _grow(self, rows: int, cap: int, live: List[Tuple[int, int, int]]):
+        """Reallocate the rings as [rows, cap] (and the embedding table as [2, rows, gin], the raw and output rings as
+        [rows, their capacity]), moving each live session's samples [a, b) of row r (``live``: (r, a, b)) to their
+        places under the new capacity."""
+        rings = self._moved(self.rings, rows, cap, live)
         se = torch.zeros(2, rows, self.gin, device=self.dev)
         se[:, : self.rows] = self.se
+        if self.raw is not None and rows != self.rows:
+            self.raw = self._moved(self.raw, rows, self.raw.shape[1], [])
+            self.orings = self._moved(self.orings, rows, self.orings.shape[1], [])
         self.rings, self.se, self.rows, self.cap = rings, se, rows, cap
+
+    def _splice(self, source: torch.Tensor, seg: torch.Tensor, segs: List[Tuple[int, int, int, int, int]],
+                dst: torch.Tensor):
+        """``ovc_splice`` of ``segs`` (on the device as ``seg``) from ``source`` into the ring array ``dst``."""
+        if self.cuda:
+            self.native.splice(source, seg, dst)
+        else:   # only the CPU stand-in converters of the host tests get here: the same writes as one index_copy_
+            cap = dst.shape[1]
+            at = np.concatenate([r * cap + np.arange(a, a + n) % cap for _, _, n, r, a in segs])
+            val = torch.cat([source[row, off:off + n] if row >= 0 else torch.zeros(n) for row, off, n, _, _ in segs])
+            dst.view(-1).index_copy_(0, torch.from_numpy(at), val)
 
     # ------------------------------------------------------------------ one step
     def _step(self, xs: Dict[int, object], final: Set[int], src: Optional[torch.Tensor] = None) -> Dict[int, np.ndarray]:
         """One step over the sessions of ``xs``: xs[sid] is the session's new host samples, or with ``src`` its runs
-        (src_row, src_off, count) of that device array; the sessions in ``final`` end after them."""
-        hop, H = self.hop, self.H
+        (src_row, src_off, count) of that device array, at the session's input rate; the sessions in ``final`` end after
+        them."""
+        hop, H, sr = self.hop, self.H, self.sr
         ses = [(sid, self.sessions[sid], xs[sid]) for sid in xs]
         if src is None:                                   # host samples: the upload's sample block is the one source row
             counts = [len(x) for _, _, x in ses]
@@ -493,30 +581,81 @@ class StreamingSessions:
         else:
             runs = [x for _, _, x in ses]
             counts = [sum(n for _, _, n in r) for r in runs]
-        need = max([s.n_in + n - self._keep_from(s) for (_, s, _), n in zip(ses, counts)], default=0)
+        # model-rate samples each session gains: its pushed samples, or the outputs of its input resampler that become
+        # ready (all of them once it ends); rin: (plan, row, in_len, m0, count, row, m0) of the ring resampling
+        gains, rin = [], []
+        for (sid, s, _), n in zip(ses, counts):
+            if s.in_sr is None:
+                gains.append(n)
+                continue
+            n_out, n_ready = resample_span(s.in_sr, sr, s.raw_n + n)[:2]
+            m1 = n_out if sid in final else n_ready
+            gains.append(m1 - s.n_in)
+            if m1 > s.n_in:
+                rin.append((self.plans[(s.in_sr, sr)], s.row, s.raw_n + n if sid in final else STREAM_OPEN, s.n_in,
+                            m1 - s.n_in, s.row, s.n_in))
+        need = max([s.n_in + n - self._keep_from(s) for (_, s, _), n in zip(ses, gains)], default=0)
         if need > self.cap:
             cap = -(-int(need * 1.25) // hop) * hop
             self._grow(self.rows, cap, [(s.row, self._keep_from(s), s.n_in) for s in self.sessions.values()])
+        need = max([s.raw_n + n - self._raw_keep(s) for (_, s, _), n in zip(ses, counts) if s.in_sr], default=0)
+        if self.raw is not None and need > self.raw.shape[1]:
+            live = [(s.row, self._raw_keep(s), s.raw_n) for s in self.sessions.values() if s.in_sr]
+            self.raw = self._moved(self.raw, self.rows, -(-int(need * 1.25) // 1024) * 1024, live)
         # windows of every named session: (session index, lo, hi, e0, e1)
         wins = []
-        for i, ((sid, s, _), n) in enumerate(zip(ses, counts)):
+        for i, ((sid, s, _), n) in enumerate(zip(ses, gains)):
             have = ready_frames(s.n_in + n, hop, self.nfft, sid in final)
             wins += [(i,) + w for w in stream_windows(s.emitted, have, self.W, H, sid in final)]
-        # splice segments: each run to the ring row of its session, at the session's next sample positions
-        segs = []
+        # splice segments: each run to the ring row (raw ring row when the session resamples its input) of its session,
+        # at the session's next sample positions
+        segs, rsegs = [], []
         for (_, s, _), r in zip(ses, runs):
-            at = s.n_in
+            at, dst = (s.n_in, segs) if s.in_sr is None else (s.raw_n, rsegs)
             for row, off, n in r:
                 if n:
-                    segs.append((row, off, n, s.row, at))
+                    dst.append((row, off, n, s.row, at))
                     at += n
-        B, nS, Ns = len(wins), len(segs), (sum(counts) if src is None else 0)
+        B, nS, nR, Ns = len(wins), len(segs), len(rsegs), (sum(counts) if src is None else 0)
         Tmax = -(-max([hi - lo for _, lo, hi, _, _ in wins], default=1) // 16) * 16
         Nf = sum(e1 - e0 for _, _, _, e0, e1 in wins)
+        # output side: the emitted frames of output-resampling sessions go to their output ring rows (osegs: splice
+        # from the gathered frames) and their new output-rate samples are packed after the frames (rout, qn)
+        emitted = [max([e1 for j, _, _, _, e1 in wins if j == i], default=s.emitted) for i, (_, s, _) in enumerate(ses)]
+        osegs, at = [], 0
+        for i, _, _, e0, e1 in wins:
+            if ses[i][1].out_sr is not None:
+                osegs.append((0, at * hop, (e1 - e0) * hop, ses[i][1].row, e0 * hop))
+            at += e1 - e0
+        rout, qn, No = [], [0] * len(ses), 0
+        for i, (sid, s, _) in enumerate(ses):
+            if s.out_sr is None:
+                continue
+            M = emitted[i] * hop
+            n_out, n_ready = resample_span(sr, s.out_sr, M)[:2]
+            qn[i] = (n_out if sid in final else n_ready) - s.out_n
+            if qn[i] > 0:
+                rout.append((self.plans[(sr, s.out_sr)], s.row, M if sid in final else STREAM_OPEN, s.out_n, qn[i], 0,
+                             Nf * hop + No))
+                No += qn[i]
+        if self.orings is not None:
+            need = max([emitted[i] * hop - self._out_keep(s) for i, (_, s, _) in enumerate(ses) if s.out_sr], default=0)
+            if need > self.orings.shape[1]:
+                live = [(s.row, self._out_keep(s), s.emitted * hop) for s in self.sessions.values() if s.out_sr]
+                self.orings = self._moved(self.orings, self.rows, -(-int(need * 1.25) // 1024) * 1024, live)
+        nO, nI, nQ = len(osegs), len(rin), len(rout)
         # packed upload (int64 words): row, lo, frames, stream length, seed, stream (0), embedding rows (2B), tau (float32),
-        # then the emitted frames' rows of the output, the splice segments (5 words each) and the pushed samples (float32)
+        # then the emitted frames' rows of the output, the splice segments (5 words each), the raw splice segments, the
+        # input resampling items (6 words each, then their plans as int32), the output splice segments, the output
+        # resampling items and the pushed samples (float32)
         nt = (B + 1) // 2
-        n_words = 8 * B + nt + Nf + 5 * nS + (Ns + 1) // 2
+        o = 8 * B + nt + Nf
+        o_r = o + 5 * nS
+        o_i = o_r + 5 * nR
+        o_o = o_i + 6 * nI + (nI + 1) // 2
+        o_q = o_o + 5 * nO
+        o_s = o_q + 6 * nQ + (nQ + 1) // 2
+        n_words = o_s + (Ns + 1) // 2
         if self._h2d_done is not None:
             self._h2d_done.synchronize()                  # the previous step's upload has left the pinned buffer
         pin = self._buf("pin", n_words, torch.int64, pinned=True)
@@ -526,32 +665,37 @@ class StreamingSessions:
             rows = np.asarray([s.row for _, s, _ in ses], dtype=np.int64)[ii]
             lo = np.asarray([v[1] for v in wins], dtype=np.int64)
             w[0:B], w[B:2 * B], w[2 * B:3 * B] = rows, lo, [hi - l for _, l, hi, _, _ in wins]
-            w[3 * B:4 * B] = [ses[i][1].n_in + counts[i] if ses[i][0] in final else STREAM_OPEN for i in ii]
+            w[3 * B:4 * B] = [ses[i][1].n_in + gains[i] if ses[i][0] in final else STREAM_OPEN for i in ii]
             from .api import seed_array
             w[4 * B:5 * B] = seed_array([ses[i][1].seed for i in ii])
             w[5 * B:6 * B] = 0
             w[6 * B:7 * B], w[7 * B:8 * B] = rows, rows + self.rows
             w[8 * B:8 * B + nt].view(np.float32)[:B] = [ses[i][1].tau for i in ii]
-            o = 8 * B + nt
-            w[o:o + Nf] = np.concatenate([b * Tmax + np.arange(e0 - l, e1 - l) for b, (_, l, _, e0, e1) in enumerate(wins)])
-        o = 8 * B + nt + Nf
-        if nS:
-            w[o:o + 5 * nS] = np.asarray(segs, dtype=np.int64).reshape(-1)
+            w[8 * B + nt:o] = np.concatenate([b * Tmax + np.arange(e0 - l, e1 - l)
+                                              for b, (_, l, _, e0, e1) in enumerate(wins)])
+        for at, sg in ((o, segs), (o_r, rsegs), (o_o, osegs)):
+            if sg:
+                w[at:at + 5 * len(sg)] = np.asarray(sg, dtype=np.int64).reshape(-1)
+        for at, it in ((o_i, rin), (o_q, rout)):
+            if it:
+                v = np.asarray(it, dtype=np.int64)
+                w[at:at + 6 * len(it)] = v[:, 1:].T.reshape(-1)
+                w[at + 6 * len(it):at + 6 * len(it) + (len(it) + 1) // 2].view(np.int32)[:len(it)] = v[:, 0]
         if Ns:
-            w[o + 5 * nS:].view(np.float32)[:Ns] = np.concatenate([x for _, _, x in ses])
+            w[o_s:].view(np.float32)[:Ns] = np.concatenate([x for _, _, x in ses])
         d = self._buf("up", n_words, torch.int64)
         d.copy_(pin, non_blocking=True)
         if self.cuda:
             self._h2d_done = torch.cuda.Event()
             self._h2d_done.record(torch.cuda.current_stream(self.dev))
+        if nS or nR:
+            source = d[o_s:].view(torch.float32)[:Ns].view(1, Ns) if src is None else src
         if nS:
-            source = d[o + 5 * nS:].view(torch.float32)[:Ns].view(1, Ns) if src is None else src
-            if self.cuda:
-                self.native.splice(source, d[o:o + 5 * nS].view(nS, 5), self.rings)
-            else:   # only the CPU stand-in converters of the host tests get here: the same writes as one index_copy_
-                at = np.concatenate([r * self.cap + np.arange(a, a + n) % self.cap for _, _, n, r, a in segs])
-                val = torch.cat([source[row, off:off + n] if row >= 0 else torch.zeros(n) for row, off, n, _, _ in segs])
-                self.rings.view(-1).index_copy_(0, torch.from_numpy(at), val)
+            self._splice(source, d[o:o + 5 * nS].view(nS, 5), segs, self.rings)
+        if nR:
+            self._splice(source, d[o_r:o_r + 5 * nR].view(nR, 5), rsegs, self.raw)
+        if nI:
+            self._resample_rings(d, o_i, nI, self.raw, self.rings, max(it[4] for it in rin))
         res = {sid: np.zeros(0, dtype=np.float32) for sid, _, _ in ses}
         if B:
             spec = self._buf("spec", B * self.S * Tmax, torch.float32).view(B, self.S, Tmax)
@@ -569,30 +713,48 @@ class StreamingSessions:
                                              ragged=True, latents=False, items=items,
                                              out=obuf[b0 * Tmax * hop:b1 * Tmax * hop])
             fo = 8 * B + nt
-            y = torch.index_select(obuf.view(B * Tmax, hop), 0, d[fo:fo + Nf],
-                                   out=self._buf("y", Nf * hop, torch.float32).view(Nf, hop))
-            host = self._buf("host", Nf * hop, torch.float32, pinned=True)
-            host.copy_(y.view(-1), non_blocking=True)
+            ybuf = self._buf("y", Nf * hop + No, torch.float32)
+            y = torch.index_select(obuf.view(B * Tmax, hop), 0, d[fo:fo + Nf], out=ybuf[:Nf * hop].view(Nf, hop))
+            if nO:
+                self._splice(y.view(1, Nf * hop), d[o_o:o_o + 5 * nO].view(nO, 5), osegs, self.orings)
+            if nQ:
+                self._resample_rings(d, o_q, nQ, self.orings, ybuf.view(1, -1), max(it[4] for it in rout))
+            host = self._buf("host", Nf * hop + No, torch.float32, pinned=True)
+            host.copy_(ybuf, non_blocking=True)
             if self.cuda:
                 torch.cuda.current_stream(self.dev).synchronize()
             y = host.numpy()
             at, per_ses = 0, {}
             for i, _, _, e0, e1 in wins:
-                per_ses.setdefault(i, []).append(y[at * hop:(at + e1 - e0) * hop])
+                if ses[i][1].out_sr is None:
+                    per_ses.setdefault(i, []).append(y[at * hop:(at + e1 - e0) * hop])
                 at += e1 - e0
             for i, parts in per_ses.items():
                 res[ses[i][0]] = np.concatenate(parts)
+            at = Nf * hop
+            for i, (sid, s, _) in enumerate(ses):
+                if qn[i] > 0:
+                    res[sid] = y[at:at + qn[i]].copy()
+                    at += qn[i]
         for i, (_, s, _) in enumerate(ses):
-            s.n_in += counts[i]
-            s.emitted = max([e1 for j, _, _, _, e1 in wins if j == i], default=s.emitted)
+            s.n_in += gains[i]
+            s.raw_n += counts[i] if s.in_sr is not None else 0
+            s.out_n += qn[i]
+            s.emitted = emitted[i]
         return res
+
+    def _resample_rings(self, d: torch.Tensor, at: int, n: int, src: torch.Tensor, dst: torch.Tensor, max_count: int):
+        """One ``ovc_resample_rings`` over the n items packed at word ``at`` of the step's upload ``d``."""
+        v = [d[at + k * n:at + (k + 1) * n] for k in range(6)]
+        plan = d[at + 6 * n:at + 6 * n + (n + 1) // 2].view(torch.int32)[:n]
+        self.native.resample_rings(plan, src, v[0], v[1], v[2], v[3], dst, v[4], v[5], max_count)
 
 
 class _CloneSession:
-    __slots__ = ("tts_keys", "conv_keys", "said", "unencoded", "plans", "length", "ended", "checked", "ss_id")
+    __slots__ = ("tts_keys", "conv_keys", "said", "unencoded", "plans", "length", "ended", "checked", "ss_id", "out_sr")
 
-    def __init__(self, tts_keys: dict, conv_keys: dict):
-        self.tts_keys, self.conv_keys = tts_keys, conv_keys
+    def __init__(self, tts_keys: dict, conv_keys: dict, out_sr: Optional[int] = None):
+        self.tts_keys, self.conv_keys, self.out_sr = tts_keys, conv_keys, out_sr
         self.said = 0                                     # sentences said so far: the next one is sentence `said`
         self.unencoded = 0                                # said sentences still waiting for the encode
         self.plans: deque = deque()                       # TTS windows to decode: (pool row, lo, hi, e0, e1, gap, last)
@@ -635,8 +797,11 @@ class CloneSessions:
     OPEN_KEYS = ("speaker", "src_se", "tgt_se", "tau", "seed", "convert_seed", "speed", "noise_scale", "noise_scale_w",
                  "sdp_ratio")
 
-    def __init__(self, converter, tts, window_frames: int = 256, first_window_frames: int = 32, label: str = "session"):
-        """``label``: how errors name a session ("session 3"); ``clone_stream_batch`` passes "request"."""
+    def __init__(self, converter, tts, window_frames: int = 256, first_window_frames: int = 32, label: str = "session",
+                 output_rates: Iterable[int] = ()):
+        """``label``: how errors name a session ("session 3"); ``clone_stream_batch`` passes "request".
+        ``output_rates``: the rates other than the model's that ``open(output_sr=)`` accepts (``StreamingSessions``
+        ``rates``: the converter side is made here, with their filter banks, rather than with the first audio)."""
         W, W1 = int(window_frames), int(first_window_frames)
         if W < 1 or W1 < 1:
             raise ValueError(f"window_frames ({W}) and first_window_frames ({W1}) must be >= 1")
@@ -646,12 +811,15 @@ class CloneSessions:
                              f"streaming text to cloned voice needs one rate (clone_batch resamples)")
         converter._check_same_device(tts)
         self.conv, self.tts, self.W, self.W1, self.sr, self.label = converter, tts, W, W1, sr, label
+        self.output_rates = tuple(output_rates)
         self.hop, self.nfft = converter.hps.data.hop_length, converter.hps.data.filter_length
         self.H = converter.HALO_FRAMES
         self.sessions: Dict[int, _CloneSession] = {}
         self.next_id = 0
         self.pending: List[Tuple[int, List[int]]] = []   # (session, token ids) said since the last encode, in order
         self.ss: Optional[StreamingSessions] = None       # the converter side, made with the first audio
+        if self.output_rates:                             # ... or here, where its filter banks may wait for the device
+            self.ss = StreamingSessions(converter, window_frames=W, rates=self.output_rates)
         self.pool = None                                  # api.TtsPool, made with the first encode
         self.free_rows: List[int] = []
         self.rows = 0                                     # pool rows handed out so far
@@ -666,22 +834,29 @@ class CloneSessions:
     # ------------------------------------------------------------------ sessions
     def open(self, speaker, src_se=None, tgt_se=None, tau: float = 0.3, seed: Optional[int] = None,
              convert_seed: Optional[int] = None, speed: float = 1.0, noise_scale: float = 0.667,
-             noise_scale_w: float = 0.6, sdp_ratio: float = 0.2) -> int:
+             noise_scale_w: float = 0.6, sdp_ratio: float = 0.2, output_sr: Optional[int] = None) -> int:
         """Start a session and return its id.  The keys are those of a ``clone_batch`` request, validated as it
         validates them, and the noise parameters as the encode checks them (ValueError naming the session); ``seed`` /
         ``convert_seed`` default to draws from torch's generator.  The speaker id is checked against the checkpoint
-        with the session's first ``say``."""
+        with the session's first ``say``.  ``output_sr``: the rate of the returned audio, the model's or one of
+        ``output_rates`` (None: the model's)."""
         from .api import check_per_item
         q = dict(speaker=speaker, src_se=src_se, tgt_se=tgt_se, tau=tau, seed=seed, convert_seed=convert_seed,
                  speed=speed, noise_scale=noise_scale, noise_scale_w=noise_scale_w, sdp_ratio=sdp_ratio)
         who = f"{self.label} {self.next_id}"
+        declared = self.ss.rates if self.ss is not None else ()
+        if output_sr is not None and (isinstance(output_sr, bool) or int(output_sr) != output_sr
+                                      or int(output_sr) not in (self.sr,) + declared):
+            raise ValueError(f"{who}: output_sr={output_sr!r}: sessions return audio at the model's rate ({self.sr} Hz) "
+                             f"or at a rate declared with output_rates= (declared: "
+                             f"{', '.join(map(str, declared)) or 'none'})")
         tts_keys = self.tts._request_keys(q, who)
         for name in ("noise_scale", "noise_scale_w", "sdp_ratio"):
             check_per_item([tts_keys[name]], 1, f"{who}: {name}")
         conv_keys = self.conv._clone_keys(q, who)
         sid = self.next_id
         self.next_id += 1
-        self.sessions[sid] = _CloneSession(tts_keys, conv_keys)
+        self.sessions[sid] = _CloneSession(tts_keys, conv_keys, None if output_sr is None else int(output_sr))
         return sid
 
     def _session(self, sid) -> _CloneSession:
@@ -838,7 +1013,7 @@ class CloneSessions:
             s = self.sessions[sid]
             if s.ss_id is None:
                 c = s.conv_keys
-                s.ss_id = ss.open(c["src_se"], c["tgt_se"], tau=c["tau"], seed=c["convert_seed"])
+                s.ss_id = ss.open(c["src_se"], c["tgt_se"], tau=c["tau"], seed=c["convert_seed"], output_sr=s.out_sr)
         sids = {sid: self.sessions[sid].ss_id for sid in runs}
         if wins:
             for enc, pairs in self._fresh:               # each row's decode key, stream and noise scale, as encoded
