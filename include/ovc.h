@@ -25,13 +25,14 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 13 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 14 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
                                * 8: ovc_spectrogram_ring; 9: OVC_OPT_PAIR_OCC; 10: ovc_splice;
                                * 11: ovc_tts_encode_state_rows, ovc_tts_state_rows; 12: OVC_OPT_STAGED_EPI;
-                               * 13: ovc_resample_plan, ovc_resample_rings */
+                               * 13: ovc_resample_plan, ovc_resample_rings;
+                               * 14: ovc_voice_conversion_frames, ovc_convert_waveform_frames, ovc_tone_track_expand */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -58,7 +59,7 @@ typedef struct ovc_hparams {
   int32_t spec_channels;            /* filter_length/2+1 = 513          api.py:25            */
   int32_t inter_channels;           /* 192                              models.py:408        */
   int32_t hidden_channels;          /* 192                              models.py:409        */
-  int32_t gin_channels;             /* 256                              models.py:422        */
+  int32_t gin_channels;             /* 256 (at most 256: ovc_finalize_weights refuses more) models.py:422 */
   int32_t resblock;                 /* 1 (ResBlock1)                    models.py:242        */
   int32_t n_resblock_kernels;       /* 3                                                     */
   int32_t resblock_kernel_sizes[4]; /* 3,7,11                           models.py:261-264    */
@@ -223,6 +224,45 @@ OVC_API int ovc_convert_waveform_items(ovc_ctx* ctx, const float* wav, const int
                                        const float* g_src, const float* g_tgt, const float* noise, uint64_t seed,
                                        float tau, float* o_hat, int64_t* frames, void* stream,
                                        const ovc_item_params* items);
+
+/* Time-varying tone colour (reference: SynthesizerTrn.voice_conversion with sid_src / sid_tgt of shape [B, gin, T]).
+ * se_frames is a bit set naming the sides given per frame:
+ *   OVC_SE_FRAMES_SRC  g_src is [B, gin, Tmax] (frame t of item b at g_src[(b*gin + c)*Tmax + t]); else [B, gin]
+ *   OVC_SE_FRAMES_TGT  the same for g_tgt
+ * The source side conditions enc_q and the flow forward, the target side the flow reverse and the generator's cond
+ * (zero_g checkpoints keep enc_q and the generator unconditioned, as the per-item calls do).  A frame whose embedding
+ * equals an item's per-item embedding gets bit-identical conditioning, so se_frames = 0 is exactly the _items entry
+ * point and a constant per-frame embedding converts to the per-item result.  Per-frame calls grow the workspace by
+ * B * Tmax * 4 bytes times 18944 (both sides) or 6656 (target only) conditioning columns; se_frames is part of the
+ * CUDA graph key.  Everything else as ovc_voice_conversion_items / ovc_convert_waveform_items (for the latter Tmax =
+ * Lmax / hop).  The conditioning kernel holds each lane's 8 weights of a row in registers and reads one side per block
+ * of 32 output columns, so ovc_finalize_weights refuses gin_channels > 256 and conditioning sections whose sizes
+ * (2 * hidden_channels per WN layer, upsample_initial_channel for the generator) are not multiples of 32, for every
+ * call; every released checkpoint has gin 256, 2 * hidden 384 and 512. */
+#define OVC_SE_FRAMES_SRC 1
+#define OVC_SE_FRAMES_TGT 2
+OVC_API int ovc_voice_conversion_frames(ovc_ctx* ctx, const float* spec, const int64_t* lengths, const float* g_src,
+                                        const float* g_tgt, int se_frames, const float* noise, uint64_t seed, float tau,
+                                        int B, int Tmax, int ragged, float* o_hat, float* z, float* z_p, float* z_hat,
+                                        void* stream, const ovc_item_params* items);
+OVC_API int ovc_convert_waveform_frames(ovc_ctx* ctx, const float* wav, const int64_t* wav_lengths, int B, int Lmax,
+                                        const float* g_src, const float* g_tgt, int se_frames, const float* noise,
+                                        uint64_t seed, float tau, float* o_hat, int64_t* frames, void* stream,
+                                        const ovc_item_params* items);
+
+/* Per-frame embeddings from keyframe tracks ("tone tracks").  Keys are n_keys pairs (key_frame[k], key_se[k, 0:gin]);
+ * track b is keys [key0[b], key0[b] + nkeys[b]) with non-decreasing frames.  out[b, c, t] = g_b(frame0[b] + t) for
+ * t < frames[b], 0 for frames[b] <= t < Tmax, where g(t) is the first key's embedding before the first key, the last
+ * key's from the last key on, and se_k + ((t - f_k) / (f_{k+1} - f_k)) * (se_{k+1} - se_k) for f_k <= t < f_{k+1}, each
+ * operation rounded to fp32 on its own; of keys sharing a frame the later one holds from that frame on (a hard switch).
+ * Item b's frame t is evaluated at absolute frame frame0[b] + t, so a window of a longer clip gets the whole clip's values.
+ *   key_frame [n_keys] int64, key_se [n_keys, gin] fp32, key0 / nkeys / frame0 / frames [B] int64 (all device); the
+ *   per-item values are clamped on the device, so no read leaves the key arrays.
+ *   out       [B, gin, Tmax] fp32: the per-frame layout ovc_*_frames read.
+ * Only enqueues on `stream`; graph-capturable. */
+OVC_API int ovc_tone_track_expand(ovc_ctx* ctx, const int64_t* key_frame, const float* key_se, int64_t n_keys,
+                                  const int64_t* key0, const int64_t* nkeys, const int64_t* frame0, const int64_t* frames,
+                                  int B, int Tmax, float* out, void* stream);
 
 /* Tone-colour embedding of extract_se (row f2): ReferenceEncoder.forward (openvoice/models.py:339-359; call site
  * openvoice/api.py:130) on device -- LayerNorm over frequency, 6 x (Conv2d 3x3 s2 + ReLU), GRU(128) last state,

@@ -13,7 +13,7 @@ from . import utils  # noqa: F401
 
 def __getattr__(name):  # lazy: importing the package must not require torch/CUDA
     import importlib
-    if name in ("ToneColorConverter", "OpenVoiceBaseClass", "BaseSpeakerTTS", "NativeSynthesizer"):
+    if name in ("ToneColorConverter", "OpenVoiceBaseClass", "BaseSpeakerTTS", "NativeSynthesizer", "ToneTrack"):
         return getattr(importlib.import_module(".api", __name__), name)
     if name in ("api", "se_extractor", "schema", "ref_enc", "distributed"):
         return importlib.import_module("." + name, __name__)

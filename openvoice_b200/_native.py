@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 13
+ABI_VERSION = 14
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -24,10 +24,26 @@ EXPORTS = (
     "ovc_convert_waveform_items", "ovc_tts_encode_items", "ovc_tts_decode_items", "ovc_philox_normals",
     "ovc_tts_encode_state", "ovc_tts_decode_windows", "ovc_spectrogram_ring", "ovc_splice",
     "ovc_tts_encode_state_rows", "ovc_tts_state_rows", "ovc_resample_plan", "ovc_resample_rings",
+    "ovc_voice_conversion_frames", "ovc_convert_waveform_frames", "ovc_tone_track_expand",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample / ovc_spectrogram_ring length of a stream that has not ended
 SPLICE_PCM16 = 1            # ovc_splice flag: the 16-bit PCM round trip of every copied value
+SE_FRAMES_SRC, SE_FRAMES_TGT = 1, 2   # ovc_*_frames: the side's embedding is given per frame
+
+
+def se_arg(g, B: int, gin: int, T: int, what: str):
+    """(float32 contiguous [B, gin] or [B, gin, T] tensor, per_frame) of a speaker embedding: B * gin values (any
+    shape: one embedding per item) or a [B, gin, T] tensor (one per frame, T > 1).  Anything else raises ValueError,
+    so an embedding is never read as some other layout.  A 3-D tensor with gin rows and more than one column is a
+    per-frame embedding and must be exactly [B, gin, T]; it is never reinterpreted as per-item values."""
+    if g.dim() == 3 and g.shape[-2] == gin and g.shape[-1] > 1:
+        if T > 1 and tuple(g.shape) == (B, gin, T):
+            return g.contiguous().float(), True
+    elif g.numel() == B * gin:
+        return g.reshape(B, gin).contiguous().float(), False
+    raise ValueError(f"{what} has shape {tuple(g.shape)}: expected {B} x {gin} values (one embedding per item) or "
+                     f"[{B}, {gin}, {T}] (one per frame)")
 
 
 class OvcHParams(C.Structure):
@@ -158,6 +174,12 @@ def load_library(path: Optional[str] = None):
     lib.ovc_tts_encode_state_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 5
     lib.ovc_tts_state_rows.argtypes = ([C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
                                        + [C.c_void_p] * 5)
+    lib.ovc_voice_conversion_frames.argtypes = (lib.ovc_voice_conversion.argtypes[:5] + [C.c_int]
+                                                + lib.ovc_voice_conversion.argtypes[5:] + [P])
+    lib.ovc_convert_waveform_frames.argtypes = (lib.ovc_convert_waveform.argtypes[:7] + [C.c_int]
+                                                + lib.ovc_convert_waveform.argtypes[7:] + [P])
+    lib.ovc_tone_track_expand.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64] + [C.c_void_p] * 4 + [
+        C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.ovc_resample_plan.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int32), C.c_void_p]
     lib.ovc_resample_rings.argtypes = ([C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64] + [C.c_void_p] * 5
                                        + [C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p])
@@ -295,7 +317,7 @@ class NativeConverter:
     # ---- hot path --------------------------------------------------------------------------
     def voice_conversion(self, spec, lengths, g_src, g_tgt, noise=None, tau: float = 0.3, seed: int = 0,
                          ragged: bool = False, latents: bool = True, stream=None, items: Optional[dict] = None, out=None):
-        """spec [B,S,T] f32 cuda, lengths [B] i64 cuda, g_* [B,gin(,1)] f32 cuda.
+        """spec [B,S,T] f32 cuda, lengths [B] i64 cuda, g_* [B,gin(,1)] (per item) or [B,gin,T] (per frame) f32 cuda.
         Returns (o_hat [B,1,hop*T], (z, z_p, z_hat) or None).  Asynchronous on `stream`.  ``items``: per-item
         parameters ``{"seed", "stream", "frame0", "tau": [B] cuda tensor}`` (see ``item_params``), or None.  ``out``:
         a caller-owned o_hat buffer of B * hop * T floats (a repeated call on stable buffers replays its CUDA graph)."""
@@ -303,8 +325,8 @@ class NativeConverter:
         assert spec.is_cuda and spec.dtype == torch.float32 and spec.is_contiguous()
         assert lengths.is_cuda and lengths.dtype == torch.int64 and lengths.is_contiguous()
         B, S, T = spec.shape
-        gs = g_src.reshape(B, -1).contiguous().float()
-        gt = g_tgt.reshape(B, -1).contiguous().float()
+        gs, fs = se_arg(g_src, B, self.hp.gin_channels, T, "g_src")
+        gt, ft = se_arg(g_tgt, B, self.hp.gin_channels, T, "g_tgt")
         if noise is not None:
             noise = noise.contiguous().float()
             assert tuple(noise.shape) == (B, self.hp.inter_channels, T)
@@ -321,8 +343,9 @@ class NativeConverter:
         st = stream if stream is not None else torch.cuda.current_stream(spec.device)
         p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
         it = item_params(items, B)
-        rc = self.lib.ovc_voice_conversion_items(
-            self.handle, p(spec), p(lengths), p(gs), p(gt), p(noise), C.c_uint64(seed & (2 ** 64 - 1)),
+        rc = self.lib.ovc_voice_conversion_frames(
+            self.handle, p(spec), p(lengths), p(gs), p(gt), (SE_FRAMES_SRC if fs else 0) | (SE_FRAMES_TGT if ft else 0),
+            p(noise), C.c_uint64(seed & (2 ** 64 - 1)),
             C.c_float(tau), B, T, 1 if ragged else 0, p(o),
             p(lat[0]) if lat else None, p(lat[1]) if lat else None, p(lat[2]) if lat else None,
             C.c_void_p(st.cuda_stream), _items_ref(it))
@@ -375,14 +398,15 @@ class NativeConverter:
         """The device work of ToneColorConverter.convert for a batch: wav [B, Lmax] f32 cuda ->
         (o_hat [B, hop * (Lmax // hop)], frames [B]).  Asynchronous on `stream`.  ``out`` / ``frames_out`` let the
         caller supply the result buffers: with every buffer at a stable address, a repeated call is replayed from a
-        CUDA graph (include/ovc.h: OVC_OPT_GRAPH).  ``items`` as in ``voice_conversion``."""
+        CUDA graph (include/ovc.h: OVC_OPT_GRAPH).  ``items`` as in ``voice_conversion``; ``g_*`` per item or
+        [B, gin, Lmax // hop] per frame."""
         import torch
         assert wav.is_cuda and wav.dtype == torch.float32 and wav.is_contiguous() and wav.dim() == 2
         assert wav_lengths.is_cuda and wav_lengths.dtype == torch.int64
         B, L = wav.shape
         T = L // self.hp.hop_length
-        gs = g_src.reshape(B, -1).contiguous().float()
-        gt = g_tgt.reshape(B, -1).contiguous().float()
+        gs, fs = se_arg(g_src, B, self.hp.gin_channels, T, "g_src")
+        gt, ft = se_arg(g_tgt, B, self.hp.gin_channels, T, "g_tgt")
         if noise is not None:
             noise = noise.contiguous().float()
             assert tuple(noise.shape) == (B, self.hp.inter_channels, T)
@@ -398,13 +422,41 @@ class NativeConverter:
             frames = torch.empty(B, device=wav.device, dtype=torch.int64)
         st = stream if stream is not None else torch.cuda.current_stream(wav.device)
         it = item_params(items, B)
-        rc = self.lib.ovc_convert_waveform_items(
+        rc = self.lib.ovc_convert_waveform_frames(
             self.handle, C.c_void_p(wav.data_ptr()), C.c_void_p(wav_lengths.data_ptr()), B, L, C.c_void_p(gs.data_ptr()),
-            C.c_void_p(gt.data_ptr()), C.c_void_p(noise.data_ptr()) if noise is not None else None,
+            C.c_void_p(gt.data_ptr()), (SE_FRAMES_SRC if fs else 0) | (SE_FRAMES_TGT if ft else 0), C.c_void_p(noise.data_ptr()) if noise is not None else None,
             C.c_uint64(seed & (2 ** 64 - 1)), C.c_float(tau), C.c_void_p(o.data_ptr()), C.c_void_p(frames.data_ptr()),
             C.c_void_p(st.cuda_stream), _items_ref(it))
         _check(self.lib, rc, "ovc_convert_waveform")
         return o, frames
+
+    def tone_track_expand(self, key_frame, key_se, key0, nkeys, frame0, frames, Tmax: int, out=None, stream=None):
+        """Per-frame embeddings [B, gin, Tmax] from keyframe tracks (include/ovc.h: ovc_tone_track_expand).
+        key_frame [K] i64, key_se [K, gin] f32, key0 / nkeys / frame0 / frames [B] i64, all cuda and contiguous; item b
+        is track keys [key0[b], key0[b] + nkeys[b]) evaluated at frames frame0[b] + t, t < frames[b] (zeros after).
+        Written into ``out`` when given.  Asynchronous on `stream`."""
+        import torch
+        gin = self.hp.gin_channels
+        K = key_frame.numel()
+        assert key_frame.is_cuda and key_frame.dtype == torch.int64 and key_frame.is_contiguous()
+        assert key_se.is_cuda and key_se.dtype == torch.float32 and key_se.is_contiguous()
+        if tuple(key_se.shape) != (K, gin):
+            raise ValueError(f"key_se has shape {tuple(key_se.shape)}, expected ({K}, {gin})")
+        B = key0.numel()
+        for t in (key0, nkeys, frame0, frames):
+            assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()
+            if tuple(t.shape) != (B,):
+                raise ValueError(f"tone_track_expand: per-item arrays need shape ({B},), got {tuple(t.shape)}")
+        shape = (B, gin, int(Tmax))
+        if out is None:
+            out = torch.empty(shape, device=key_se.device, dtype=torch.float32)
+        assert out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == shape
+        st = stream if stream is not None else torch.cuda.current_stream(key_se.device)
+        p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+        rc = self.lib.ovc_tone_track_expand(self.handle, p(key_frame), p(key_se), K, p(key0), p(nkeys), p(frame0), p(frames),
+                                            B, int(Tmax), p(out), C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_tone_track_expand")
+        return out
 
     def reference_encoder(self, spec, lengths=None, stream=None):
         """spec [N, S, T] f32 cuda (ovc_spectrogram layout) -> tone-colour embedding [N, gin]

@@ -26,6 +26,119 @@ from .schema import hot_path_keys, ref_enc_keys, tts_keys
 AudioLike = Union[str, np.ndarray]
 
 
+class ToneTrack:
+    """A tone colour that changes over time: keyframes ``(frame, embedding)`` at non-decreasing spectrogram frames
+    (256 samples at the model's rate each).  At frame t the embedding is the first key's before the first key, the last
+    key's from the last key on, and between keys f_k <= t < f_{k+1} the fp32 interpolation
+    ``se_k + ((t - f_k) / (f_{k+1} - f_k)) * (se_{k+1} - se_k)``; two keys at the same frame switch hard to the later one
+    there.  A track means exactly the per-frame embedding ``dense`` returns, and the conversion paths evaluate it on the
+    device (include/ovc.h: ovc_tone_track_expand) with the same arithmetic."""
+
+    def __init__(self, keys):
+        ks = list(keys)
+        if not ks:
+            raise ValueError("a ToneTrack needs at least one keyframe")
+        frames, ses = [], []
+        for f, se in ks:
+            if int(f) != f or f < 0:
+                raise ValueError(f"keyframe frame {f!r} is not a non-negative integer")
+            frames.append(int(f))
+            ses.append(torch.as_tensor(se, dtype=torch.float32).detach().reshape(-1).cpu())
+        if any(b < a for a, b in zip(frames, frames[1:])):
+            raise ValueError(f"keyframe frames must not decrease: {frames}")
+        if any(s_.numel() != ses[0].numel() for s_ in ses):
+            raise ValueError("keyframe embeddings differ in size")
+        self.frames = np.asarray(frames, dtype=np.int64)
+        self.se = torch.stack(ses).contiguous()          # [K, gin]
+
+    def dense(self, T: int, frame0: int = 0) -> torch.Tensor:
+        """[1, gin, T] float32 (host): the embedding at frames frame0 .. frame0 + T - 1."""
+        kf, kse = self.frames, self.se.numpy()
+        t = np.arange(frame0, frame0 + T, dtype=np.int64)
+        hi = np.searchsorted(kf, t, side="right")                  # first key with frame > t
+        lo = np.clip(hi - 1, 0, len(kf) - 1)
+        nx = np.clip(hi, 0, len(kf) - 1)
+        inner = (hi > 0) & (hi < len(kf))
+        span = np.where(inner, kf[nx] - kf[lo], 1).astype(np.float32)
+        u = np.where(inner, (t - kf[lo]).astype(np.float32) / span, np.float32(0)).astype(np.float32)
+        a, b = kse[lo], kse[nx]                                     # [T, gin]
+        out = np.where(inner[:, None], a + u[:, None] * (b - a), a).astype(np.float32)
+        return torch.from_numpy(np.ascontiguousarray(out.T))[None]
+
+
+def _take(side, idx):
+    """Items ``idx`` of a ``ToneColorConverter._se_items`` result (tensor rows or list entries)."""
+    return [side[i] for i in idx] if isinstance(side, list) else side[idx]
+
+
+def is_per_frame_se(se, gin: Optional[int] = None) -> bool:
+    """Whether ``se`` (an embedding or a per-item sequence of them) varies over time: a ToneTrack or a [n, gin, T]
+    tensor with T > 1.  Without ``gin`` any [n, C, T] with C > 1 and T > 1 counts, so a [1, 1, gin] row vector stays
+    one embedding per item, as it always was."""
+    if isinstance(se, (list, tuple)):
+        return any(is_per_frame_se(x, gin) for x in se)
+    if isinstance(se, ToneTrack):
+        return True
+    if not torch.is_tensor(se) or se.dim() != 3 or se.shape[-1] <= 1:
+        return False
+    return se.shape[-2] == gin if gin is not None else se.shape[-2] > 1
+
+
+def pack_tone_keys(entries, frame0: Sequence[int], frames: Sequence[int], what: str = "embedding",
+                   clip: Optional[int] = None):
+    """Keyframes for ``ovc_tone_track_expand`` of items whose embeddings are ``entries``: a [gin] tensor (one
+    embedding), a [gin, T] tensor (per frame over the item's whole clip, T == ``clip``, default frames[b]) or a
+    ``ToneTrack``; item b is read at frames frame0[b] .. frame0[b] + frames[b] - 1.  Returns (key_frame [K] int64,
+    key_se [K, gin] float32, key0 [B], nkeys [B]), all on the host.
+
+    Only the keys a window can read are packed: a per-frame tensor gives one key per frame of the window (a key at
+    every integer frame reproduces the values exactly), a track its keys from the last one at or before the window's
+    first frame to the first one after its last frame.  Items that read the same keys share them.  So K is at most the
+    windows' frames plus a few keys per track, whatever the clip's length or the track's history."""
+    key_frame, key_se, key0, nkeys, seen = [], [], [], [], {}
+    for b, e in enumerate(entries):
+        f0, n = int(frame0[b]), int(frames[b])
+        if isinstance(e, ToneTrack):
+            kf = e.frames
+            k0 = max(0, int(np.searchsorted(kf, f0, side="right")) - 1)
+            k1 = min(len(kf), int(np.searchsorted(kf, f0 + n - 1, side="right")) + 1)
+            tag = (id(e), k0, k1)
+            if tag not in seen:
+                seen[tag] = (len(key_frame), k1 - k0)
+                key_frame.extend(kf[k0:k1].tolist())
+                key_se.append(e.se[k0:k1])
+        elif e.dim() == 2:
+            want = n if clip is None else clip
+            if e.shape[1] != want:
+                raise ValueError(f"{what}: item {b} has {want} frames but its per-frame embedding {e.shape[1]}")
+            tag = (id(e), f0, n)
+            if tag not in seen:
+                seen[tag] = (len(key_frame), n)
+                key_frame.extend(range(f0, f0 + n))
+                key_se.append(e[:, f0:f0 + n].T)
+        else:
+            tag = (id(e),)
+            if tag not in seen:
+                seen[tag] = (len(key_frame), 1)
+                key_frame.append(0)
+                key_se.append(e.reshape(1, -1))
+        key0.append(seen[tag][0])
+        nkeys.append(seen[tag][1])
+    ks = torch.cat([k.detach().to(torch.float32).cpu() for k in key_se], 0).contiguous()
+    return np.asarray(key_frame, dtype=np.int64), ks, key0, nkeys
+
+
+def expand_tone_keys(native, entries, frame0, frames, Tmax: int, out=None, what: str = "embedding",
+                     clip: Optional[int] = None):
+    """The per-frame [B, gin, Tmax] embedding of ``entries`` (``pack_tone_keys``), expanded on the device by the
+    tone-track kernel into ``out`` when given (zeros past each item's frames)."""
+    dev = torch.device("cuda", native.device_index)
+    kf, ks, key0, nkeys = pack_tone_keys(entries, frame0, frames, what, clip)
+    i64 = lambda v: torch.as_tensor(np.asarray(v, dtype=np.int64)).to(dev)  # noqa: E731
+    return native.tone_track_expand(i64(kf), ks.to(dev), i64(key0), i64(nkeys), i64(list(frame0)), i64(list(frames)),
+                                    Tmax, out=out)
+
+
 def check_seeds(seeds, n: int, what: str = "seeds") -> Optional[List[int]]:
     """Per-item Philox keys: None, or ``n`` integers in [0, 2^64).  ValueError otherwise (before any launch)."""
     if seeds is None:
@@ -322,7 +435,8 @@ class NativeSynthesizer:
         (openvoice/models.py:492-499).  ``noise`` ([B,192,T]) replaces the reference's
         ``randn_like``; when None, Philox normals are drawn in-kernel from ``seed`` (default: a
         draw from torch's global CPU generator, so ``torch.manual_seed`` makes runs repeatable).
-        ``ragged=True`` converts every item at its exact length (what ``convert`` does).
+        ``ragged=True`` converts every item at its exact length (what ``convert`` does).  ``sid_src`` / ``sid_tgt`` may
+        each be per item ([B or 1, gin(, 1)]) or per frame ([B or 1, gin, T]), as in the reference.
 
         Per-item sampling (include/ovc.h: ovc_item_params): ``seeds`` gives item b its own Philox key, drawn at stream
         ``streams[b]`` (default 0 for every item: a request's own noise, independent of its batch index) and frame
@@ -343,8 +457,8 @@ class NativeSynthesizer:
             raise ValueError(f"streams needs {B} values in [0, 2^32)")
         y = y.to(self.device, torch.float32).contiguous()
         y_lengths = y_lengths.to(self.device, torch.int64).contiguous()
-        sid_src = self._expand_se(sid_src, B)
-        sid_tgt = self._expand_se(sid_tgt, B)
+        sid_src = self._expand_se(sid_src, B, T)
+        sid_tgt = self._expand_se(sid_tgt, B, T)
         if noise is None and seed is None:
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())
         if noise is not None:
@@ -531,10 +645,15 @@ class NativeSynthesizer:
             [ln for _, _, ln in windows], [state.dec_keys[r] for r in rows], [state.dec_streams[r] for r in rows],
             [state.dec_noise_scale[r] for r in rows], w_max, latents=latents, slot=slot)
 
-    def _expand_se(self, se, B):
-        se = se.to(self.device, torch.float32).reshape(se.shape[0], -1)
+    def _expand_se(self, se, B, T=1):
+        """[B, gin] (per item) or [B, gin, T] (per frame) on the device; a batch of 1 serves every item."""
+        se = se.to(self.device, torch.float32)
+        per_frame = is_per_frame_se(se, self.native.hp.gin_channels)
+        if per_frame and se.shape[-1] != T:
+            raise ValueError(f"per-frame speaker embedding has {se.shape[-1]} frames, the batch {T}")
+        se = se if per_frame else se.reshape(se.shape[0], -1)
         if se.shape[0] == 1 and B > 1:
-            se = se.expand(B, -1)
+            se = se.expand(B, *se.shape[1:])
         if se.shape[0] != B:
             raise ValueError(f"speaker embedding batch {se.shape[0]} does not match batch {B}")
         return se.contiguous()
@@ -894,7 +1013,10 @@ class ToneColorConverter(OpenVoiceBaseClass):
                       seeds: Optional[Sequence[int]] = None) -> List[np.ndarray]:
         """Convert a list of utterances (paths or waveforms at the model sampling rate); every item
         gets exactly what ``convert`` would return for it alone.  ``src_se`` / ``tgt_se`` are either
-        one [1,gin,1] embedding for all items or a sequence of per-item embeddings.
+        one [1,gin,1] embedding for all items or a sequence of per-item embeddings.  An embedding may vary over time:
+        a ``ToneTrack`` or a [1, gin, T] tensor with T = the item's frames (samples // 256 at the model's rate), as the
+        reference's ``voice_conversion`` takes; one [1, gin, T] for the whole call needs every item to have T frames.
+        Items with a constant embedding convert exactly as they would alone.
 
         ``sr``: sampling rate of the NumPy waveform items when it is not the model's.  They are uploaded as they are
         and resampled on the device (``scipy.signal.resample_poly`` arithmetic, within one fp32 ulp of it) into the
@@ -915,14 +1037,14 @@ class ToneColorConverter(OpenVoiceBaseClass):
             raise ValueError("pass either noise or seeds, not both")
         rate = self._input_rate(audios, sr)
         waves = [_load_audio(a, hps.data.sampling_rate) for a in audios]
-        src = self._stack_se(src_se, n)
-        tgt = self._stack_se(tgt_se, n)
+        src = self._se_items(src_se, n, "src_se")
+        tgt = self._se_items(tgt_se, n, "tgt_se")
         out: List[Optional[np.ndarray]] = [None] * n
         order = sorted(range(n), key=lambda i: -len(waves[i]))     # similar lengths share a launch
         hop = hps.data.hop_length
         for lo in range(0, n, max_batch):
             idx = order[lo: lo + max_batch]
-            res = self._convert_chunk([waves[i] for i in idx], src[idx], tgt[idx],
+            res = self._convert_chunk([waves[i] for i in idx], _take(src, idx), _take(tgt, idx),
                                       tau if taus is None else [taus[i] for i in idx],
                                       None if noise is None else [noise[i] for i in idx], rate,
                                       None if seeds is None else [seeds[i] for i in idx])
@@ -966,6 +1088,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
         for name in ("src_se", "tgt_se"):
             if q.get(name) is None:
                 raise ValueError(f"{who} has no {name}")
+            if isinstance(q[name], ToneTrack):
+                raise ValueError(f"{who}: {name} is a ToneTrack; text to cloned voice takes one embedding per request")
             se = torch.as_tensor(q[name], dtype=torch.float32).reshape(1, -1)
             if se.shape[1] != gin:
                 raise ValueError(f"{who}: {name} has {se.shape[1]} values, the converter's embeddings have {gin}")
@@ -1094,8 +1218,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
         tau, taus = check_per_item(tau, n, "tau")
         seeds = check_seeds(seeds, n)
         rate = self._input_rate(audios, sr)
-        src = self._stack_se(src_se, n)
-        tgt = self._stack_se(tgt_se, n)
+        src = self._se_items(src_se, n, "src_se")
+        tgt = self._se_items(tgt_se, n, "tgt_se")
         reps = self._replicas(max(1, min(streams, n)))
         S, depth = len(reps), 2                       # requests in flight per stream (pinned staging slots)
         out: List[Optional[np.ndarray]] = [None] * n
@@ -1105,8 +1229,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
             for j, i in enumerate(wave):
                 conv, stream = reps[j % S]
                 with torch.cuda.stream(stream):
-                    pending.append(conv._enqueue_single(_load_audio(audios[i], self.hps.data.sampling_rate), src[i: i + 1],
-                                                        tgt[i: i + 1], tau if taus is None else taus[i], j // S, rate,
+                    pending.append(conv._enqueue_single(_load_audio(audios[i], self.hps.data.sampling_rate), _take(src, [i]),
+                                                        _take(tgt, [i]), tau if taus is None else taus[i], j // S, rate,
                                                         None if seeds is None else seeds[i]))
             for _, stream in reps:
                 stream.synchronize()
@@ -1145,6 +1269,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
         wlen = torch.tensor([L], dtype=torch.int64, device=dev)
         items = None if seed is None else self._item_arrays(f"c{slot}", [seed], None)
         seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+        src = self._se_device(src, [L // hop], [0], L // hop, "src_se")
+        tgt = self._se_device(tgt, [L // hop], [0], L // hop, "tgt_se")
         o, _ = self.model.native.convert_waveform(wav, wlen, src, tgt, tau=float(tau), seed=seed, items=items)
         host = self._pinned(f"cout{slot}", o.numel())
         host.copy_(o.view(-1), non_blocking=True)
@@ -1166,7 +1292,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
         a NumPy waveform that is not at the model's; it is resampled on the device first (see ``convert_batch``).
         ``seed``: the request's own key; each window then draws the whole clip's noise at its absolute frames in-kernel
         (frame0 = the window's first frame), so the result matches ``convert(seed=seed)`` and no noise tensor is
-        built.  ``seed`` with ``noise`` raises ValueError."""
+        built.  ``seed`` with ``noise`` raises ValueError.  ``src_se`` / ``tgt_se`` may vary over time (a ``ToneTrack``
+        or [1, gin, T], as in ``convert_batch``): each window reads the whole clip's embedding at its absolute frames."""
         hps = self.hps
         seed = None if seed is None else check_seeds([seed], 1, "seed")[0]
         if seed is not None and noise is not None:
@@ -1192,8 +1319,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
         wins = [(max(0, s - H), min(T, s + window_frames + H), s, min(T, s + window_frames)) for s in starts]
         Wmax = max(hi - lo for lo, hi, _, _ in wins)
         out = torch.empty(T * hop, device=dev, dtype=torch.float32)
-        src = self._stack_se(src_se, 1)
-        tgt = self._stack_se(tgt_se, 1)
+        src = self._se_items(src_se, 1, "src_se")
+        tgt = self._se_items(tgt_se, 1, "tgt_se")
         for i0 in range(0, len(wins), max_batch):
             chunk = wins[i0: i0 + max_batch]
             B = len(chunk)
@@ -1205,7 +1332,10 @@ class ToneColorConverter(OpenVoiceBaseClass):
                     nz[b, :, : hi - lo] = noise[:, lo:hi]
             lens = torch.tensor([hi - lo for lo, hi, _, _ in chunk], dtype=torch.int64, device=dev)
             keyed = {} if seed is None else dict(seeds=[seed] * B, frame0=[lo for lo, _, _, _ in chunk])
-            o, _, _ = self.model.voice_conversion(sp, lens, src.expand(B, -1), tgt.expand(B, -1), tau=tau, noise=nz,
+            f0s, fr = [lo for lo, _, _, _ in chunk], [hi - lo for lo, hi, _, _ in chunk]
+            g_s = src.expand(B, -1) if not isinstance(src, list) else self._se_device(src * B, fr, f0s, Wmax, "src_se", clip=T)
+            g_t = tgt.expand(B, -1) if not isinstance(tgt, list) else self._se_device(tgt * B, fr, f0s, Wmax, "tgt_se", clip=T)
+            o, _, _ = self.model.voice_conversion(sp, lens, g_s, g_t, tau=tau, noise=nz,
                                                   ragged=True, latents=False, **keyed)
             for b, (lo, hi, s, e) in enumerate(chunk):
                 out[s * hop: e * hop] = o[b, 0, (s - lo) * hop: (e - lo) * hop]
@@ -1234,6 +1364,9 @@ class ToneColorConverter(OpenVoiceBaseClass):
         return n if sr is None else resample_span(sr, self.hps.data.sampling_rate, n)[0]
 
     def _stack_se(self, se, n):
+        """[n, gin] per-item embeddings on the device; ValueError for one that varies over time."""
+        if is_per_frame_se(se, int(getattr(self.hps.model, "gin_channels", 256))):
+            raise ValueError("this path takes one embedding per item ([1, gin] or [1, gin, 1]), not a per-frame one")
         if isinstance(se, (list, tuple)):
             se = torch.cat([s.reshape(1, -1) for s in se], 0)
         se = se.to(self.device, torch.float32).reshape(se.shape[0], -1)
@@ -1241,6 +1374,47 @@ class ToneColorConverter(OpenVoiceBaseClass):
             se = se.expand(n, -1)
         assert se.shape[0] == n, "one speaker embedding per utterance (or a single one for all)"
         return se
+
+    def _se_items(self, se, n, what: str):
+        """The embeddings of n items: ``_stack_se``'s [n, gin] tensor when none varies over time (the per-item path,
+        unchanged), else a list of n entries, each a [gin] tensor (per item), a [gin, T] tensor (per frame, T > 1) or a
+        ``ToneTrack``.  ValueError for an embedding of the wrong size or shape."""
+        gin = int(getattr(self.hps.model, "gin_channels", 256))
+        if not is_per_frame_se(se, gin):
+            return self._stack_se(se, n)
+        items = list(se) if isinstance(se, (list, tuple)) else [se] * n
+        if len(items) != n:
+            raise ValueError(f"{what}: {len(items)} embeddings for {n} items")
+        out = []
+        for i, e in enumerate(items):
+            if isinstance(e, ToneTrack):
+                if e.se.shape[1] != gin:
+                    raise ValueError(f"{what}[{i}]: ToneTrack embeddings have {e.se.shape[1]} values, the model's {gin}")
+                out.append(e)
+                continue
+            e = torch.as_tensor(e, dtype=torch.float32)
+            if e.numel() == gin:
+                out.append(e.reshape(gin))
+            elif e.dim() == 3 and e.shape[0] == 1 and e.shape[1] == gin and e.shape[2] > 1:
+                out.append(e[0])
+            else:
+                raise ValueError(f"{what}[{i}] has shape {tuple(e.shape)}: expected [1, {gin}(, 1)], [1, {gin}, T] or a "
+                                 f"ToneTrack")
+        return out
+
+    def _se_device(self, side, frames, frame0, Tmax: int, what: str, buf: Optional[str] = None,
+                   clip: Optional[int] = None):
+        """One side of a launch on the device: a [B, gin] tensor as it is, or a list of ``_se_items`` entries as the
+        per-frame [B, gin, Tmax] embedding (item b at frames frame0[b] + t, t < frames[b]; zeros after), expanded by the
+        tone-track kernel (``pack_tone_keys``).  A [gin, T] entry must cover the item's whole clip: T == ``clip``
+        (default frames[b]).
+        ``buf`` names a cached device buffer for the result (a stable address: the launch can be replayed from its CUDA
+        graph)."""
+        if not isinstance(side, list):
+            return side
+        gin = int(getattr(self.hps.model, "gin_channels", 256))
+        out = None if buf is None else self._dev(buf, len(side) * gin * Tmax, torch.float32).view(len(side), gin, Tmax)
+        return expand_tone_keys(self.model.native, side, frame0, frames, Tmax, out, what, clip)
 
     def _enqueue_chunk(self, waves, src, tgt, tau, noise, slot=0, sr=None, seeds=None, fill=None):
         """Stage, upload and launch one ragged batch on the current stream WITHOUT synchronising the host.
@@ -1299,10 +1473,16 @@ class ToneColorConverter(OpenVoiceBaseClass):
         lens_pin.copy_(torch.tensor(lens, dtype=torch.int64))
         wlen = self._dev(f"len{slot}", B, torch.int64)
         wlen.copy_(lens_pin, non_blocking=True)
-        src_d = self._dev(f"src{slot}", src.numel(), torch.float32).view(B, -1)
-        src_d.copy_(src.reshape(B, -1), non_blocking=True)
-        tgt_d = self._dev(f"tgt{slot}", tgt.numel(), torch.float32).view(B, -1)
-        tgt_d.copy_(tgt.reshape(B, -1), non_blocking=True)
+        if isinstance(src, list):
+            src_d = self._se_device(src, frames, [0] * B, Lmax // hop, "src_se", f"srcf{slot}")
+        else:
+            src_d = self._dev(f"src{slot}", src.numel(), torch.float32).view(B, -1)
+            src_d.copy_(src.reshape(B, -1), non_blocking=True)
+        if isinstance(tgt, list):
+            tgt_d = self._se_device(tgt, frames, [0] * B, Lmax // hop, "tgt_se", f"tgtf{slot}")
+        else:
+            tgt_d = self._dev(f"tgt{slot}", tgt.numel(), torch.float32).view(B, -1)
+            tgt_d.copy_(tgt.reshape(B, -1), non_blocking=True)
         taus = None if np.ndim(tau) == 0 else list(tau)
         items = None if seeds is None and taus is None else self._item_arrays(f"b{slot}", seeds, taus)
         ev = torch.cuda.Event()
@@ -1367,7 +1547,7 @@ class ToneColorConverter(OpenVoiceBaseClass):
         seeds = check_seeds(seeds, n)
         rate = self._input_rate(audios, sr)
         waves = [_load_audio(a, self.hps.data.sampling_rate) for a in audios]
-        o, frames = self._enqueue_chunk(waves, self._stack_se(src_se, n), self._stack_se(tgt_se, n),
+        o, frames = self._enqueue_chunk(waves, self._se_items(src_se, n, "src_se"), self._se_items(tgt_se, n, "tgt_se"),
                                         tau if taus is None else taus, None, slot, rate, seeds)
         hop = self.hps.data.hop_length
         return o, [f * hop for f in frames]

@@ -70,6 +70,8 @@ struct ConvArgs {
   int split;        // RESSKIP: rows < split update x, rows >= split go to skip[row-split]
   unsigned long long seed;   // PROJ without explicit noise
   const CallParams* callp;   // PROJ: when set, seed and tau are read from here instead (graph replay)
+  long long bias_ts;         // LINEAR / GATE: per-frame bias, + min(t, tmax - 1) * bias_ts (0: one vector per item; a
+                             // non-zero stride launches the PF instantiation, so per-item launches run the kernels as before)
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -291,8 +293,9 @@ __device__ __forceinline__ void stage_x_activate(float* xs, float slope) {
 // ---------------------------------------------------------------------------------------------
 // the kernel
 // ---------------------------------------------------------------------------------------------
-template <class C>
-__global__ void __launch_bounds__(C::THREADS, C::MIN_BLOCKS) conv1d_f32(const ConvArgs a) {
+// PF: the LINEAR / GATE bias is read per frame (ConvArgs.bias_ts); conv1d_f32_pf instantiates it
+template <class C, bool PF>
+__device__ __forceinline__ void conv1d_f32_body(const ConvArgs& a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
   float* wsm = reinterpret_cast<float*>(smem_raw + 16);
@@ -376,10 +379,15 @@ __global__ void __launch_bounds__(C::THREADS, C::MIN_BLOCKS) conv1d_f32(const Co
       if (t >= out_lim) continue;
 #pragma unroll
       for (int r = 0; r < 8; ++r) {
-        const float bv = bias[r];
         float v[4];
+        if constexpr (PF) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) v[j] = acc[c][r][j] + bv;
+          for (int j = 0; j < 4; ++j) v[j] = acc[c][r][j] + bias[(size_t)min(t + j, a.tmax - 1) * a.bias_ts + r];
+        } else {
+          const float bv = bias[r];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) v[j] = acc[c][r][j] + bv;
+        }
         float* yp = yb + (size_t)(row0 + r) * a.y_pitch + t;
         if (t + 3 < out_lim) {
           if (rb) {
@@ -423,7 +431,10 @@ __global__ void __launch_bounds__(C::THREADS, C::MIN_BLOCKS) conv1d_f32(const Co
         float v[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j)
-          v[j] = tanhf(acc[c][r][j] + gb[r]) * sigmoidf_acc(acc[c][r + 4][j] + gb[r + 4]);
+        {
+          const float* gt = PF ? gb + (size_t)min(t + j, a.tmax - 1) * a.bias_ts : gb;
+          v[j] = tanhf(acc[c][r][j] + gt[r]) * sigmoidf_acc(acc[c][r + 4][j] + gt[r + 4]);
+        }
         float* yp = yb + (size_t)(ch0 + r) * a.y_pitch + t;
         if (t + 3 < out_lim) {
           *reinterpret_cast<float4*>(yp) = make_float4(v[0], v[1], v[2], v[3]);
@@ -559,14 +570,39 @@ __global__ void __launch_bounds__(C::THREADS, C::MIN_BLOCKS) conv1d_f32(const Co
   }
 }
 
+template <class C>
+__global__ void __launch_bounds__(C::THREADS, C::MIN_BLOCKS) conv1d_f32(const ConvArgs a) {
+  conv1d_f32_body<C, false>(a);
+}
+template <class C>
+__global__ void __launch_bounds__(C::THREADS, C::MIN_BLOCKS) conv1d_f32_pf(const ConvArgs a) {
+  conv1d_f32_body<C, true>(a);
+}
+
 // host-side launcher for one configuration
 template <class C>
 struct ConvLaunch {
+  // the layers a per-frame conditioning vector feeds: the WaveNet in_layers (GATE) and the generator's conv_pre (LINEAR,
+  // k 7); only they get the bias_ts instantiation
+  static constexpr bool kPerFrame = C::EPI == EPI_GATE || (C::EPI == EPI_LINEAR && C::K == 7 && C::DIL == 1);
   static cudaError_t prepare() {
+    if constexpr (kPerFrame) {
+      const cudaError_t e = cudaFuncSetAttribute(conv1d_f32_pf<C>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 (int)C::SMEM_BYTES);
+      if (e != cudaSuccess) return e;
+    }
     return cudaFuncSetAttribute(conv1d_f32<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES);
   }
   static cudaError_t launch(const ConvArgs& a, int t_len, int row_tiles, int B, cudaStream_t st) {
     dim3 grid((t_len + C::T_T - 1) / C::T_T, row_tiles, B);
+    if constexpr (kPerFrame) {
+      if (a.bias_ts) {
+        conv1d_f32_pf<C><<<grid, C::THREADS, C::SMEM_BYTES, st>>>(a);
+        return cudaGetLastError();
+      }
+    } else if (a.bias_ts) {
+      return cudaErrorInvalidValue;   // a per-frame bias on a config without the bias_ts instantiation: refuse it
+    }
     conv1d_f32<C><<<grid, C::THREADS, C::SMEM_BYTES, st>>>(a);
     return cudaGetLastError();
   }

@@ -202,6 +202,12 @@ struct ovc_ctx {
   int cond_rows_out = 0;
   int cond_off_enc = 0, cond_off_fsrc = 0, cond_off_ftgt = 0, cond_off_dec = 0;
   int cond_off_enc_tc = 0, cond_off_fsrc_tc = 0, cond_off_ftgt_tc = 0;   // same vectors in the tc kernel's column order
+  // per-frame conditioning (a side whose embedding varies over time): the output columns of the sections that read a
+  // varying side, for column order o (0 fp32 kernels, 1 tensor cores) and varying sides m (1 src, 2 tgt, 3 both; index
+  // m - 1); cond_pf_off: column of section enc / flow src / flow tgt / dec in that vector, -1 = the per-item vector
+  int* d_cond_cols[2][3] = {};
+  int cond_pf_cols[2][3] = {};
+  int cond_pf_off[2][3][4] = {};
 
   // STFT tables (twiddles exp(-2 pi i m / 1024), periodic hann window)
   float2* d_tw = nullptr;
@@ -602,6 +608,37 @@ static int finalize(ovc_ctx* c) {
     c->cond_w_off = append(c->h_w, cw);
     c->cond_b_off = append(c->h_w, cbias);
   }
+  if (G > COND_GIN_MAX) return fail(OVC_ERR_INVALID, "gin_channels %d exceeds the conditioning kernel's %d", G, COND_GIN_MAX);
+  std::vector<int> pf_cols[2][3];
+  {
+    const int sec_off[2][4] = {{c->cond_off_enc, c->cond_off_fsrc, c->cond_off_ftgt, c->cond_off_dec},
+                               {c->cond_off_enc_tc, c->cond_off_fsrc_tc, c->cond_off_ftgt_tc, c->cond_off_dec}};
+    const int sec_len[4] = {c->cond_off_fsrc - c->cond_off_enc, c->cond_off_ftgt - c->cond_off_fsrc,
+                            c->cond_off_enc_tc - c->cond_off_ftgt, 512};
+    for (int o = 0; o < 2; ++o)
+      for (int m = 1; m <= 3; ++m) {
+        std::vector<int>& cols = pf_cols[o][m - 1];
+        for (int sec = 0; sec < 4; ++sec) {
+          const int sl = sel[sec_off[o][sec]];
+          c->cond_pf_off[o][m - 1][sec] = -1;
+          if (sl == 0 || !(m & sl)) continue;
+          c->cond_pf_off[o][m - 1][sec] = (int)cols.size();
+          for (int i = 0; i < sec_len[sec]; ++i) cols.push_back(sec_off[o][sec] + i);
+        }
+        c->cond_pf_cols[o][m - 1] = (int)cols.size();
+      }
+    // cond_kernel reads one side per CTA: every aligned block of COND_ROWS output columns must read the same side
+    auto uniform = [&](const std::vector<int>& cols, int n) {
+      auto col = [&](int i) { return cols.empty() ? i : cols[i]; };
+      for (int i = 0; i < n; ++i)
+        if (sel[col(i)] != sel[col(i / COND_ROWS * COND_ROWS)]) return false;
+      return true;
+    };
+    bool ok = uniform({}, (int)sel.size());
+    for (auto& oc : pf_cols)
+      for (auto& cols : oc) ok = ok && uniform(cols, (int)cols.size());
+    if (!ok) return fail(OVC_ERR_INVALID, "conditioning sections are not aligned to %d rows", COND_ROWS);
+  }
   // ---- ReferenceEncoder (optional: only extract_se needs it; models.py:301-338)
   c->has_refenc = false;
   if (find(c, "ref_enc.proj.weight")) {
@@ -668,6 +705,14 @@ static int finalize(ovc_ctx* c) {
   CK(cudaMalloc(&c->d_cond_sel, sel.size() * sizeof(int)));
   CK(cudaMemcpy(c->d_cond_wrow, wrow.data(), wrow.size() * sizeof(int), cudaMemcpyHostToDevice));
   CK(cudaMemcpy(c->d_cond_sel, sel.data(), sel.size() * sizeof(int), cudaMemcpyHostToDevice));
+  for (int o = 0; o < 2; ++o)
+    for (int m = 0; m < 3; ++m) {
+      if (c->d_cond_cols[o][m]) cudaFree(c->d_cond_cols[o][m]);
+      c->d_cond_cols[o][m] = nullptr;
+      if (pf_cols[o][m].empty()) continue;
+      CK(cudaMalloc(&c->d_cond_cols[o][m], pf_cols[o][m].size() * sizeof(int)));
+      CK(cudaMemcpy(c->d_cond_cols[o][m], pf_cols[o][m].data(), pf_cols[o][m].size() * sizeof(int), cudaMemcpyHostToDevice));
+    }
   if (!c->d_tw) {
     std::vector<float2> tw(STFT_N);
     std::vector<float> win(STFT_N);
@@ -694,16 +739,18 @@ static int finalize(ovc_ctx* c) {
 // ---------------------------------------------------------------------------------------------
 struct WsLayout {
   int P;   // frame pitch (multiple of 4)
-  size_t cond, x, skip, acts, z, dpre, bufA, bufB, bufC, bufD, bufE, bufF, spec, frames, win_g, win_len, total;
+  size_t cond, cond_pf, x, skip, acts, z, dpre, bufA, bufB, bufC, bufD, bufE, bufF, spec, frames, win_g, win_len, total;
   size_t brB[2], brC[2];   // per-branch ResBlock buffers of the concurrent-branch mode (small calls only)
   bool branches;
 };
-static WsLayout ws_layout(const ovc_ctx* c, int B, int Tmax) {
+// pf_cols: columns of the per-frame conditioning vector (0: every embedding is per item, no per-frame buffer)
+static WsLayout ws_layout(const ovc_ctx* c, int B, int Tmax, int pf_cols = 0) {
   WsLayout L;
   L.P = (int)round_up((size_t)Tmax, 4);
   size_t o = 0;
   auto take = [&](size_t n) { size_t r = o; o = round_up(o + n, 64); return r; };
   L.cond = take((size_t)B * c->cond_rows_out);
+  L.cond_pf = pf_cols ? take((size_t)B * Tmax * pf_cols) : 0;
   L.x = take((size_t)B * 192 * L.P);
   L.skip = take((size_t)B * 192 * L.P);
   L.acts = take((size_t)B * 192 * L.P);
@@ -838,7 +885,7 @@ static const char* variant_name(int v) {
 struct TcExtra {
   int epi = 0;                    // 0 linear, 1 WN gate, 2 WN res/skip
   const float* bias = nullptr;    // override (per-utterance conditioning vector), with stride
-  long long bias_bs = 0;
+  long long bias_bs = 0, bias_ts = 0;
   float* s = nullptr;             // skip accumulator (EPI 2)
   int split = 0, first = 0;
   int y_ld = 0;                   // output row width when it differs from Ntot
@@ -869,7 +916,7 @@ static int launch_tc(Run& r, const TcLayer& T, const float* x, float* y, const f
   const int y_ld = ex.y_ld ? ex.y_ld : T.Ntot;
   a.x = x; a.x_bs = (long long)T.Cin * r.P * mul;
   a.w = reinterpret_cast<const uint16_t*>(r.c->d_tcw + T.w_off);
-  a.bias = ex.bias ? ex.bias : r.c->d_tcw + T.b_off; a.bias_bs = ex.bias_bs;
+  a.bias = ex.bias ? ex.bias : r.c->d_tcw + T.b_off; a.bias_bs = ex.bias_bs; a.bias_ts = ex.bias_ts;
   a.y = y; a.y_bs = (long long)y_ld * r.P * mul; a.y_ld = y_ld;
   a.r = res;
   a.s = ex.s; a.s_bs = a.y_bs;
@@ -941,15 +988,21 @@ static int launch_transpose(Run& r, const float* src, float* dst, int rows, int 
   return OVC_OK;
 }
 
+// where a conditioned layer reads its vector: item b, frame t, column n at p + b * bs + min(t, Tmax - 1) * ts + n
+struct CondRef {
+  const float* p; long long bs, ts;
+  CondRef at(int col) const { return {p + col, bs, ts}; }
+};
+
 // one WN stack (modules.py:185-210): x <- in place, skip <- output
-static int run_wn(Run& r, const WNLayers& wn, float* x, float* skip, float* acts, const float* cond, int cond_bs) {
+static int run_wn(Run& r, const WNLayers& wn, float* x, float* skip, float* acts, const CondRef& cond) {
   const int P = r.P, T = r.Tmax;
   const long long bs = 192LL * P;
   const int n = (int)wn.in.size();
   for (int i = 0; i < n; ++i) {
     ConvArgs a{};
     a.x = x; a.x_bs = bs; a.x_pitch = P;
-    a.bias = cond + (size_t)i * 384; a.bias_bs = cond_bs;
+    a.bias = cond.p + (size_t)i * 384; a.bias_bs = cond.bs; a.bias_ts = cond.ts;
     a.y = acts; a.y_bs = bs; a.y_pitch = P;
     a.lens_in = r.lens; a.lens_out = r.lens; a.mul_in = 1; a.mul_out = 1;
     a.slope = 1.f;
@@ -971,13 +1024,14 @@ static int run_wn(Run& r, const WNLayers& wn, float* x, float* skip, float* acts
 // the same stack on the tensor cores: x, acts, skip live channels-last inside the stack; h comes in and the
 // output leaves in the [C][T] layout of the small FFMA kernels around it (pre / proj / post)
 static int run_wn_tc(Run& r, const WNLayers& wn, float* x, float* skip, float* acts, float* x_cl, float* skip_cl,
-                     const float* cond_tc, int cond_bs) {
+                     const CondRef& cond_tc) {
   const int P = r.P, T = r.Tmax;
   const int n = (int)wn.tc_in.size();
   TRY(launch_transpose(r, x, x_cl, 192, P));
   for (int i = 0; i < n; ++i) {
     TcExtra g;
-    g.epi = 1; g.bias = cond_tc + (size_t)i * 384; g.bias_bs = cond_bs; g.y_ld = 192; g.use_lens_frames = true;
+    g.epi = 1; g.bias = cond_tc.p + (size_t)i * 384; g.bias_bs = cond_tc.bs; g.bias_ts = cond_tc.ts; g.y_ld = 192;
+    g.use_lens_frames = true;
     TRY(launch_tc(r, wn.tc_in[i], x_cl, acts, nullptr, T, 1, 1.f, 1.f, 0, 0, g));
     TcExtra q;
     q.epi = 2; q.s = skip_cl; q.split = (i < n - 1) ? 192 : 0; q.first = (i == 0); q.y_ld = 192; q.use_lens_frames = true;
@@ -987,7 +1041,9 @@ static int run_wn_tc(Run& r, const WNLayers& wn, float* x, float* skip, float* a
   return OVC_OK;
 }
 
-static int run_flow(Run& r, const WsLayout& W, float* ws, bool reverse, const float* cond_all) {
+// cond: the conditioning of this direction's couplings (flow src forward, flow tgt in reverse), in the column order of
+// the precision mode
+static int run_flow(Run& r, const WsLayout& W, float* ws, bool reverse, const CondRef& cond) {
   ovc_ctx* c = r.c;
   const int P = r.P, T = r.Tmax;
   const long long bs = 192LL * P;
@@ -995,7 +1051,6 @@ static int run_flow(Run& r, const WsLayout& W, float* ws, bool reverse, const fl
   float* x = ws + W.x;
   float* skip = ws + W.skip;
   float* acts = ws + W.acts;
-  const int sect = reverse ? c->cond_off_ftgt : c->cond_off_fsrc;
   for (int step = 0; step < 4; ++step) {
     const int f = reverse ? 3 - step : step;
     const bool flipped = f & 1;
@@ -1008,10 +1063,9 @@ static int run_flow(Run& r, const WsLayout& W, float* ws, bool reverse, const fl
     a.slope = 1.f; a.scale = 1.f;
     TRY(launch(r, c->flow_pre[f], a, T));
     if (c->precision >= 1) {
-      const int sect_tc = reverse ? c->cond_off_ftgt_tc : c->cond_off_fsrc_tc;
-      TRY(run_wn_tc(r, c->flow_wn[f], x, skip, acts, ws + W.bufA, ws + W.bufB, cond_all + sect_tc + f * 4 * 384, c->cond_rows_out));
+      TRY(run_wn_tc(r, c->flow_wn[f], x, skip, acts, ws + W.bufA, ws + W.bufB, cond.at(f * 4 * 384)));
     } else {
-      TRY(run_wn(r, c->flow_wn[f], x, skip, acts, cond_all + sect + f * 4 * 384, c->cond_rows_out));
+      TRY(run_wn(r, c->flow_wn[f], x, skip, acts, cond.at(f * 4 * 384)));
     }
     // post + coupling update of x1 in place                                (modules.py:441-454)
     ConvArgs b{};
@@ -1136,6 +1190,31 @@ static int ensure_ws(ovc_ctx* c, const WsLayout& W, int B, int Tmax, cudaStream_
   return OVC_OK;
 }
 
+// one side of a cond_kernel launch: [B][gin] per item, or [B][gin][Tmax] per frame
+struct CondSide { const float* g; long long bs, cs, fs; };
+static CondSide cond_side(const ovc_ctx* c, const float* g, bool per_frame, int Tmax) {
+  const long long G = c->hp.gin_channels;
+  return per_frame ? CondSide{g, G * Tmax, Tmax, 1} : CondSide{g, G, 1, 0};
+}
+
+// every speaker-conditioning 1x1 conv in one launch: the stacked list (cols NULL, n_out = cond_rows_out) or the
+// per-frame columns `cols`, for `frames` frames of each of B items
+static int launch_cond(ovc_ctx* c, cudaStream_t st, int B, int frames, const int* cols, int n_out, const CondSide& src,
+                       const CondSide& tgt, float* out, long long out_bs, long long out_fs) {
+  CondArgs a;
+  a.w = c->d_w + c->cond_w_off; a.bias = c->d_w + c->cond_b_off;
+  a.w_row = c->d_cond_wrow; a.sel = c->d_cond_sel; a.cols = cols;
+  a.g_src = src.g; a.src_bs = src.bs; a.src_cs = src.cs; a.src_fs = src.fs;
+  a.g_tgt = tgt.g; a.tgt_bs = tgt.bs; a.tgt_cs = tgt.cs; a.tgt_fs = tgt.fs;
+  a.out = out; a.out_bs = out_bs; a.out_fs = out_fs;
+  a.n_out = n_out; a.gin = c->hp.gin_channels; a.frames = frames;
+  dim3 grid((n_out + COND_ROWS - 1) / COND_ROWS, B, (frames + COND_FCHUNK - 1) / COND_FCHUNK);
+  cond_kernel<<<grid, 256, 0, st>>>(a);
+  CK(cudaGetLastError());
+  c->launches++;
+  return OVC_OK;
+}
+
 // z (workspace, [B][192][P]) -> a caller tensor [B][192][Tmax], zero past each length
 static int copy_latent_out(Run& r, const WsLayout& W, float* ws, float* dst) {
   if (!dst) return OVC_OK;
@@ -1147,7 +1226,7 @@ static int copy_latent_out(Run& r, const WsLayout& W, float* ws, float* dst) {
 }
 
 // HiFi-GAN generator on the latent in ws.z (models.py:272-291): shared by voice_conversion and the TTS decode
-static int run_dec(Run& r, const WsLayout& W, float* ws, const float* cond, const long long* lens, float* o_hat) {
+static int run_dec(Run& r, const WsLayout& W, float* ws, const CondRef& cond, const long long* lens, float* o_hat) {
   ovc_ctx* c = r.c;
   cudaStream_t st = r.st;
   const int B = r.B, Tmax = r.Tmax, P = W.P;
@@ -1157,7 +1236,7 @@ static int run_dec(Run& r, const WsLayout& W, float* ws, const float* cond, cons
   if (!pre_tc) {
     ConvArgs a{};
     a.x = ws + W.z; a.x_bs = bs192; a.x_pitch = P;
-    a.bias = cond + c->cond_off_dec; a.bias_bs = c->cond_rows_out;
+    a.bias = cond.p; a.bias_bs = cond.bs; a.bias_ts = cond.ts;
     a.y = ws + W.dpre; a.y_bs = 512LL * P; a.y_pitch = P;
     a.lens_in = lens;          // z_hat * y_mask
     a.lens_out = r.glens; a.mul_in = 1; a.mul_out = 1;
@@ -1182,7 +1261,7 @@ static int run_dec(Run& r, const WsLayout& W, float* ws, const float* cond, cons
       // bufE; the input is cut at the frame lengths (z_hat * y_mask), the output runs over the generator's own limit
       TRY(launch_transpose(r, ws + W.z, bufA, 192, P));
       TcExtra e;
-      e.bias = cond + c->cond_off_dec; e.bias_bs = c->cond_rows_out;
+      e.bias = cond.p; e.bias_bs = cond.bs; e.bias_ts = cond.ts;
       e.lens_x = lens; e.has_lens_x = lens != nullptr;
       TRY(launch_tc(r, c->tc_pre, bufA, bufE, nullptr, Tmax, 1, 1.f, 1.f, 0, 0, e));
       TRY(tap_cl("dec.pre", bufE, 512, Tmax, P));
@@ -1335,10 +1414,16 @@ static int run_dec(Run& r, const WsLayout& W, float* ws, const float* cond, cons
   return OVC_OK;
 }
 
+static int cond_pf_cols(const ovc_ctx* c, int se_frames) {
+  return se_frames ? c->cond_pf_cols[c->precision >= 1][se_frames - 1] : 0;
+}
+
+// se_frames: OVC_SE_FRAMES_SRC / _TGT bits, the sides given per frame ([B][gin][Tmax]) rather than per item ([B][gin])
 static int run_vc(ovc_ctx* c, const float* spec, int spec_pitch, const long long* lens, const float* g_src, const float* g_tgt,
-                  const float* noise, uint64_t seed, float tau, int B, int Tmax, int ragged, float* o_hat,
+                  int se_frames, const float* noise, uint64_t seed, float tau, int B, int Tmax, int ragged, float* o_hat,
                   float* z_out, float* zp_out, float* zh_out, cudaStream_t st) {
-  const WsLayout W = ws_layout(c, B, Tmax);
+  const int n_pf = cond_pf_cols(c, se_frames);
+  const WsLayout W = ws_layout(c, B, Tmax, n_pf);
   TRY(ensure_ws(c, W, B, Tmax, st));
   float* ws = c->d_ws;
   Run r{c, st, B, Tmax, W.P, lens, ragged ? lens : nullptr, (double)B * Tmax};
@@ -1346,20 +1431,25 @@ static int run_vc(ovc_ctx* c, const float* spec, int spec_pitch, const long long
   const int P = W.P;
   const long long bs192 = 192LL * P;
 
-  // ---- every speaker-conditioning 1x1 conv in one launch
-  {
-    CondArgs a;
-    a.w = c->d_w + c->cond_w_off; a.bias = c->d_w + c->cond_b_off;
-    a.w_row = c->d_cond_wrow; a.sel = c->d_cond_sel;
-    a.g_src = g_src; a.g_tgt = g_tgt; a.out = ws + W.cond;
-    a.rows_out = c->cond_rows_out; a.gin = c->hp.gin_channels;
-    dim3 grid((c->cond_rows_out + 7) / 8, B);
-    cond_kernel<<<grid, 256, 0, st>>>(a);
-    CK(cudaGetLastError());
-    c->launches++;
-  }
+  // ---- every speaker-conditioning 1x1 conv in one launch; with a time-varying side, a second launch computes the
+  // sections that read it for every frame (the per-item vectors of those sections then go unread)
+  const int o = c->precision >= 1;
+  const bool src_pf = se_frames & OVC_SE_FRAMES_SRC, tgt_pf = se_frames & OVC_SE_FRAMES_TGT;
+  TRY(launch_cond(c, st, B, 1, nullptr, c->cond_rows_out, cond_side(c, src_pf ? nullptr : g_src, false, Tmax),
+                  cond_side(c, tgt_pf ? nullptr : g_tgt, false, Tmax), ws + W.cond, c->cond_rows_out, 0));
+  if (n_pf)
+    TRY(launch_cond(c, st, B, Tmax, c->d_cond_cols[o][se_frames - 1], n_pf, cond_side(c, src_pf ? g_src : nullptr, true, Tmax),
+                    cond_side(c, tgt_pf ? g_tgt : nullptr, true, Tmax), ws + W.cond_pf, (long long)Tmax * n_pf, n_pf));
   const float* cond = ws + W.cond;
   TRY(tap(r, "cond", cond, 1, c->cond_rows_out, c->cond_rows_out));
+  const int sec[2][4] = {{c->cond_off_enc, c->cond_off_fsrc, c->cond_off_ftgt, c->cond_off_dec},
+                         {c->cond_off_enc_tc, c->cond_off_fsrc_tc, c->cond_off_ftgt_tc, c->cond_off_dec}};
+  CondRef cr[4];   // enc, flow src, flow tgt, dec
+  for (int k = 0; k < 4; ++k) {
+    const int pf = n_pf ? c->cond_pf_off[o][se_frames - 1][k] : -1;
+    cr[k] = pf < 0 ? CondRef{cond + sec[o][k], c->cond_rows_out, 0}
+                   : CondRef{ws + W.cond_pf + pf, (long long)Tmax * n_pf, n_pf};
+  }
 
   // ---- posterior encoder (models.py:212-221)
   {
@@ -1373,10 +1463,9 @@ static int run_vc(ovc_ctx* c, const float* spec, int spec_pitch, const long long
     TRY(launch(r, aligned ? c->enc_pre16 : c->enc_pre, a, Tmax));
     TRY(tap(r, "enc.pre", ws + W.x, 192, Tmax, P));
     if (c->precision >= 1) {
-      TRY(run_wn_tc(r, c->enc_wn, ws + W.x, ws + W.skip, ws + W.acts, ws + W.bufA, ws + W.bufB, cond + c->cond_off_enc_tc,
-                    c->cond_rows_out));
+      TRY(run_wn_tc(r, c->enc_wn, ws + W.x, ws + W.skip, ws + W.acts, ws + W.bufA, ws + W.bufB, cr[0]));
     } else {
-      TRY(run_wn(r, c->enc_wn, ws + W.x, ws + W.skip, ws + W.acts, cond + c->cond_off_enc, c->cond_rows_out));
+      TRY(run_wn(r, c->enc_wn, ws + W.x, ws + W.skip, ws + W.acts, cr[0]));
     }
     TRY(tap(r, "enc.wn", ws + W.skip, 192, Tmax, P));
     ConvArgs p{};
@@ -1392,12 +1481,12 @@ static int run_vc(ovc_ctx* c, const float* spec, int spec_pitch, const long long
   auto copy_latent = [&](float* dst) -> int { return copy_latent_out(r, W, ws, dst); };
   TRY(copy_latent(z_out));
   // ---- flow forward with g_src, reverse with g_tgt (models.py:496-497)
-  TRY(run_flow(r, W, ws, false, cond));
+  TRY(run_flow(r, W, ws, false, cr[1]));
   TRY(copy_latent(zp_out));
-  TRY(run_flow(r, W, ws, true, cond));
+  TRY(run_flow(r, W, ws, true, cr[2]));
   TRY(copy_latent(zh_out));
 
-  return run_dec(r, W, ws, cond, lens, o_hat);
+  return run_dec(r, W, ws, cr[3], lens, o_hat);
 }
 
 #include "ovc_tts_run.inc"    // run_tts_encode() / run_tts_decode(): SynthesizerTrn.infer on the device
@@ -1446,6 +1535,9 @@ void ovc_destroy(ovc_ctx* c) {
   if (c->d_tts) cudaFree(c->d_tts);
   if (c->d_cond_wrow) cudaFree(c->d_cond_wrow);
   if (c->d_cond_sel) cudaFree(c->d_cond_sel);
+  for (auto& oc : c->d_cond_cols)
+    for (int* p : oc)
+      if (p) cudaFree(p);
   if (c->d_tcw) cudaFree(c->d_tcw);
   if (c->d_re) cudaFree(c->d_re);
   for (auto& kv : c->rs_banks) cudaFree(kv.second);
@@ -1499,7 +1591,15 @@ int ovc_voice_conversion(ovc_ctx* c, const float* spec, const int64_t* lengths, 
 int ovc_voice_conversion_items(ovc_ctx* c, const float* spec, const int64_t* lengths, const float* g_src, const float* g_tgt,
                                const float* noise, uint64_t seed, float tau, int B, int Tmax, int ragged, float* o_hat,
                                float* z, float* z_p, float* z_hat, void* stream, const ovc_item_params* items) {
+  return ovc_voice_conversion_frames(c, spec, lengths, g_src, g_tgt, 0, noise, seed, tau, B, Tmax, ragged, o_hat, z, z_p, z_hat,
+                                     stream, items);
+}
+
+int ovc_voice_conversion_frames(ovc_ctx* c, const float* spec, const int64_t* lengths, const float* g_src, const float* g_tgt,
+                                int se_frames, const float* noise, uint64_t seed, float tau, int B, int Tmax, int ragged,
+                                float* o_hat, float* z, float* z_p, float* z_hat, void* stream, const ovc_item_params* items) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (se_frames & ~(OVC_SE_FRAMES_SRC | OVC_SE_FRAMES_TGT)) return fail(OVC_ERR_INVALID, "unknown se_frames bits 0x%x", se_frames);
   if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
   if (!spec || !lengths || !g_src || !g_tgt || !o_hat) return fail(OVC_ERR_INVALID, "null tensor argument");
   if (B < 1 || Tmax < 1) return fail(OVC_ERR_INVALID, "B and Tmax must be positive (got %d, %d)", B, Tmax);
@@ -1508,15 +1608,16 @@ int ovc_voice_conversion_items(ovc_ctx* c, const float* spec, const int64_t* len
   ON_DEVICE(c);
   c->ev_used = c->prof ? c->ev_used : 0;
   cudaStream_t st = (cudaStream_t)stream;
-  TRY(ensure_ws(c, ws_layout(c, B, Tmax), B, Tmax, st));
+  TRY(ensure_ws(c, ws_layout(c, B, Tmax, cond_pf_cols(c, se_frames)), B, Tmax, st));
   const ItemParams it = item_params(items);
   TRY(set_call_params(c, seed, tau, it, st));
   std::vector<uintptr_t> key = {1, (uintptr_t)spec, (uintptr_t)lengths, (uintptr_t)g_src, (uintptr_t)g_tgt, (uintptr_t)noise,
                                 (uintptr_t)o_hat, (uintptr_t)z, (uintptr_t)z_p, (uintptr_t)z_hat, (uintptr_t)B, (uintptr_t)Tmax,
-                                (uintptr_t)ragged, option_bits(c)};
+                                (uintptr_t)ragged, option_bits(c), (uintptr_t)se_frames};
   append_item_key(key, it);
   return run_graphed(c, key, st, [&](cudaStream_t s) {
-    return run_vc(c, spec, Tmax, (const long long*)lengths, g_src, g_tgt, noise, seed, tau, B, Tmax, ragged, o_hat, z, z_p, z_hat, s);
+    return run_vc(c, spec, Tmax, (const long long*)lengths, g_src, g_tgt, se_frames, noise, seed, tau, B, Tmax, ragged, o_hat, z,
+                  z_p, z_hat, s);
   });
 }
 
@@ -1574,7 +1675,14 @@ int ovc_convert_waveform(ovc_ctx* c, const float* wav, const int64_t* wav_length
 int ovc_convert_waveform_items(ovc_ctx* c, const float* wav, const int64_t* wav_lengths, int B, int Lmax, const float* g_src,
                                const float* g_tgt, const float* noise, uint64_t seed, float tau, float* o_hat, int64_t* frames,
                                void* stream, const ovc_item_params* items) {
+  return ovc_convert_waveform_frames(c, wav, wav_lengths, B, Lmax, g_src, g_tgt, 0, noise, seed, tau, o_hat, frames, stream, items);
+}
+
+int ovc_convert_waveform_frames(ovc_ctx* c, const float* wav, const int64_t* wav_lengths, int B, int Lmax, const float* g_src,
+                                const float* g_tgt, int se_frames, const float* noise, uint64_t seed, float tau, float* o_hat,
+                                int64_t* frames, void* stream, const ovc_item_params* items) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (se_frames & ~(OVC_SE_FRAMES_SRC | OVC_SE_FRAMES_TGT)) return fail(OVC_ERR_INVALID, "unknown se_frames bits 0x%x", se_frames);
   if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
   if (!wav || !wav_lengths || !g_src || !g_tgt || !o_hat) return fail(OVC_ERR_INVALID, "null tensor argument");
   const int Tmax = Lmax / c->hp.hop_length;
@@ -1582,22 +1690,41 @@ int ovc_convert_waveform_items(ovc_ctx* c, const float* wav, const int64_t* wav_
   if ((long long)Tmax * 256 * 64 > 2000000000LL) return fail(OVC_ERR_INVALID, "Lmax %d too large for 32-bit indexing", Lmax);
   ON_DEVICE(c);
   cudaStream_t st = (cudaStream_t)stream;
-  const WsLayout W = ws_layout(c, B, Tmax);
+  const WsLayout W = ws_layout(c, B, Tmax, cond_pf_cols(c, se_frames));
   TRY(ensure_ws(c, W, B, Tmax, st));
   const ItemParams it = item_params(items);
   TRY(set_call_params(c, seed, tau, it, st));
   std::vector<uintptr_t> key = {2, (uintptr_t)wav, (uintptr_t)wav_lengths, (uintptr_t)g_src, (uintptr_t)g_tgt, (uintptr_t)noise,
-                                (uintptr_t)o_hat, (uintptr_t)frames, (uintptr_t)B, (uintptr_t)Lmax, option_bits(c)};
+                                (uintptr_t)o_hat, (uintptr_t)frames, (uintptr_t)B, (uintptr_t)Lmax, option_bits(c),
+                                (uintptr_t)se_frames};
   append_item_key(key, it);
   return run_graphed(c, key, st, [&](cudaStream_t s) {
     float* spec = c->d_ws + W.spec;
     long long* fr = reinterpret_cast<long long*>(c->d_ws + W.frames);
     TRY(launch_stft(c, wav, wav_lengths, B, Lmax, Tmax, spec, W.P, fr, s));
     if (frames) CK(cudaMemcpyAsync(frames, fr, (size_t)B * sizeof(long long), cudaMemcpyDeviceToDevice, s));
-    const int rc = run_vc(c, spec, W.P, fr, g_src, g_tgt, noise, seed, tau, B, Tmax, 1, o_hat, nullptr, nullptr, nullptr, s);
+    const int rc = run_vc(c, spec, W.P, fr, g_src, g_tgt, se_frames, noise, seed, tau, B, Tmax, 1, o_hat, nullptr, nullptr,
+                          nullptr, s);
     c->launches += 1;
     return rc;
   });
+}
+
+int ovc_tone_track_expand(ovc_ctx* c, const int64_t* key_frame, const float* key_se, int64_t n_keys, const int64_t* key0,
+                          const int64_t* nkeys, const int64_t* frame0, const int64_t* frames, int B, int Tmax, float* out,
+                          void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (!key_frame || !key_se || !key0 || !nkeys || !frame0 || !frames || !out) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (n_keys < 1 || B < 1 || B > 65535 || Tmax < 1) return fail(OVC_ERR_INVALID, "bad sizes n_keys=%lld B=%d Tmax=%d", (long long)n_keys, B, Tmax);
+  const int G = c->hp.gin_channels;
+  if (G > 65535) return fail(OVC_ERR_INVALID, "gin_channels %d exceeds the grid limit", G);
+  ON_DEVICE(c);
+  dim3 grid((Tmax + 255) / 256, G, B);
+  tone_track_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const long long*)key_frame, key_se, (long long)n_keys,
+                                                            (const long long*)key0, (const long long*)nkeys,
+                                                            (const long long*)frame0, (const long long*)frames, G, Tmax, out);
+  CK(cudaGetLastError());
+  return OVC_OK;
 }
 
 // ovc_reference_encoder (lengths == nullptr: every item T frames) and ovc_reference_encoder_ragged

@@ -12,33 +12,142 @@ namespace ovc {
 // models.py:274-275) is a mat-vec.  All of them run in ONE launch: row `i` of the stacked,
 // pre-permuted matrix dotted with g_src / g_tgt / zeros (zero_g) of batch item b.  The bias of
 // the conv that consumes the result (in_layer / conv_pre) is pre-added on the host, so the conv
-// epilogues add a single per-(batch,row) vector.  One warp per output, warp-shuffle reduction.
+// epilogues add a single per-(batch,row) vector.
+//
+// Frames: an embedding may vary over time (reference: sid_src / sid_tgt of shape [B, gin, T]).
+// Side s of item b at frame f is g_s[b * bs + c * cs + f * fs] (fs = 0: one embedding per item),
+// and output column i of frame f goes to out[b * out_bs + f * out_fs + i].  A per-item call is the
+// one-frame case.  Every (frame, row) output is the same arithmetic whatever the call: lane l
+// accumulates fmaf over c = l, l + 32, ... from 0, then the 32 partials are summed by the xor
+// butterfly, plus the bias -- so a frame whose embedding equals a per-item one gets the bit-identical
+// vector.  A warp holds the 8 weights per lane of COND_RW rows in registers and sweeps the CTA's
+// frames, staged COND_FT at a time in shared memory; its COND_RW x COND_FW partial sums are reduced
+// in one transposed butterfly (each step exchanges half of the remaining values, lane l ends with
+// sum l, and every sum gets the additions of the plain xor tree, in the same pairing).
 // ---------------------------------------------------------------------------------------------
+constexpr int COND_GIN_MAX = 256;   // 8 weights per lane and row
+constexpr int COND_RW = 4, COND_FW = 8;   // COND_RW * COND_FW == 32 sums per butterfly
+constexpr int COND_ROWS = 8 * COND_RW;    // output columns of one CTA (8 warps); each CTA reads one side
+constexpr int COND_FT = 32;               // frames staged per pass
+constexpr int COND_FCHUNK = 256;          // frames of one CTA (blockIdx.z)
+static_assert(COND_RW * COND_FW == 32, "one butterfly reduces 32 sums");
+
 struct CondArgs {
   const float* w;        // [rows_w][gin]
-  const float* bias;     // [rows_out]
-  const int* w_row;      // [rows_out] matrix row feeding output row i
-  const int* sel;        // [rows_out] 0 = zeros, 1 = g_src, 2 = g_tgt
-  const float* g_src; const float* g_tgt;   // [B][gin]
-  float* out;            // [B][rows_out]
-  int rows_out; int gin;
+  const float* bias;     // [rows] of the stacked list
+  const int* w_row;      // [rows] matrix row feeding stacked row i
+  const int* sel;        // [rows] 0 = zeros, 1 = g_src, 2 = g_tgt; uniform over aligned blocks of COND_ROWS outputs
+  const int* cols;       // [n_out] stacked row of output column i; NULL = identity
+  const float* g_src; const float* g_tgt;   // a NULL side reads as zeros (the caller does not use its columns)
+  long long src_bs, src_cs, src_fs, tgt_bs, tgt_cs, tgt_fs;
+  float* out; long long out_bs, out_fs;
+  int n_out; int gin; int frames;
 };
 
-__global__ void __launch_bounds__(256) cond_kernel(const CondArgs a) {
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  const int b = blockIdx.y;
-  if (warp >= a.rows_out) return;
-  const int sel = a.sel[warp];
-  float s = 0.f;
-  if (sel != 0) {
-    const float* g = (sel == 1 ? a.g_src : a.g_tgt) + (size_t)b * a.gin;
-    const float* w = a.w + (size_t)a.w_row[warp] * a.gin;
-    for (int c = lane; c < a.gin; c += 32) s = fmaf(w[c], g[c], s);
+// one step of the transposed butterfly: of the 2H sums a lane holds, it keeps half (the upper half when lane bit H is
+// set) and adds its xor-H partner's partial of each kept sum
+template <int H>
+__device__ __forceinline__ void cond_fold(float (&acc)[32], int lane) {
+  const bool up = lane & H;
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  for (int p = 0; p < H; ++p) {
+    const float got = __shfl_xor_sync(0xffffffffu, up ? acc[p] : acc[p + H], H);
+    acc[p] = (up ? acc[p + H] : acc[p]) + got;
   }
-  if (lane == 0) a.out[(size_t)b * a.rows_out + warp] = s + a.bias[warp];
+}
+
+__global__ void __launch_bounds__(256) cond_kernel(const CondArgs a) {
+  __shared__ float gsm[COND_FT][COND_GIN_MAX + 1];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int b = blockIdx.y;
+  const int i_blk = blockIdx.x * COND_ROWS;
+  const int i0 = i_blk + warp * COND_RW;
+  const int sel = a.sel[a.cols ? a.cols[i_blk] : i_blk];   // block-uniform (host-checked)
+  const float* g = sel == 1 ? a.g_src : sel == 2 ? a.g_tgt : nullptr;
+  const bool live = g != nullptr;                           // block-uniform
+  const long long gcs = sel == 1 ? a.src_cs : a.tgt_cs, gfs = sel == 1 ? a.src_fs : a.tgt_fs;
+  if (live) g += (size_t)b * (sel == 1 ? a.src_bs : a.tgt_bs);
+  float w[COND_RW][COND_GIN_MAX / 32];
+#pragma unroll
+  for (int r = 0; r < COND_RW; ++r) {
+    const int i = min(i0 + r, a.n_out - 1);
+    const float* wr = a.w + (size_t)a.w_row[a.cols ? a.cols[i] : i] * a.gin;
+#pragma unroll
+    for (int k = 0; k < COND_GIN_MAX / 32; ++k) w[r][k] = (live && lane + 32 * k < a.gin) ? wr[lane + 32 * k] : 0.f;
+  }
+  const int fz0 = blockIdx.z * COND_FCHUNK, fz1 = min(a.frames, fz0 + COND_FCHUNK);
+  for (int f0 = fz0; f0 < fz1; f0 += COND_FT) {
+    const int nf = min(COND_FT, fz1 - f0);
+    const int nfp = (nf + COND_FW - 1) / COND_FW * COND_FW;
+    __syncthreads();
+    if (live)
+      for (int e = threadIdx.x; e < nfp * a.gin; e += blockDim.x) {
+        const int c = e / nfp, f = e % nfp;   // consecutive threads: consecutive frames of one channel
+        gsm[f][c] = f < nf ? g[(size_t)c * gcs + (size_t)(f0 + f) * gfs] : 0.f;
+      }
+    __syncthreads();
+    for (int fb = 0; fb < nf; fb += COND_FW) {
+      float acc[32];   // sum r * COND_FW + f
+#pragma unroll
+      for (int r = 0; r < COND_RW; ++r)
+#pragma unroll
+        for (int f = 0; f < COND_FW; ++f) {
+          float s = 0.f;
+#pragma unroll
+          for (int k = 0; k < COND_GIN_MAX / 32; ++k)
+            if (live && lane + 32 * k < a.gin) s = fmaf(w[r][k], gsm[fb + f][lane + 32 * k], s);
+          acc[r * COND_FW + f] = s;
+        }
+      cond_fold<16>(acc, lane);
+      cond_fold<8>(acc, lane);
+      cond_fold<4>(acc, lane);
+      cond_fold<2>(acc, lane);
+      cond_fold<1>(acc, lane);
+      const int i = i0 + lane / COND_FW, f = f0 + fb + lane % COND_FW;
+      if (i < a.n_out && f < f0 + nf)
+        a.out[(size_t)b * a.out_bs + (size_t)f * a.out_fs + i] = acc[0] + a.bias[a.cols ? a.cols[i] : i];
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// tone_track_kernel: per-frame embeddings from keyframe tracks.  Track b has keys [key0[b], key0[b] + nkeys[b]) of
+// (key_frame, key_se [gin]); out[b][c][t] = g_b(frame0[b] + t) for t < frames[b], zeros up to Tmax, where
+//   g(t) = se_0 before the first key, se_last from the last key on, and
+//   se_k + ((t - f_k) / (f_{k+1} - f_k)) * (se_{k+1} - se_k) for f_k <= t < f_{k+1}
+// in fp32 with every operation rounded on its own (no contraction), so a host statement of the rule reproduces it
+// bit for bit; of two keys at the same frame the later one holds from that frame on.  Descriptors are clamped here, so
+// no read leaves the key arrays whatever they hold.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float tone_track_at(const long long* kf, const float* kse, int n, int gin, int c, long long t) {
+  int lo = 0, hi = n;   // first key with frame > t
+  while (lo < hi) {
+    const int m = (lo + hi) >> 1;
+    if (kf[m] <= t) lo = m + 1; else hi = m;
+  }
+  if (lo == 0) return kse[c];
+  if (lo == n) return kse[(size_t)(n - 1) * gin + c];
+  const long long f0 = kf[lo - 1], f1 = kf[lo];
+  const float a = kse[(size_t)(lo - 1) * gin + c], d = __fsub_rn(kse[(size_t)lo * gin + c], a);
+  const float u = __fdiv_rn((float)(t - f0), (float)(f1 - f0));
+  return __fadd_rn(a, __fmul_rn(u, d));
+}
+
+__global__ void __launch_bounds__(256) tone_track_kernel(const long long* __restrict__ key_frame,
+                                                         const float* __restrict__ key_se, long long n_keys,
+                                                         const long long* __restrict__ key0,
+                                                         const long long* __restrict__ nkeys,
+                                                         const long long* __restrict__ frame0,
+                                                         const long long* __restrict__ frames, int gin, int Tmax,
+                                                         float* __restrict__ out) {
+  const int b = blockIdx.z, c = blockIdx.y;
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= Tmax || n_keys < 1) return;
+  const long long k0 = max(0LL, min(key0[b], n_keys - 1));
+  const int n = (int)max(1LL, min(nkeys[b], n_keys - k0));
+  const long long T = max(0LL, min(frames[b], (long long)Tmax));
+  const long long at = max(0LL, min(frame0[b], 1LL << 40)) + t;
+  out[((size_t)b * gin + c) * Tmax + t] = t < T ? tone_track_at(key_frame + k0, key_se + (size_t)k0 * gin, n, gin, c, at) : 0.f;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -57,6 +57,7 @@ struct TcConvArgs {
   float slope; float scale; int accumulate;
   int passes;   // 3: split precision (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo); 1: single-pass fp16 (11-bit operands, like cuDNN's TF32 default)
   const uint16_t* w2; const float* bias2;   // PAIR: conv 2 (Cin = Ntot = TN, dilation 1); x is also the residual
+  long long bias_ts;                   // per-frame conditioning: + min(t, tmax - 1) * bias_ts (0: one vector per item)
 };
 
 // Programmatic dependent launch (launch_tc sets the stream-serialization attribute): the NEXT kernel's CTAs may start
@@ -88,15 +89,19 @@ __device__ __forceinline__ float tc_result(const float (&d)[TN], bool two, int j
 // with the fragment layout of the MMA thread it stands in for, so both paths perform the same operations on the same
 // fp32 values.  Four consecutive threads cover 32 contiguous bytes of an output row, so every global access of a warp is
 // whole sectors.
-template <int TN, class V>
-__device__ __forceinline__ void tc_epilogue_v(const TcConvArgs& a, V v_at, int b, int t0, int n0, int lim, int row_a) {
+// PF: a per-frame conditioning vector (bias_ts != 0); tc_epilogue_v picks the instantiation, so a per-item call runs
+// the epilogue it always ran.
+template <int TN, bool PF, class V>
+__device__ __forceinline__ void tc_epilogue_body(const TcConvArgs& a, V v_at, int b, int t0, int n0, int lim, int row_a) {
   const int csub = (threadIdx.x & 3) * 2;
   float* yb = a.y + (size_t)b * a.y_bs;
   const float* rb = a.r ? a.r + (size_t)b * a.y_bs : nullptr;
   float* sb = a.s ? a.s + (size_t)b * a.s_bs : nullptr;
-  const float* bias = a.bias + (size_t)b * a.bias_bs;
   const int ta = t0 + row_a, tb = ta + 8;
   const bool oka = ta < lim, okb = tb < lim;
+  // rows ta and tb are different frames: with a per-frame conditioning vector each reads its own
+  const float* bias_a = a.bias + (size_t)b * a.bias_bs + (PF ? (size_t)min(ta, a.tmax - 1) * a.bias_ts : 0);
+  const float* bias_b = a.bias + (size_t)b * a.bias_bs + (PF ? (size_t)min(tb, a.tmax - 1) * a.bias_ts : 0);
 #pragma unroll
   for (int c0 = 0; c0 < TN; c0 += 32) {
     float v[16];
@@ -104,8 +109,9 @@ __device__ __forceinline__ void tc_epilogue_v(const TcConvArgs& a, V v_at, int b
     for (int i = 0; i < 16; ++i) v[i] = v_at(c0 / 2 + i);
 #pragma unroll
     for (int g = 0; g < 4; ++g) {
-      const float2 bq = __ldg(reinterpret_cast<const float2*>(bias + n0 + c0 + 8 * g + csub));
-      v[4 * g] += bq.x; v[4 * g + 1] += bq.y; v[4 * g + 2] += bq.x; v[4 * g + 3] += bq.y;
+      const float2 bq = __ldg(reinterpret_cast<const float2*>(bias_a + n0 + c0 + 8 * g + csub));
+      const float2 br = PF ? __ldg(reinterpret_cast<const float2*>(bias_b + n0 + c0 + 8 * g + csub)) : bq;
+      v[4 * g] += bq.x; v[4 * g + 1] += bq.y; v[4 * g + 2] += br.x; v[4 * g + 3] += br.y;
     }
     if (a.epi == 0) {
       // ---- linear: bias, residual, MRF accumulate, scale
@@ -166,6 +172,13 @@ __device__ __forceinline__ void tc_epilogue_v(const TcConvArgs& a, V v_at, int b
     }
   }
 }
+
+template <int TN, class V>
+__device__ __forceinline__ void tc_epilogue_v(const TcConvArgs& a, V v_at, int b, int t0, int n0, int lim, int row_a) {
+  if (a.bias_ts) tc_epilogue_body<TN, true>(a, v_at, b, t0, n0, lim, row_a);
+  else tc_epilogue_body<TN, false>(a, v_at, b, t0, n0, lim, row_a);
+}
+
 template <int TN>
 __device__ __forceinline__ void tc_epilogue(const TcConvArgs& a, const float (&d)[TN], int b, int t0, int n0, int lim, int row_a) {
   const bool two = a.passes == 3;
@@ -175,7 +188,7 @@ __device__ __forceinline__ void tc_epilogue(const TcConvArgs& a, const float (&d
 // t0 + R are the discarded output steps of the tile
 __device__ __forceinline__ TcConvArgs tc_pair_epilogue_args(const TcConvArgs& a, int TN) {
   TcConvArgs e = a;
-  e.y_ld = TN; e.r = a.x; e.bias = a.bias2; e.bias_bs = 0; e.epi = 0;
+  e.y_ld = TN; e.r = a.x; e.bias = a.bias2; e.bias_bs = 0; e.bias_ts = 0; e.epi = 0;
   return e;
 }
 

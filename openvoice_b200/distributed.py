@@ -101,13 +101,20 @@ def gather_waveforms(local: List[np.ndarray], local_idx: List[int], n_total: int
     return out  # type: ignore[return-value]
 
 
+def _check_per_item_se(src_se, tgt_se) -> None:
+    from .api import is_per_frame_se
+    if is_per_frame_se(src_se) or is_per_frame_se(tgt_se):
+        raise ValueError("sharded conversion takes one embedding per item, not a per-frame one or a ToneTrack")
+
+
 def convert_sharded(convert_fn: Callable[..., List[np.ndarray]], audios: Sequence[np.ndarray], src_se, tgt_se,
                     device: str = "cpu", **kw) -> Optional[List[np.ndarray]]:
     """Every rank holds the same utterance list; each converts its LPT shard with ``convert_fn``
     (normally ``ToneColorConverter.convert_batch``) and rank 0 receives all results in order.
     ``src_se`` / ``tgt_se``: one embedding for all items, or a per-item sequence.  A per-item ``seeds`` or ``tau``
     keyword follows its utterance into the shard that converts it (``convert_fn`` receives the shard's values), so with
-    ``seeds`` every result is independent of the world size."""
+    ``seeds`` every result is independent of the world size.  Embeddings that vary over time are refused (ValueError)."""
+    _check_per_item_se(src_se, tgt_se)
     rank, world = _world()
     shards = lpt_shard([len(a) for a in audios], world)
     mine = shards[rank]
@@ -163,8 +170,10 @@ def convert_sharded_async(converter, audios: Sequence[np.ndarray], src_se, tgt_s
     ONE device-to-device collective on a side stream, and rank ``dst`` alone downloads them.  Shapes of every
     rank's block follow from the shared list, so no size exchange is needed.  Returns at once; call ``.result()``.
     ``src_se`` / ``tgt_se``: one embedding for all items, or a per-item sequence.  ``tau`` (scalar or per item) and
-    ``seeds`` (one key per item) follow their utterance as in ``convert_sharded``."""
+    ``seeds`` (one key per item) follow their utterance as in ``convert_sharded``.  Embeddings that vary over time are
+    refused (ValueError)."""
     import torch
+    _check_per_item_se(src_se, tgt_se)
     rank, world = _world()
     hop = converter.hps.data.hop_length
     samples = [len(a) // hop * hop for a in audios]

@@ -134,6 +134,34 @@ class StreamingResampler:
         return self._emit(resample_span(self.sr_in, self.sr_out, self.n_in)[0], self.n_in)
 
 
+def retarget_track(track, f: int, new, ramp_frames: int = 0):
+    """The ``ToneTrack`` that follows ``track`` on frames < f and then moves to ``new``: hard at f (``ramp_frames`` 0),
+    else linearly from ``track``'s value at f to ``new`` at f + ramp_frames.  Frames < f keep ``track``'s values bit for
+    bit: the old keys before f stay, and where f falls inside a ramp of ``track`` its frames since the ramp's last key are
+    pinned by one key each (a key at every integer frame reproduces the values exactly)."""
+    from .api import ToneTrack
+    ramp = int(ramp_frames)
+    if ramp < 0 or int(f) < 0:
+        raise ValueError(f"retarget: frame {f} and ramp_frames {ramp_frames} must be >= 0")
+    new = torch.as_tensor(new, dtype=torch.float32).reshape(-1).cpu()
+    kf, kse = [int(v) for v in track.frames], track.se
+    keys = []
+    if f > 0:
+        i = sum(1 for v in kf if v < f)                   # old keys before f
+        keys = [(kf[k], kse[k]) for k in range(i)]
+        p = kf[i - 1] if i else f - 1
+        if 0 < i < len(kf):                               # inside a ramp: pin frames (p, f - 1] one by one
+            d = track.dense(f - 1 - p, p + 1)[0]
+            keys += [(p + 1 + t, d[:, t]) for t in range(f - 1 - p)]
+        elif p < f - 1 or not i:                          # holding a value: one key at f - 1 holds it to there
+            keys.append((f - 1, track.dense(1, f - 1)[0, :, 0]))
+    if ramp:
+        keys += [(f, track.dense(1, f)[0, :, 0]), (f + ramp, new)]
+    else:
+        keys.append((f, new))
+    return ToneTrack(keys)
+
+
 class StreamingConverter:
     def __init__(self, converter, src_se, tgt_se, tau: float = 0.3, window_frames: int = 256,
                  noise_fn: Optional[Callable[[int, int], torch.Tensor]] = None, seed: Optional[int] = None,
@@ -170,6 +198,7 @@ class StreamingConverter:
         self.dev = converter.device
         self.src = converter._stack_se(src_se, 1)
         self.tgt = converter._stack_se(tgt_se, 1)
+        self.tracks = {"src": None, "tgt": None}          # ToneTrack of a side once it has been retargeted
         if noise_fn is None and request_seed is None:
             gen = torch.Generator(device=self.dev)
             gen.manual_seed(int(seed if seed is not None else torch.randint(0, 2 ** 62, (1,)).item()))
@@ -224,16 +253,50 @@ class StreamingConverter:
             self.audio = self.audio[keep_from - self.a0:]
             self.a0 = keep_from
 
+    def _window_se(self, name: str, lo: int, hi: int):
+        """A side's embedding for the window's frames [lo, hi): [1, gin] where it is constant over them (the per-item
+        launch, as before any retarget), else [1, gin, hi - lo] expanded from its track at the window's absolute frames."""
+        tr = self.tracks[name]
+        if tr is None:
+            return self.src if name == "src" else self.tgt
+        if hi - 1 < tr.frames[0]:
+            return tr.se[:1].to(self.dev)
+        if lo >= tr.frames[-1]:
+            return tr.se[-1:].to(self.dev)
+        return self.conv._se_device([tr], [hi - lo], [lo], hi - lo, name)
+
+    @torch.no_grad()
+    def retarget(self, src_se=None, tgt_se=None, ramp_frames: int = 0) -> int:
+        """Change the stream's source and / or target embedding without closing it.  The change starts at frame f, the
+        first frame no window has read yet (the frames ready so far), and is hard (``ramp_frames`` 0) or linear over
+        ``ramp_frames`` frames (``retarget_track``).  Returns f.  The stream's output then equals ``convert`` on the whole
+        clip with ``tone_track(side)`` as that side's embedding, bit for bit.  A window that overlaps no transition runs
+        exactly the per-item launch.  ValueError for an embedding that is not one per item."""
+        assert not self.closed, "the stream has been flushed"
+        f = self.f0 + int(self.spec.shape[2])
+        for name, se in (("src", src_se), ("tgt", tgt_se)):
+            if se is not None:
+                new = self.conv._stack_se(se, 1)[0].cpu()
+                self.tracks[name] = retarget_track(self.tone_track(name), f, new, ramp_frames)
+        return f
+
+    def tone_track(self, name: str):
+        """The ``ToneTrack`` of side ``"src"`` or ``"tgt"`` over the whole stream so far."""
+        from .api import ToneTrack
+        tr = self.tracks[name]
+        return tr if tr is not None else ToneTrack([(0, (self.src if name == "src" else self.tgt)[0].cpu())])
+
     def _convert_window(self, lo: int, hi: int, e0: int, e1: int) -> np.ndarray:
         """Samples of frames [e0, e1): one ragged batch-1 call over the window's frames [lo, hi)."""
         sp = self.spec[:, :, lo - self.f0: hi - self.f0].contiguous()
         lens = torch.tensor([hi - lo], dtype=torch.int64, device=self.dev)
+        src, tgt = self._window_se("src", lo, hi), self._window_se("tgt", lo, hi)
         if self.request_seed is None:
             nz = self.noise[None, :, lo - self.f0: hi - self.f0].contiguous()
-            o, _, _ = self.conv.model.voice_conversion(sp, lens, self.src, self.tgt, tau=self.tau, noise=nz, ragged=True,
+            o, _, _ = self.conv.model.voice_conversion(sp, lens, src, tgt, tau=self.tau, noise=nz, ragged=True,
                                                        latents=False)
         else:
-            o, _, _ = self.conv.model.voice_conversion(sp, lens, self.src, self.tgt, tau=self.tau, ragged=True,
+            o, _, _ = self.conv.model.voice_conversion(sp, lens, src, tgt, tau=self.tau, ragged=True,
                                                        latents=False, seeds=[self.request_seed], frame0=[lo])
         out = o[0, 0, (e0 - lo) * self.hop: (e1 - lo) * self.hop].cpu().numpy().copy()
         self.emitted = e1
@@ -291,7 +354,7 @@ SESSION_BATCH_FRAMES = 32768
 
 
 class _Session:
-    __slots__ = ("row", "seed", "tau", "n_in", "emitted", "in_sr", "out_sr", "raw_n", "out_n")
+    __slots__ = ("row", "seed", "tau", "n_in", "emitted", "in_sr", "out_sr", "raw_n", "out_n", "se", "tracks")
 
     def __init__(self, row: int, seed: int, tau: float, in_sr: Optional[int] = None, out_sr: Optional[int] = None):
         self.row, self.seed, self.tau = row, seed, tau
@@ -300,6 +363,8 @@ class _Session:
         self.in_sr, self.out_sr = in_sr, out_sr           # rates of the pushed / returned audio; None: the model's
         self.raw_n = 0                                    # samples received at in_sr
         self.out_n = 0                                    # samples returned at out_sr
+        self.se = None                                    # [2, gin] host copy of the embedding table row
+        self.tracks = [None, None]                        # ToneTrack of the source / target once retargeted
 
 
 class StreamingSessions:
@@ -404,7 +469,7 @@ class StreamingSessions:
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None else check_seeds([seed], 1, "seed")[0]
         ses = []
         for name, se in (("src_se", src_se), ("tgt_se", tgt_se)):
-            se = torch.as_tensor(se, dtype=torch.float32).reshape(-1)
+            se = self._per_item_se(name, se)
             if se.numel() != self.gin:
                 raise ValueError(f"{name} has {se.numel()} values, the model's embeddings have {self.gin}")
             ses.append(se)
@@ -418,7 +483,62 @@ class StreamingSessions:
         sid = self.next_id
         self.next_id += 1
         self.sessions[sid] = _Session(row, seed, tau, sr["input_sr"], sr["output_sr"])
+        self.sessions[sid].se = torch.stack(ses)
         return sid
+
+    def retarget(self, sid: int, src_se=None, tgt_se=None, ramp_frames: int = 0) -> int:
+        """``StreamingConverter.retarget`` for session ``sid``: the change starts at the session's ready frames (the
+        first frame no window of it has read) and the call returns that frame; ``tone_track(sid, side)`` then gives the
+        whole-clip schedule, and the session equals ``StreamingConverter`` with the same retargets bit for bit.  A step
+        none of whose windows overlaps a transition runs exactly the launches it did before; one that has such windows
+        adds one tone-track expansion per varying side (after a small upload of the keys) and the per-frame conditioning
+        of that side's launches.  ValueError for an embedding that is not ``gin`` values."""
+        s = self.sessions[self._check_ids([sid])[0]]
+        f = ready_frames(s.n_in, self.hop, self.nfft, False)
+        for k, se in enumerate((src_se, tgt_se)):
+            if se is None:
+                continue
+            new = self._per_item_se(("src_se", "tgt_se")[k], se)
+            if new.numel() != self.gin:
+                raise ValueError(f"{('src_se', 'tgt_se')[k]} has {new.numel()} values, the model's embeddings have {self.gin}")
+            s.tracks[k] = retarget_track(self.tone_track(sid, ("src", "tgt")[k]), f, new, ramp_frames)
+            s.se[k] = new                                 # windows past the last key read the table as before
+            self.se[k, s.row] = new.to(self.dev)
+        return f
+
+    @staticmethod
+    def _per_item_se(name: str, se) -> torch.Tensor:
+        """One embedding as a flat host tensor; a ``ToneTrack`` is refused (a session's schedule changes by
+        ``retarget``)."""
+        from .api import ToneTrack
+        if isinstance(se, ToneTrack):
+            raise ValueError(f"{name} is a ToneTrack: a session takes one embedding per side and changes it with retarget")
+        return torch.as_tensor(se, dtype=torch.float32).reshape(-1)
+
+    def tone_track(self, sid: int, side: str):
+        """The ``ToneTrack`` of session ``sid``'s ``"src"`` or ``"tgt"`` embedding over its whole stream so far."""
+        from .api import ToneTrack
+        s = self.sessions[sid]
+        k = ("src", "tgt").index(side)
+        return s.tracks[k] if s.tracks[k] is not None else ToneTrack([(0, s.se[k].clone())])
+
+    def _window_tracks(self, ses, wins, b0: int, b1: int, Tmax: int, g):
+        """Per side, the [b1 - b0, gin, Tmax] per-frame embeddings of launch windows b0 .. b1 - 1 when one of them
+        overlaps a transition of that side (a track whose last key lies past the window's first frame), else the
+        gathered per-item rows g[side] (the launch is then exactly the per-item one)."""
+        out = []
+        for k in range(2):
+            var = [ses[i][1].tracks[k] is not None and lo < ses[i][1].tracks[k].frames[-1]
+                   for i, lo, _, _, _ in wins[b0:b1]]
+            if not any(var):
+                out.append(g[k][b0:b1])
+                continue
+            from .api import expand_tone_keys
+            entries = [ses[i][1].tracks[k] if v else ses[i][1].se[k] for v, (i, _, _, _, _) in zip(var, wins[b0:b1])]
+            buf = self._buf(f"gpf{k}", (b1 - b0) * self.gin * Tmax, torch.float32).view(b1 - b0, self.gin, Tmax)
+            out.append(expand_tone_keys(self.native, entries, [lo for _, lo, _, _, _ in wins[b0:b1]],
+                                        [hi - lo for _, lo, hi, _, _ in wins[b0:b1]], Tmax, buf, ("src_se", "tgt_se")[k]))
+        return out
 
     @property
     def rows_in_use(self) -> int:
@@ -709,7 +829,8 @@ class StreamingSessions:
                 b1 = min(B, b0 + per)
                 items = {"seed": d[4 * B + b0:4 * B + b1], "stream": d[5 * B + b0:5 * B + b1],
                          "frame0": d[B + b0:B + b1], "tau": taus[b0:b1]}
-                self.native.voice_conversion(spec[b0:b1], d[2 * B + b0:2 * B + b1], g[b0:b1], g[B + b0:B + b1],
+                gs, gt = self._window_tracks(ses, wins, b0, b1, Tmax, (g[:B], g[B:]))
+                self.native.voice_conversion(spec[b0:b1], d[2 * B + b0:2 * B + b1], gs, gt,
                                              ragged=True, latents=False, items=items,
                                              out=obuf[b0 * Tmax * hop:b1 * Tmax * hop])
             fo = 8 * B + nt
