@@ -25,14 +25,16 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 14 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 15 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
                                * 8: ovc_spectrogram_ring; 9: OVC_OPT_PAIR_OCC; 10: ovc_splice;
                                * 11: ovc_tts_encode_state_rows, ovc_tts_state_rows; 12: OVC_OPT_STAGED_EPI;
                                * 13: ovc_resample_plan, ovc_resample_rings;
-                               * 14: ovc_voice_conversion_frames, ovc_convert_waveform_frames, ovc_tone_track_expand */
+                               * 14: ovc_voice_conversion_frames, ovc_convert_waveform_frames, ovc_tone_track_expand;
+                               * 15: ovc_tts_encode_g, ovc_tts_encode_state_tokens, ovc_tts_decode_windows_tokens,
+                               *     ovc_tts_encode_state_rows_tokens, ovc_tts_state_rows_tokens */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -428,6 +430,46 @@ OVC_API int ovc_tts_decode_windows(ovc_ctx* ctx, const float* stats, const int32
                                    const int64_t* y_lengths, int N, int T, const int64_t* row, const int64_t* frame0,
                                    const int64_t* len, int W, int Wmax, const uint64_t* seed, const int64_t* stream,
                                    const float* noise_scale, float* o, float* z_p, void* cuda_stream);
+
+/* Speaking style from caller-supplied speaker vectors instead of emb_g(sid): blends of emb_g rows, or vectors that
+ * change from token to token (every conditioning layer of the reference's dp / sdp / flow / dec is a 1x1 conv added to
+ * per-token or per-frame activations, so each accepts g [B, gin, T]).
+ *
+ * ovc_tts_encode_g is ovc_tts_encode_items with `g` (device, fp32) in place of sid:
+ *   g_tokens 0   g [B][gin], one vector per row.  Everything after the encode is the sid path with g = that vector;
+ *                a row whose vector equals emb_g[id] gives the results of sid = id bit for bit.
+ *   g_tokens 1   g [B][gin][T] (ovc_tone_track_expand's layout), token t of row b at g[(b * gin + c) * T + t].  The
+ *                duration predictors add cond(g[b][:][t]) to token t (the same fmaf chain as the per-row vector, so a
+ *                token whose vector equals the row's gets bit-identical values).  The decode expands g along the
+ *                alignment path exactly as it expands m_p: frame y takes the vector of the token covering it, and
+ *                frames no token covers (past y_length) take 0.  The flow reverse and the generator are then
+ *                conditioned per frame; only their 6 656 target-side columns are computed per frame.
+ * The context keeps its own copy of g, so the caller may reuse the buffer after the call.  ovc_tts_decode(_items)
+ * needs nothing more.  Workspace: a per-token encode adds B * gin * T floats to the text-side workspace; its decode adds
+ * B * Ymax * (gin + 6 656) floats (the per-frame vectors and their conditioning columns) to the decode workspace.
+ *
+ * After a per-token encode ovc_tts_encode_state and ovc_tts_encode_state_rows fail with OVC_ERR_STATE (their g holds
+ * one vector per row); ovc_tts_encode_state_tokens copies the state with g [B][gin][T] instead, and fails with
+ * OVC_ERR_STATE after any other encode.  ovc_tts_encode_state_rows_tokens / ovc_tts_state_rows_tokens are the pool
+ * writes of ovc_tts_encode_state_rows / ovc_tts_state_rows with a per-token pool g [N][gin][Tp] (source g [B][gin][T]);
+ * tokens T <= t < Tp get g = 0, as their stats.  A checkpoint whose generator ignores g (zero_g) refuses per-token
+ * vectors with OVC_ERR_INVALID.  ovc_tts_decode_windows_tokens is ovc_tts_decode_windows on such state
+ * (g [N][gin][T], T as encoded): window w's frame frame0[w] + t gets the vector the whole decode gives that frame, and
+ * the same exactness rules hold.  Its workspace adds W * Wmax * (gin + 6 656) floats. */
+OVC_API int ovc_tts_encode_g(ovc_ctx* ctx, const int64_t* tokens, const int64_t* x_lengths, const float* g, int g_tokens,
+                             const float* noise_w, uint64_t seed, float noise_scale_w, float length_scale, float sdp_ratio,
+                             int B, int T, int64_t* y_lengths, float* w_ceil, float* logw, void* stream,
+                             const ovc_item_params* items);
+OVC_API int ovc_tts_encode_state_tokens(ovc_ctx* ctx, float* stats, int32_t* cum, float* g, void* stream);
+OVC_API int ovc_tts_encode_state_rows_tokens(ovc_ctx* ctx, const int64_t* dst_row, int N, int Tp, float* stats, int32_t* cum,
+                                             float* g, int64_t* y_lengths, void* stream);
+OVC_API int ovc_tts_state_rows_tokens(ovc_ctx* ctx, const float* stats, const int32_t* cum, const float* g,
+                                      const int64_t* y_lengths, int B, int T, const int64_t* dst_row, int N, int Tp,
+                                      float* d_stats, int32_t* d_cum, float* d_g, int64_t* d_y_lengths, void* stream);
+OVC_API int ovc_tts_decode_windows_tokens(ovc_ctx* ctx, const float* stats, const int32_t* cum, const float* g,
+                                          const int64_t* y_lengths, int N, int T, const int64_t* row, const int64_t* frame0,
+                                          const int64_t* len, int W, int Wmax, const uint64_t* seed, const int64_t* stream,
+                                          const float* noise_scale, float* o, float* z_p, void* cuda_stream);
 
 /* Arithmetic of the convolutions (generator ResBlocks = 90 % of the FLOPs, WaveNet stacks, upsamplers):
  *   0            fp32 FFMA on the CUDA cores

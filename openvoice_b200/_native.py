@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -25,6 +25,8 @@ EXPORTS = (
     "ovc_tts_encode_state", "ovc_tts_decode_windows", "ovc_spectrogram_ring", "ovc_splice",
     "ovc_tts_encode_state_rows", "ovc_tts_state_rows", "ovc_resample_plan", "ovc_resample_rings",
     "ovc_voice_conversion_frames", "ovc_convert_waveform_frames", "ovc_tone_track_expand",
+    "ovc_tts_encode_g", "ovc_tts_encode_state_tokens", "ovc_tts_decode_windows_tokens", "ovc_tts_encode_state_rows_tokens",
+    "ovc_tts_state_rows_tokens",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample / ovc_spectrogram_ring length of a stream that has not ended
@@ -167,13 +169,18 @@ def load_library(path: Optional[str] = None):
     lib.ovc_philox_normals.argtypes = [C.c_uint64, C.c_int64, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_void_p,
                                        C.c_void_p]
     lib.ovc_tts_encode_state.argtypes = [C.c_void_p] * 5
+    lib.ovc_tts_encode_state_tokens.argtypes = [C.c_void_p] * 5
+    lib.ovc_tts_encode_g.argtypes = lib.ovc_tts_encode.argtypes[:4] + [C.c_int] + lib.ovc_tts_encode.argtypes[4:] + [P]
     lib.ovc_tts_decode_windows.argtypes = ([C.c_void_p] * 5 + [C.c_int, C.c_int] + [C.c_void_p] * 3 + [C.c_int, C.c_int]
                                            + [C.c_void_p] * 6)
+    lib.ovc_tts_decode_windows_tokens.argtypes = lib.ovc_tts_decode_windows.argtypes
     lib.ovc_splice.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int,
                                C.c_int, C.c_void_p]
     lib.ovc_tts_encode_state_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 5
     lib.ovc_tts_state_rows.argtypes = ([C.c_void_p] * 5 + [C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
                                        + [C.c_void_p] * 5)
+    lib.ovc_tts_encode_state_rows_tokens.argtypes = lib.ovc_tts_encode_state_rows.argtypes
+    lib.ovc_tts_state_rows_tokens.argtypes = lib.ovc_tts_state_rows.argtypes
     lib.ovc_voice_conversion_frames.argtypes = (lib.ovc_voice_conversion.argtypes[:5] + [C.c_int]
                                                 + lib.ovc_voice_conversion.argtypes[5:] + [P])
     lib.ovc_convert_waveform_frames.argtypes = (lib.ovc_convert_waveform.argtypes[:7] + [C.c_int]
@@ -578,14 +585,21 @@ class NativeConverter:
         return dict(zip(keys, (int(v) for v in out)))
 
     def tts_encode(self, tokens, x_lengths, sid, noise_w=None, seed: int = 0, noise_scale_w: float = 1.0,
-                   length_scale: float = 1.0, sdp_ratio: float = 0.2, stream=None, items: Optional[dict] = None):
+                   length_scale: float = 1.0, sdp_ratio: float = 0.2, stream=None, items: Optional[dict] = None,
+                   g=None):
         """tokens [B,T] i64 cuda, x_lengths [B] i64 cuda, sid [B] i64 cuda, noise_w [B,2,T] or None (Philox).
         Returns (y_lengths [B] i64, w_ceil [B,T], logw [B,T]), all on the device; asynchronous on `stream`.
-        ``items``: per-item ``{"seed", "stream", "noise_scale_w", "length_scale", "sdp_ratio"}`` (``item_params``)."""
+        ``items``: per-item ``{"seed", "stream", "noise_scale_w", "length_scale", "sdp_ratio"}`` (``item_params``).
+        ``g``: speaker vectors instead of ``sid`` (which is then ignored), f32 cuda [B, gin] or per token [B, gin, T]
+        (include/ovc.h: ovc_tts_encode_g)."""
         import torch
-        for t in (tokens, x_lengths, sid):
+        for t in (tokens, x_lengths) + ((sid,) if g is None else ()):
             assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()
         B, T = tokens.shape
+        if g is not None:
+            gin = self.hp.gin_channels
+            assert g.is_cuda and g.dtype == torch.float32 and g.is_contiguous()
+            assert tuple(g.shape) in ((B, gin), (B, gin, T)), tuple(g.shape)
         if noise_w is not None:
             noise_w = noise_w.contiguous().float()
             assert tuple(noise_w.shape) == (B, 2, T)
@@ -595,10 +609,12 @@ class NativeConverter:
         st = stream if stream is not None else torch.cuda.current_stream(tokens.device)
         p = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
         it = item_params(items, B)
-        rc = self.lib.ovc_tts_encode_items(self.handle, p(tokens), p(x_lengths), p(sid), p(noise_w),
-                                           C.c_uint64(seed & (2 ** 64 - 1)), C.c_float(noise_scale_w),
-                                           C.c_float(length_scale), C.c_float(sdp_ratio), B, T, p(y_lengths), p(w_ceil),
-                                           p(logw), C.c_void_p(st.cuda_stream), _items_ref(it))
+        rest = (p(noise_w), C.c_uint64(seed & (2 ** 64 - 1)), C.c_float(noise_scale_w), C.c_float(length_scale),
+                C.c_float(sdp_ratio), B, T, p(y_lengths), p(w_ceil), p(logw), C.c_void_p(st.cuda_stream), _items_ref(it))
+        if g is None:
+            rc = self.lib.ovc_tts_encode_items(self.handle, p(tokens), p(x_lengths), p(sid), *rest)
+        else:
+            rc = self.lib.ovc_tts_encode_g(self.handle, p(tokens), p(x_lengths), p(g), 1 if g.dim() == 3 else 0, *rest)
         _check(self.lib, rc, "ovc_tts_encode")
         return y_lengths, w_ceil, logw
 
@@ -624,17 +640,19 @@ class NativeConverter:
         _check(self.lib, rc, "ovc_tts_decode")
         return o, lat
 
-    def tts_encode_state(self, B: int, T: int, device, stream=None):
+    def tts_encode_state(self, B: int, T: int, device, stream=None, per_token: bool = False):
         """Caller-owned copies of what the last ``tts_encode`` (B rows of T tokens) left in the context (include/ovc.h:
         ovc_tts_encode_state): (stats [B,T,2*inter] f32, cum [B,T] int32, g [B,gin] f32) on the device.  A later
-        ``tts_encode`` does not touch them.  Asynchronous on `stream`."""
+        ``tts_encode`` does not touch them.  ``per_token``: the encode took per-token vectors, and g is [B,gin,T]
+        (ovc_tts_encode_state_tokens).  Asynchronous on `stream`."""
         import torch
         stats = torch.empty(B, T, 2 * self.hp.inter_channels, device=device, dtype=torch.float32)
         cum = torch.empty(B, T, device=device, dtype=torch.int32)
-        g = torch.empty(B, self.hp.gin_channels, device=device, dtype=torch.float32)
+        g = torch.empty(B, self.hp.gin_channels, *((T,) if per_token else ()), device=device, dtype=torch.float32)
         st = stream if stream is not None else torch.cuda.current_stream(device)
-        rc = self.lib.ovc_tts_encode_state(self.handle, C.c_void_p(stats.data_ptr()), C.c_void_p(cum.data_ptr()),
-                                           C.c_void_p(g.data_ptr()), C.c_void_p(st.cuda_stream))
+        fn = self.lib.ovc_tts_encode_state_tokens if per_token else self.lib.ovc_tts_encode_state
+        rc = fn(self.handle, C.c_void_p(stats.data_ptr()), C.c_void_p(cum.data_ptr()), C.c_void_p(g.data_ptr()),
+                C.c_void_p(st.cuda_stream))
         _check(self.lib, rc, "ovc_tts_encode_state")
         return stats, cum, g
 
@@ -642,12 +660,16 @@ class NativeConverter:
         """Write encoded rows into rows ``dst_row`` (host ints) of a state pool (include/ovc.h: ovc_tts_encode_state_rows,
         ovc_tts_state_rows): stats [N,Tp,2*inter] f32, cum [N,Tp] int32, g [N,gin] f32, y_lengths [N] int64 on the device,
         written in place.  ``src``: None for the rows of the last ``tts_encode``, or caller-owned state (stats, cum, g,
-        y_lengths) of B rows.  Tokens past the source's pitch get the library's padding.  Asynchronous on `stream`."""
+        y_lengths) of B rows.  Tokens past the source's pitch get the library's padding.  A per-token pool has g
+        [N,gin,Tp] (its source g is [B,gin,T]; ovc_tts_encode_state_rows_tokens / ovc_tts_state_rows_tokens).
+        Asynchronous on `stream`."""
         import torch
         N, Tp = cum.shape
         dev = cum.device
+        per_token = g.dim() == 3
         for t, dt, shape in ((stats, torch.float32, (N, Tp, 2 * self.hp.inter_channels)), (cum, torch.int32, (N, Tp)),
-                             (g, torch.float32, (N, self.hp.gin_channels)), (y_lengths, torch.int64, (N,))):
+                             (g, torch.float32, (N, self.hp.gin_channels) + ((Tp,) if per_token else ())),
+                             (y_lengths, torch.int64, (N,))):
             assert t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, t.shape)
         st = stream if stream is not None else torch.cuda.current_stream(dev)
         # the row table goes up through a pinned buffer, reused once its previous upload has left it: no host sync
@@ -667,7 +689,8 @@ class NativeConverter:
             cache["ev"].record(st)
         p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
         if src is None:
-            rc = self.lib.ovc_tts_encode_state_rows(self.handle, p(rows), N, Tp, p(stats), p(cum), p(g), p(y_lengths),
+            fn = self.lib.ovc_tts_encode_state_rows_tokens if per_token else self.lib.ovc_tts_encode_state_rows
+            rc = fn(self.handle, p(rows), N, Tp, p(stats), p(cum), p(g), p(y_lengths),
                                                     C.c_void_p(st.cuda_stream))
         else:
             s_stats, s_cum, s_g, s_len = src
@@ -675,11 +698,13 @@ class NativeConverter:
             if len(dst_row) != B:
                 raise ValueError(f"tts_state_rows: {len(dst_row)} destination rows for {B} source rows")
             for t, dt, shape in ((s_stats, torch.float32, (B, T, 2 * self.hp.inter_channels)),
-                                 (s_cum, torch.int32, (B, T)), (s_g, torch.float32, (B, self.hp.gin_channels)),
+                                 (s_cum, torch.int32, (B, T)),
+                                 (s_g, torch.float32, (B, self.hp.gin_channels) + ((T,) if per_token else ())),
                                  (s_len, torch.int64, (B,))):
                 assert t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, t.shape)
-            rc = self.lib.ovc_tts_state_rows(self.handle, p(s_stats), p(s_cum), p(s_g), p(s_len), B, T, p(rows), N, Tp,
-                                             p(stats), p(cum), p(g), p(y_lengths), C.c_void_p(st.cuda_stream))
+            fn = self.lib.ovc_tts_state_rows_tokens if per_token else self.lib.ovc_tts_state_rows
+            rc = fn(self.handle, p(s_stats), p(s_cum), p(s_g), p(s_len), B, T, p(rows), N, Tp, p(stats), p(cum), p(g),
+                    p(y_lengths), C.c_void_p(st.cuda_stream))
         _check(self.lib, rc, "ovc_tts_state_rows")
         return stats, cum, g, y_lengths
 
@@ -690,7 +715,8 @@ class NativeConverter:
         ``noise_scale`` are host sequences of W values.  They are staged through slot ``slot``'s pinned and device
         buffers, and ``o`` is written into the slot's device buffer: with every address stable, a repeated (W, w_max)
         call is replayed from a CUDA graph with the new values.  Returns (o [W, hop * w_max], z_p [W, inter, w_max] or
-        None); ``o`` is overwritten by the next call on the slot.  Asynchronous on `stream`."""
+        None); ``o`` is overwritten by the next call on the slot.  A per-token ``g`` [N, gin, T]
+        (``tts_encode_state(per_token=True)``) decodes through ovc_tts_decode_windows_tokens.  Asynchronous on `stream`."""
         import numpy as np
         import torch
         W = len(row)
@@ -700,8 +726,10 @@ class NativeConverter:
                              f"{[len(v) for v in vals]}")
         N, T = cum.shape
         dev = cum.device
+        per_token = g.dim() == 3
         for t, dt, shape in ((stats, torch.float32, (N, T, 2 * self.hp.inter_channels)), (cum, torch.int32, (N, T)),
-                             (g, torch.float32, (N, self.hp.gin_channels)), (y_lengths, torch.int64, (N,))):
+                             (g, torch.float32, (N, self.hp.gin_channels) + ((T,) if per_token else ())),
+                             (y_lengths, torch.int64, (N,))):
             assert t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, t.shape)
         cache = self.__dict__.setdefault("_win_bufs", {})
         ev = cache.get(("ev", slot))
@@ -733,7 +761,8 @@ class NativeConverter:
         o = buf("o", W * hop * int(w_max), torch.float32).view(W, hop * int(w_max))
         zp = torch.empty(W, self.hp.inter_channels, int(w_max), device=dev, dtype=torch.float32) if latents else None
         p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
-        rc = self.lib.ovc_tts_decode_windows(
+        fn = self.lib.ovc_tts_decode_windows_tokens if per_token else self.lib.ovc_tts_decode_windows
+        rc = fn(
             self.handle, p(stats), p(cum), p(g), p(y_lengths), N, T, p(d_i[0:W]), p(d_i[W:2 * W]), p(d_i[2 * W:3 * W]), W,
             int(w_max), p(d_i[3 * W:4 * W]), p(d_i[4 * W:]), p(d_f), p(o), p(zp) if zp is not None else None,
             C.c_void_p(st.cuda_stream))

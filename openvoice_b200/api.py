@@ -291,7 +291,7 @@ def splice_table(runs: Sequence[Sequence[Tuple[int, int, int]]], pitch: int) -> 
 
 class TtsState(NamedTuple):
     """Encode state of ``NativeSynthesizer.tts_encode``, owned by the caller: device tensors stats [N,T,2*inter],
-    cum [N,T] int32, g [N,gin] and y_lengths [N], each row's decoded frames (host), and the decode key, stream and
+    cum [N,T] int32, g [N,gin] ([N,gin,T] after a per-token encode) and y_lengths [N], each row's decoded frames (host), and the decode key, stream and
     noise scale ``infer`` would draw each row's prior noise with."""
     stats: torch.Tensor
     cum: torch.Tensor
@@ -307,12 +307,25 @@ class TtsPool:
     """Encode state shared by the sentences of many live requests: device tensors stats [N,Tp,2*inter], cum [N,Tp] int32,
     g [N,gin] and y_lengths [N], grown on demand and never shrunk.  ``NativeSynthesizer.tts_encode(..., pool=, rows=)``
     writes an encode's rows into any rows of it (include/ovc.h: ovc_tts_encode_state_rows); a larger token pitch
-    re-pitches the rows already there once, with the library's padding.  The owner tracks which rows are live."""
+    re-pitches the rows already there once, with the library's padding.  The owner tracks which rows are live.
+
+    Once a per-token encode is written into it, the pool holds g per token, [N,gin,Tp], for good (``to_per_token``):
+    the rows already there keep their vector in every token column, later rows with one vector get it in every column,
+    and its windows decode through ovc_tts_decode_windows_tokens (bit-identical for a constant row)."""
 
     def __init__(self, native, device):
         self.native, self.device = native, torch.device(device)
         self.N = self.Tp = 0
         self.stats = self.cum = self.g = self.y_lengths = None
+        self.per_token = False
+
+    def to_per_token(self) -> None:
+        """Hold g per token from now on; each row's vector fills its token columns."""
+        if self.per_token:
+            return
+        self.per_token = True
+        if self.N:
+            self.g = self.g[:, :, None].expand(-1, -1, self.Tp).contiguous()
 
     def fit(self, N: int, T: int) -> None:
         """At least ``N`` rows at a pitch of at least ``T`` tokens; the rows already held keep their contents."""
@@ -323,7 +336,7 @@ class TtsPool:
         hp, dev = self.native.hp, self.device
         stats = torch.zeros(N2, Tp2, 2 * hp.inter_channels, device=dev)
         cum = torch.zeros(N2, Tp2, dtype=torch.int32, device=dev)
-        g = torch.zeros(N2, hp.gin_channels, device=dev)
+        g = torch.zeros(N2, hp.gin_channels, *((Tp2,) if self.per_token else ()), device=dev)
         y_lengths = torch.zeros(N2, dtype=torch.int64, device=dev)
         if self.N:
             self.native.tts_state_rows(range(self.N), stats, cum, g, y_lengths,
@@ -482,7 +495,8 @@ class NativeSynthesizer:
     @torch.no_grad()
     def infer(self, x, x_lengths, sid=None, noise_scale=1, length_scale=1, noise_scale_w=1.0, sdp_ratio=0.2,
               max_len=None, noise_w=None, noise=None, ragged: bool = False, seed: Optional[int] = None,
-              latents: bool = True, seeds: Optional[Sequence[int]] = None, streams: Optional[Sequence[int]] = None):
+              latents: bool = True, seeds: Optional[Sequence[int]] = None, streams: Optional[Sequence[int]] = None,
+              g=None):
         """(o, attn, y_mask, (z, z_p, None, None)) = SynthesizerTrn.infer (openvoice/models.py:467-490) for a V1
         base-speaker checkpoint.  ``x`` [B,T] token ids, ``x_lengths`` [B], ``sid`` [B] speaker ids.
         ``noise_w`` ([B,2,T]) / ``noise`` ([B,192,>=Ty]) replace the two random draws (models.py:173, 487); when None,
@@ -494,14 +508,19 @@ class NativeSynthesizer:
         ``sdp_ratio`` each take one value per item as well as a scalar; ``seeds`` gives item b its own key (the
         duration noise draws from ``seeds[b]``, the prior noise from ``seeds[b] + 1``, as a scalar ``seed`` does) at
         stream ``streams[b]`` (default: b).  Sentence j of a call with ``seed=s`` is reproduced in any batch by
-        ``seeds[i] = s, streams[i] = j`` and the same parameters."""
-        a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams)
+        ``seeds[i] = s, streams[i] = j`` and the same parameters.
+
+        ``g`` replaces ``sid`` with speaker vectors (include/ovc.h: ovc_tts_encode_g): [B or 1, gin(, 1)] one per row
+        (e.g. a blend of ``BaseSpeakerTTS.style`` rows), or [B or 1, gin, T] one per token.  Per token, the duration
+        predictors read token t's vector and the flow and generator read, at frame y, the vector of the token that
+        covers y (0 past the row's frames), as m_p is expanded."""
+        a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams, g)
         x, x_lengths, sid, seed, B = a["x"], a["x_lengths"], a["sid"], a["seed"], a["B"]
         noise_scale, enc_items, dec_items = a["noise_scale"], a["enc_items"], a["dec_items"]
         if noise_w is not None:
             noise_w = noise_w.to(self.device, torch.float32)
         y_lengths, w_ceil, _ = self.native.tts_encode(x, x_lengths, sid, noise_w=noise_w, seed=seed, items=enc_items,
-                                                      **a["enc_scalars"])
+                                                      g=a["g"], **a["enc_scalars"])
         Ty = int(y_lengths.max().item())                       # the sync
         if noise is not None:
             noise = noise.to(self.device, torch.float32)[:, :, :Ty].contiguous()
@@ -518,29 +537,31 @@ class NativeSynthesizer:
     @torch.no_grad()
     def infer_ragged(self, x, x_lengths, sid=None, noise_scale=1, length_scale=1, noise_scale_w=1.0, sdp_ratio=0.2,
                      seed: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
-                     streams: Optional[Sequence[int]] = None) -> Tuple[torch.Tensor, List[int]]:
+                     streams: Optional[Sequence[int]] = None, g=None) -> Tuple[torch.Tensor, List[int]]:
         """The audio of ``infer(..., ragged=True, latents=False)`` (same arguments and draws) left on the device, with
         each row's decoded frames on the host: (o [B, hop * max(frames)], frames).  Row b's samples are
         o[b, : hop * frames[b]], zeros after.  One host sync (y_lengths), as in ``infer``."""
-        a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams)
+        a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams, g)
         y_lengths, _, _ = self.native.tts_encode(a["x"], a["x_lengths"], a["sid"], seed=a["seed"], items=a["enc_items"],
-                                                 **a["enc_scalars"])
+                                                 g=a["g"], **a["enc_scalars"])
         frames = [int(v) for v in y_lengths.cpu()]             # the sync
         o, _ = self.native.tts_decode(a["B"], max(frames), self.device, seed=a["seed"] + 1,
                                       noise_scale=float(a["noise_scale"]), ragged=True, latents=False,
                                       items=a["dec_items"])
         return o[:, 0], frames
 
-    def check_tts_input(self, x, sid):
+    def check_tts_input(self, x, sid, need_sid: bool = True):
         """The token and speaker checks of ``infer`` / ``tts_encode``, before anything is launched: RuntimeError for a
         checkpoint without the TTS half, ValueError for a token id outside [0, n_vocab), a missing ``sid`` or a speaker id
         outside [0, n_speakers).  ``x``: int64 token ids (any shape, at least one); returns ``sid`` as a flat int64
-        tensor."""
+        tensor, or None without ``need_sid`` (speaker vectors given instead)."""
         info = self.native.tts_info()
         if not info["has_tts"]:
             raise RuntimeError("this checkpoint has no enc_p / dp / sdp / emb_g: infer() needs a V1 base speaker")
         if int(x.min()) < 0 or int(x.max()) >= info["n_vocab"]:
             raise ValueError(f"token ids must lie in [0, {info['n_vocab']})")
+        if not need_sid:
+            return None
         if sid is None:
             raise ValueError("sid is required (n_speakers > 0)")
         sid = sid.to(torch.int64).reshape(-1)
@@ -548,16 +569,40 @@ class NativeSynthesizer:
             raise ValueError(f"speaker ids must lie in [0, {info['n_speakers']})")
         return sid
 
-    def _tts_args(self, x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams):
-        """The checks and device inputs ``infer`` and ``tts_encode`` share: validated tokens, lengths and speakers on the
-        device, the call's key, the per-item parameter arrays of both halves, and each row's decode key, stream and
-        noise scale as host lists (what the whole decode draws row b with)."""
+    def check_tts_g(self, g, B: int, T: int) -> torch.Tensor:
+        """Speaker vectors for ``infer(g=...)`` as the library takes them: [B, gin] (one per row) or [B, gin, T] (one per
+        token; only a 3-D tensor with more than one column is per token).  A batch of 1 serves every row.  ValueError
+        for any other shape, before anything is launched."""
+        gin = self.native.hp.gin_channels
+        g = torch.as_tensor(g).to(self.device, torch.float32)
+        per_token = g.dim() == 3 and g.shape[-1] > 1
+        if per_token and (g.shape[1] != gin or g.shape[2] != T):
+            raise ValueError(f"per-token speaker vectors must be [B, {gin}, {T}] (gin, tokens), got {tuple(g.shape)}")
+        if not per_token:
+            if g.dim() not in (2, 3) or g.shape[1] != gin or g.numel() != g.shape[0] * gin:
+                raise ValueError(f"speaker vectors must be [B, {gin}] or [B, {gin}, 1], got {tuple(g.shape)}")
+            g = g.reshape(g.shape[0], gin)
+        if g.shape[0] == 1 and B > 1:
+            g = g.expand(B, *g.shape[1:])
+        if g.shape[0] != B:
+            raise ValueError(f"speaker vectors for {g.shape[0]} rows, the batch has {B}")
+        return g.contiguous()
+
+    def _tts_args(self, x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams,
+                  g=None):
+        """The checks and device inputs ``infer`` and ``tts_encode`` share: validated tokens, lengths and speakers (ids,
+        or vectors ``g``) on the device, the call's key, the per-item parameter arrays of both halves, and each row's
+        decode key, stream and noise scale as host lists (what the whole decode draws row b with)."""
         x = x.to(torch.int64)
-        sid = self.check_tts_input(x, sid)
+        if g is None:
+            sid = self.check_tts_input(x, sid)
+        else:
+            sid = self.check_tts_input(x, None, need_sid=False)
+            g = self.check_tts_g(g, x.shape[0], x.shape[1])
         x = x.to(self.device).contiguous()
         B, T = x.shape
         x_lengths = x_lengths.to(self.device, torch.int64).contiguous()
-        sid = sid.to(self.device).contiguous()
+        sid = sid.to(self.device).contiguous() if sid is not None else None
         seeds = check_seeds(seeds, B)
         if streams is not None:
             streams = [int(v) for v in streams]
@@ -579,7 +624,7 @@ class NativeSynthesizer:
             enc_items = {"seed": key, "stream": stream_d, "noise_scale_w": f32(nsw_b), "length_scale": f32(ls_b),
                          "sdp_ratio": f32(sr_b)}
             dec_items = {"seed": key1, "stream": stream_d, "noise_scale": f32(ns_b)}
-        return dict(x=x, x_lengths=x_lengths, sid=sid, seed=seed, B=B, noise_scale=noise_scale, enc_items=enc_items,
+        return dict(x=x, x_lengths=x_lengths, sid=sid, g=g, seed=seed, B=B, noise_scale=noise_scale, enc_items=enc_items,
                     dec_items=dec_items,
                     enc_scalars=dict(noise_scale_w=float(noise_scale_w), length_scale=float(length_scale),
                                      sdp_ratio=float(sdp_ratio)),
@@ -591,7 +636,7 @@ class NativeSynthesizer:
     def tts_encode(self, x, x_lengths, sid=None, noise_scale=1, length_scale=1, noise_scale_w=1.0, sdp_ratio=0.2,
                    seed: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
                    streams: Optional[Sequence[int]] = None, pool: Optional["TtsPool"] = None,
-                   rows: Optional[Sequence[int]] = None) -> "TtsState":
+                   rows: Optional[Sequence[int]] = None, g=None) -> "TtsState":
         """The encode half of ``infer`` (same arguments and draws), returning state the caller owns: a later
         ``tts_encode`` or ``infer`` does not change it.  ``tts_decode_windows`` decodes any frames of its rows, each
         row with the decode key, stream and noise scale ``infer`` would give it.  One host sync (y_lengths), as in
@@ -599,19 +644,33 @@ class NativeSynthesizer:
 
         ``pool`` / ``rows``: encoded row b is written into row ``rows[b]`` of ``pool`` instead (one
         ``ovc_tts_encode_state_rows``; the pool grows to fit first).  The returned state then holds the pool's tensors,
-        and its host lists (frames, decode keys, streams, noise scales) describe the encoded rows in order."""
-        a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams)
+        and its host lists (frames, decode keys, streams, noise scales) describe the encoded rows in order.
+
+        ``g`` as in ``infer``.  With per-token vectors the state's g is [B, gin, T] (include/ovc.h:
+        ovc_tts_encode_state_tokens), and a pool turns per-token (``TtsPool.to_per_token``).  Into a per-token pool,
+        rows with one vector (or a speaker id) are encoded with it in every token column, which gives the same
+        values."""
+        a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams, g)
         x = a["x"]
         B, T = x.shape
+        per_token = a["g"] is not None and a["g"].dim() == 3
+        if pool is not None and (per_token or pool.per_token):
+            if not per_token:
+                vec = a["g"]
+                if vec is None:
+                    vec = self._state_dict["emb_g.weight"].to(self.device, torch.float32)[a["sid"]]
+                a["g"] = vec[:, :, None].expand(-1, -1, T).contiguous()
+                per_token = True
+            pool.to_per_token()
         if pool is not None:
             rows = [int(r) for r in rows]
             if len(rows) != B or min(rows) < 0:
                 raise ValueError(f"tts_encode: {len(rows)} pool rows for {B} encoded rows (each >= 0)")
             pool.fit(max(rows) + 1, T)
         y_lengths, _, _ = self.native.tts_encode(x, a["x_lengths"], a["sid"], seed=a["seed"], items=a["enc_items"],
-                                                 **a["enc_scalars"])
+                                                 g=a["g"], **a["enc_scalars"])
         if pool is None:
-            stats, cum, g = self.native.tts_encode_state(B, T, self.device)
+            stats, cum, g = self.native.tts_encode_state(B, T, self.device, per_token=per_token)
         else:
             stats, cum, g, _ = self.native.tts_state_rows(rows, pool.stats, pool.cum, pool.g, pool.y_lengths)
         frames = [int(v) for v in y_lengths.cpu()]             # the sync
@@ -729,6 +788,78 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
         frontend = self.text_frontend or self._reference_frontend
         return frontend(text, mark)
 
+    def tokenize(self, text, language="English") -> List[List[int]]:
+        """The token-id lists (one per sentence, blanks included) that ``tts`` / ``tts_batch`` synthesise for ``text``:
+        where a per-token speaker places its keys.  Sentence j's tokens sit at positions [o_j, o_j + len(ids_j)) of the
+        request's token stream, o_j the earlier sentences' token count."""
+        return [list(q) for q in self._sentences(text, language)]
+
+    def style(self, name_or_id) -> torch.Tensor:
+        """The speaker vector [gin] (float32, host) of a style of the checkpoint, by name (``hps.speakers``, e.g.
+        "cheerful") or id: the emb_g row ``speaker=name_or_id`` conditions with.  Blends are tensor arithmetic, e.g.
+        ``speaker=0.7 * tts.style("cheerful") + 0.3 * tts.style("default")``."""
+        return self._emb_g()[self._speaker_id(name_or_id, "style")].clone()
+
+    def _emb_g(self) -> torch.Tensor:
+        return self.model._state_dict["emb_g.weight"].detach().to("cpu", torch.float32)
+
+    def _speaker_id(self, spk, who: str) -> int:
+        """A style name or id as an emb_g row; ValueError for an unknown name or an id outside the table."""
+        if isinstance(spk, str):
+            names = self.hps.get("speakers", {})
+            if spk not in names:
+                raise ValueError(f"{who}: unknown style {spk!r} (the checkpoint has {sorted(names)})")
+            return int(names[spk])
+        n = int(self.hps.data.n_speakers)
+        if not 0 <= int(spk) < n:
+            raise ValueError(f"{who}: speaker id {spk!r} is not in [0, {n})")
+        return int(spk)
+
+    def _speaker(self, spk, who: str):
+        """A request's ``speaker``: (id, None) for a name or an id (an id is range-checked by the encode, as before),
+        else (None, entry) with entry a [gin] vector, a ``ToneTrack`` over token positions or a [gin, N] per-token
+        tensor (host, float32).  ValueError names ``who``."""
+        if isinstance(spk, str):
+            return self._speaker_id(spk, who), None
+        gin = int(self.hps.model.gin_channels)
+        if isinstance(spk, ToneTrack):
+            if spk.se.shape[1] != gin:
+                raise ValueError(f"{who}: the ToneTrack's embeddings have {spk.se.shape[1]} values, the model's {gin}")
+            return None, spk
+        if not (torch.is_tensor(spk) or isinstance(spk, np.ndarray)) or np.ndim(spk) == 0:
+            return int(spk), None
+        e = torch.as_tensor(spk).detach().to("cpu", torch.float32)
+        if e.dim() == 3 and e.shape[0] == 1 and e.shape[1] == gin and e.shape[2] > 1:
+            return None, e[0].contiguous()
+        if e.numel() != gin:
+            raise ValueError(f"{who}: speaker embedding of shape {tuple(e.shape)} is not [{gin}], [1, {gin}, 1] or "
+                             f"[1, {gin}, N] (N = the request's tokens)")
+        return None, e.reshape(gin)
+
+    def _speaker_rows(self, rows, T: int) -> Optional[torch.Tensor]:
+        """Speaker vectors for sentences ``rows`` = [(id, entry, offset, tokens)] (``_speaker``; offset = o_j): None
+        when every row names an id (the emb_g path), [n, gin] when each has one vector, else [n, gin, T] per token
+        (zero past each sentence).  Per token, sentence j reads the ToneTrack at positions o_j + t
+        (``ToneTrack.dense``) or columns [o_j, o_j + n_j) of a per-token tensor; an id or a vector fills its row."""
+        if all(e is None for _, e, _, _ in rows):
+            return None
+        table = self._emb_g()
+        for i, e, _, _ in rows:
+            if e is None and not 0 <= i < table.shape[0]:       # the ids ride as emb_g rows: the encode's own check
+                raise ValueError(f"speaker ids must lie in [0, {table.shape[0]})")
+        vec = lambda i, e: table[i] if e is None else e  # noqa: E731
+        if not any(isinstance(e, ToneTrack) or (e is not None and e.dim() == 2) for _, e, _, _ in rows):
+            return torch.stack([vec(i, e) for i, e, _, _ in rows]).contiguous()
+        g = torch.zeros(len(rows), table.shape[1], T)
+        for b, (i, e, o, n) in enumerate(rows):
+            if isinstance(e, ToneTrack):
+                g[b, :, :n] = e.dense(n, o)[0]
+            elif e is not None and e.dim() == 2:
+                g[b, :, :n] = e[:, o:o + n]
+            else:
+                g[b, :, :n] = vec(i, e)[:, None]
+        return g
+
     @torch.no_grad()
     def tts_batch(self, requests: Sequence[dict]) -> List[np.ndarray]:
         """Many TTS requests in ONE ragged ``infer``, each with its own speaker, speed, seed and noise parameters.
@@ -749,34 +880,51 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
 
     def _request_sentences(self, reqs):
         """The sentences of ``tts_batch`` requests: (token-id lists, speaker ids, owning request, each request's speed,
-        the per-sentence ``infer`` keywords).  Sentence j of request r is keyed (seed_r, stream j) with r's parameters."""
-        seqs, sid, seeds, streams, owner = [], [], [], [], []
+        the per-sentence ``infer`` keywords).  Sentence j of request r is keyed (seed_r, stream j) with r's parameters.
+        When a request's speaker is an embedding or a track, the keywords carry ``g`` (``_speaker_rows``) for every
+        sentence and the speaker ids are placeholders."""
+        seqs, sid, seeds, streams, owner, rows = [], [], [], [], [], []
         par = {"noise_scale": [], "noise_scale_w": [], "length_scale": [], "sdp_ratio": []}
         speeds = []
         for r, q in enumerate(reqs):
-            ids = q["ids"] if "ids" in q else self._sentences(q["text"], q.get("language", "English"))
+            ids = [list(q_ids) for q_ids in (q["ids"] if "ids" in q else self._sentences(q["text"], q.get("language", "English")))]
             k = self._request_keys(q, f"request {r}")
+            self._check_speaker_tokens(k["g"], [len(q_ids) for q_ids in ids], f"request {r}")
             speeds.append(k["speed"])
+            o = 0
             for j, q_ids in enumerate(ids):
-                seqs.append(list(q_ids))
-                sid.append(k["speaker"])
+                seqs.append(q_ids)
+                sid.append(0 if k["speaker"] is None else k["speaker"])
+                rows.append((k["speaker"], k["g"], o, len(q_ids)))
+                o += len(q_ids)
                 seeds.append(k["seed"])
                 streams.append(j)
                 owner.append(r)
                 self._sentence_params(k, par)
-        return seqs, sid, owner, speeds, dict(seeds=seeds, streams=streams, **par)
+        kw = dict(seeds=seeds, streams=streams, **par)
+        g = self._speaker_rows(rows, max((len(q) for q in seqs), default=1))
+        if g is not None:
+            kw["g"] = g
+        return seqs, sid, owner, speeds, kw
+
+    @staticmethod
+    def _check_speaker_tokens(entry, lengths: Sequence[int], who: str) -> None:
+        """ValueError when a per-token speaker tensor's columns are not the request's token count."""
+        if torch.is_tensor(entry) and entry.dim() == 2 and entry.shape[1] != sum(lengths):
+            raise ValueError(f"{who}: the per-token speaker tensor has {entry.shape[1]} columns, the request "
+                             f"{sum(lengths)} tokens")
 
     def _request_keys(self, q, who: str) -> dict:
-        """The TTS keys of one request (all but its text), validated: speaker id, speed, seed (drawn from torch's
-        generator when absent) and the noise parameters.  ValueError names the request as ``who``."""
-        spk = q["speaker"]
-        spk = self.hps.speakers[spk] if isinstance(spk, str) else int(spk)
+        """The TTS keys of one request (all but its text), validated: speaker (``speaker``: an id or None; ``g``: None
+        or the embedding / track, ``_speaker``), speed, seed (drawn from torch's generator when absent) and the noise
+        parameters.  ValueError names the request as ``who``."""
+        spk, g = self._speaker(q["speaker"], who)
         speed = float(q.get("speed", 1.0))
         if not (math.isfinite(speed) and speed > 0):
             raise ValueError(f"{who}: speed {speed!r} must be a positive number")
         seed = q.get("seed")
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None else check_seeds([seed], 1, "seed")[0]
-        return dict(speaker=spk, speed=speed, seed=seed, noise_scale=float(q.get("noise_scale", 0.667)),
+        return dict(speaker=spk, g=g, speed=speed, seed=seed, noise_scale=float(q.get("noise_scale", 0.667)),
                     noise_scale_w=float(q.get("noise_scale_w", 0.6)), sdp_ratio=float(q.get("sdp_ratio", 0.2)))
 
     @staticmethod
@@ -865,13 +1013,22 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
                      seed: Optional[int] = None) -> List[np.ndarray]:
         """All sentences in ONE batched infer() (the reference loops over them at batch 1, api.py:79-91); every
         sentence gets what its own batch-1 call would give (ragged decode).  ``seed``: the call's key (sentence j
-        draws at stream j); default: one drawn from torch's global generator."""
-        speaker_id = self.hps.speakers[speaker] if isinstance(speaker, str) else int(speaker)
+        draws at stream j); default: one drawn from torch's global generator.  ``speaker``: a style name or id, a
+        speaker vector ([gin] or [1, gin, 1], e.g. a blend of ``style`` rows), a ``ToneTrack`` keyed in token positions
+        of the whole call (sentence j's tokens at [o_j, o_j + n_j)) or a [1, gin, N] per-token tensor with N the
+        call's token count; ValueError for anything else."""
+        sequences = [list(q) for q in sequences]
+        speaker_id, entry = self._speaker(speaker, "speaker")
+        self._check_speaker_tokens(entry, [len(q) for q in sequences], "speaker")
         n = len(sequences)
         if n == 0:      # the reference's loop over zero sentences yields no audio (api.py:79-91)
             return []
-        return self._infer_sentences(sequences, [speaker_id] * n, noise_scale=noise_scale, noise_scale_w=noise_scale_w,
-                                     length_scale=1.0 / speed, sdp_ratio=sdp_ratio, seed=seed)
+        offs = np.cumsum([0] + [len(q) for q in sequences]).tolist()
+        g = self._speaker_rows([(speaker_id, entry, offs[j], len(q)) for j, q in enumerate(sequences)],
+                               max(len(q) for q in sequences))
+        return self._infer_sentences(sequences, [0 if speaker_id is None else speaker_id] * n, noise_scale=noise_scale,
+                                     noise_scale_w=noise_scale_w, length_scale=1.0 / speed, sdp_ratio=sdp_ratio, seed=seed,
+                                     **({} if g is None else {"g": g}))
 
     def tts(self, text, output_path, speaker, language="English", speed=1.0, seed: Optional[int] = None):
         """openvoice/api.py:73-98.  ``seed``: the request's key (``tts_from_ids``); same seed, same audio."""

@@ -240,6 +240,7 @@ struct ovc_ctx {
   float* d_tts = nullptr;
   size_t tts_floats = 0;
   int tts_B = 0, tts_T = 0;
+  bool tts_gtok = false;   // the pending encode took per-token speaker vectors
 
   // profiling
   bool prof = false;
@@ -739,18 +740,20 @@ static int finalize(ovc_ctx* c) {
 // ---------------------------------------------------------------------------------------------
 struct WsLayout {
   int P;   // frame pitch (multiple of 4)
-  size_t cond, cond_pf, x, skip, acts, z, dpre, bufA, bufB, bufC, bufD, bufE, bufF, spec, frames, win_g, win_len, total;
+  size_t cond, cond_pf, g_pf, x, skip, acts, z, dpre, bufA, bufB, bufC, bufD, bufE, bufF, spec, frames, win_g, win_len, total;
   size_t brB[2], brC[2];   // per-branch ResBlock buffers of the concurrent-branch mode (small calls only)
   bool branches;
 };
-// pf_cols: columns of the per-frame conditioning vector (0: every embedding is per item, no per-frame buffer)
-static WsLayout ws_layout(const ovc_ctx* c, int B, int Tmax, int pf_cols = 0) {
+// pf_cols: columns of the per-frame conditioning vector (0: every embedding is per item, no per-frame buffer);
+// g_frames: also a [B][gin][Tmax] per-frame speaker embedding (the TTS decode after a per-token encode)
+static WsLayout ws_layout(const ovc_ctx* c, int B, int Tmax, int pf_cols = 0, bool g_frames = false) {
   WsLayout L;
   L.P = (int)round_up((size_t)Tmax, 4);
   size_t o = 0;
   auto take = [&](size_t n) { size_t r = o; o = round_up(o + n, 64); return r; };
   L.cond = take((size_t)B * c->cond_rows_out);
   L.cond_pf = pf_cols ? take((size_t)B * Tmax * pf_cols) : 0;
+  L.g_pf = g_frames ? take((size_t)B * c->hp.gin_channels * Tmax) : 0;
   L.x = take((size_t)B * 192 * L.P);
   L.skip = take((size_t)B * 192 * L.P);
   L.acts = take((size_t)B * 192 * L.P);
@@ -1970,21 +1973,50 @@ int ovc_tts_encode(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, 
                               w_ceil, logw, stream, nullptr);
 }
 
-int ovc_tts_encode_items(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid, const float* noise_w,
-                         uint64_t seed, float noise_scale_w, float length_scale, float sdp_ratio, int B, int T,
-                         int64_t* y_lengths, float* w_ceil, float* logw, void* stream, const ovc_item_params* items) {
+// Per-token speaker vectors condition the flow reverse and the generator per frame; both sections must read the target
+// embedding (a zero_g checkpoint's generator does not, and its section has no per-frame columns).
+static int check_tts_per_frame_cond(const ovc_ctx* c) {
+  const int tc = c->precision >= 1, m = OVC_SE_FRAMES_TGT - 1;
+  if (c->cond_pf_off[tc][m][2] < 0 || c->cond_pf_off[tc][m][3] < 0)
+    return fail(OVC_ERR_INVALID, "per-token speaker vectors need a flow and a generator conditioned on g (zero_g is not)");
+  return OVC_OK;
+}
+
+// the TTS encode with speaker ids (sid) or caller-supplied vectors (g, per row or with g_tokens per token)
+static int tts_encode_any(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid, const float* g,
+                          int g_tokens, const float* noise_w, uint64_t seed, float noise_scale_w, float length_scale,
+                          float sdp_ratio, int B, int T, int64_t* y_lengths, float* w_ceil, float* logw, void* stream,
+                          const ovc_item_params* items) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
   if (!c->tts.ready) return fail(OVC_ERR_STATE, "the checkpoint has no TTS members (enc_p / dp / sdp / emb_g): not a V1 base speaker");
-  if (!tokens || !x_lengths || !sid || !y_lengths) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (!tokens || !x_lengths || !(sid || g) || !y_lengths) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (g_tokens != 0 && g_tokens != 1) return fail(OVC_ERR_INVALID, "g_tokens must be 0 or 1 (got %d)", g_tokens);
+  if (g_tokens) TRY(check_tts_per_frame_cond(c));
   if (B < 1 || T < 1) return fail(OVC_ERR_INVALID, "B and T must be positive (got %d, %d)", B, T);
   if (B > 65535 || (long long)T * T > 2000000000LL / 256) return fail(OVC_ERR_INVALID, "B %d / T %d exceed the grid limits", B, T);
   if (!(length_scale > 0.f)) return fail(OVC_ERR_INVALID, "length_scale must be positive");
   ON_DEVICE(c);
   c->ev_used = c->prof ? c->ev_used : 0;
-  return run_tts_encode(c, (const long long*)tokens, (const long long*)x_lengths, (const long long*)sid, noise_w, seed,
-                        noise_scale_w, length_scale, sdp_ratio, B, T, (long long*)y_lengths, w_ceil, logw, item_params(items),
-                        (cudaStream_t)stream);
+  return run_tts_encode(c, (const long long*)tokens, (const long long*)x_lengths, (const long long*)sid, g, g_tokens, noise_w,
+                        seed, noise_scale_w, length_scale, sdp_ratio, B, T, (long long*)y_lengths, w_ceil, logw,
+                        item_params(items), (cudaStream_t)stream);
+}
+
+int ovc_tts_encode_items(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid, const float* noise_w,
+                         uint64_t seed, float noise_scale_w, float length_scale, float sdp_ratio, int B, int T,
+                         int64_t* y_lengths, float* w_ceil, float* logw, void* stream, const ovc_item_params* items) {
+  if (!sid) return fail(OVC_ERR_INVALID, "null tensor argument");
+  return tts_encode_any(c, tokens, x_lengths, sid, nullptr, 0, noise_w, seed, noise_scale_w, length_scale, sdp_ratio, B, T,
+                        y_lengths, w_ceil, logw, stream, items);
+}
+
+int ovc_tts_encode_g(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, const float* g, int g_tokens,
+                     const float* noise_w, uint64_t seed, float noise_scale_w, float length_scale, float sdp_ratio, int B, int T,
+                     int64_t* y_lengths, float* w_ceil, float* logw, void* stream, const ovc_item_params* items) {
+  if (!g) return fail(OVC_ERR_INVALID, "null tensor argument");
+  return tts_encode_any(c, tokens, x_lengths, nullptr, g, g_tokens, noise_w, seed, noise_scale_w, length_scale, sdp_ratio, B,
+                        T, y_lengths, w_ceil, logw, stream, items);
 }
 
 int ovc_tts_decode(ovc_ctx* c, const float* noise, uint64_t seed, float noise_scale, int B, int Ymax, int max_len, int ragged,
@@ -2008,64 +2040,112 @@ int ovc_tts_decode_items(ovc_ctx* c, const float* noise, uint64_t seed, float no
                         (cudaStream_t)stream);
 }
 
-int ovc_tts_encode_state(ovc_ctx* c, float* stats, int32_t* cum, float* g, void* stream) {
+// g_tok: the caller's g is [B][gin][T] and the pending encode must have taken per-token vectors; else [B][gin] and it
+// must not (either mismatch is OVC_ERR_STATE: a per-token encode never yields one vector per row)
+static int tts_encode_state(ovc_ctx* c, float* stats, int32_t* cum, float* g, bool g_tok, void* stream) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
   if (c->tts_B < 1) return fail(OVC_ERR_STATE, "ovc_tts_encode_state needs a preceding ovc_tts_encode");
+  if (c->tts_gtok != g_tok)
+    return fail(OVC_ERR_STATE, g_tok ? "ovc_tts_encode_state_tokens needs a per-token encode (ovc_tts_encode_g, g_tokens = 1)"
+                                     : "the pending encode took per-token speaker vectors: use ovc_tts_encode_state_tokens");
   if (!stats || !cum || !g) return fail(OVC_ERR_INVALID, "null tensor argument");
   ON_DEVICE(c);
   const int B = c->tts_B, T = c->tts_T;
-  const TtsWs TW = tts_ws_layout(c, B, T);
+  const TtsWs TW = tts_ws_layout(c, B, T, g_tok);
   cudaStream_t st = (cudaStream_t)stream;
   CK(cudaMemcpyAsync(stats, c->d_tts + TW.STATS, (size_t)B * T * 2 * c->tts.C * sizeof(float), cudaMemcpyDeviceToDevice, st));
   CK(cudaMemcpyAsync(cum, c->d_tts + TW.cum, (size_t)B * T * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-  CK(cudaMemcpyAsync(g, c->d_tts + TW.g, (size_t)B * c->hp.gin_channels * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  CK(cudaMemcpyAsync(g, c->d_tts + (g_tok ? TW.gtok : TW.g), (size_t)B * c->hp.gin_channels * (g_tok ? T : 1) * sizeof(float),
+                     cudaMemcpyDeviceToDevice, st));
   return OVC_OK;
 }
 
-static int tts_state_rows(ovc_ctx* c, const float* stats, const int* cum, const float* g, const long long* y_len, int B, int T,
-                          const int64_t* dst_row, int N, int Tp, float* d_stats, int32_t* d_cum, float* d_g, int64_t* d_ylen,
-                          cudaStream_t st) {
+int ovc_tts_encode_state(ovc_ctx* c, float* stats, int32_t* cum, float* g, void* stream) {
+  return tts_encode_state(c, stats, cum, g, false, stream);
+}
+
+int ovc_tts_encode_state_tokens(ovc_ctx* c, float* stats, int32_t* cum, float* g, void* stream) {
+  return tts_encode_state(c, stats, cum, g, true, stream);
+}
+
+// g_tok: g [B][gin][T] -> d_g [N][gin][Tp] (tts_state_rows_g_kernel); else g [B][gin] -> d_g [N][gin]
+static int tts_state_rows(ovc_ctx* c, const float* stats, const int* cum, const float* g, bool g_tok, const long long* y_len,
+                          int B, int T, const int64_t* dst_row, int N, int Tp, float* d_stats, int32_t* d_cum, float* d_g,
+                          int64_t* d_ylen, cudaStream_t st) {
   if (!dst_row || !d_stats || !d_cum || !d_g || !d_ylen) return fail(OVC_ERR_INVALID, "null tensor argument");
   if (N < 1 || Tp < T) return fail(OVC_ERR_INVALID, "pool of %d rows at pitch %d cannot take rows of %d tokens", N, Tp, T);
-  const long long per_row = (long long)Tp * 2 * c->tts.C + Tp + c->hp.gin_channels + 1;
+  const int gin = g_tok ? 0 : c->hp.gin_channels;   // per token: the g part is the second kernel's
+  const long long per_row = (long long)Tp * 2 * c->tts.C + Tp + gin + 1;
   const int gx = (int)std::max(1LL, std::min((per_row + 255) / 256, std::max(1LL, 4LL * c->sm_count / B)));
-  tts_state_rows_kernel<<<dim3(gx, std::min(B, 65535)), 256, 0, st>>>(stats, cum, g, y_len, B, T, 2 * c->tts.C, c->hp.gin_channels,
+  tts_state_rows_kernel<<<dim3(gx, std::min(B, 65535)), 256, 0, st>>>(stats, cum, g, y_len, B, T, 2 * c->tts.C, gin,
                                                      (const long long*)dst_row, N, Tp, d_stats, d_cum, d_g,
                                                      (long long*)d_ylen);
   CK(cudaGetLastError());
+  if (g_tok) {
+    const long long n = (long long)c->hp.gin_channels * Tp;
+    const int gx2 = (int)std::max(1LL, std::min((n + 255) / 256, std::max(1LL, 4LL * c->sm_count / B)));
+    tts_state_rows_g_kernel<<<dim3(gx2, std::min(B, 65535)), 256, 0, st>>>(g, B, T, c->hp.gin_channels,
+                                                                           (const long long*)dst_row, N, Tp, d_g);
+    CK(cudaGetLastError());
+  }
   return OVC_OK;
+}
+
+static int tts_encode_state_rows(ovc_ctx* c, bool g_tok, const int64_t* dst_row, int N, int Tp, float* stats, int32_t* cum,
+                                 float* g, int64_t* y_lengths, void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
+  if (c->tts_B < 1) return fail(OVC_ERR_STATE, "ovc_tts_encode_state_rows needs a preceding ovc_tts_encode");
+  if (c->tts_gtok != g_tok)
+    return fail(OVC_ERR_STATE, g_tok ? "ovc_tts_encode_state_rows_tokens needs a per-token encode (ovc_tts_encode_g, g_tokens = 1)"
+                                     : "the pending encode took per-token speaker vectors: use ovc_tts_encode_state_rows_tokens");
+  ON_DEVICE(c);
+  const int B = c->tts_B, T = c->tts_T;
+  const TtsWs TW = tts_ws_layout(c, B, T, g_tok);
+  return tts_state_rows(c, c->d_tts + TW.STATS, reinterpret_cast<const int*>(c->d_tts + TW.cum),
+                        c->d_tts + (g_tok ? TW.gtok : TW.g), g_tok, reinterpret_cast<const long long*>(c->d_tts + TW.ylen),
+                        B, T, dst_row, N, Tp, stats, cum, g, y_lengths, (cudaStream_t)stream);
 }
 
 int ovc_tts_encode_state_rows(ovc_ctx* c, const int64_t* dst_row, int N, int Tp, float* stats, int32_t* cum, float* g,
                               int64_t* y_lengths, void* stream) {
-  if (!c) return fail(OVC_ERR_INVALID, "null context");
-  if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
-  if (c->tts_B < 1) return fail(OVC_ERR_STATE, "ovc_tts_encode_state_rows needs a preceding ovc_tts_encode");
-  ON_DEVICE(c);
-  const int B = c->tts_B, T = c->tts_T;
-  const TtsWs TW = tts_ws_layout(c, B, T);
-  return tts_state_rows(c, c->d_tts + TW.STATS, reinterpret_cast<const int*>(c->d_tts + TW.cum),
-                        c->d_tts + TW.g, reinterpret_cast<const long long*>(c->d_tts + TW.ylen), B, T, dst_row, N, Tp,
-                        stats, cum, g, y_lengths, (cudaStream_t)stream);
+  return tts_encode_state_rows(c, false, dst_row, N, Tp, stats, cum, g, y_lengths, stream);
 }
 
-int ovc_tts_state_rows(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths, int B,
-                       int T, const int64_t* dst_row, int N, int Tp, float* d_stats, int32_t* d_cum, float* d_g,
-                       int64_t* d_y_lengths, void* stream) {
+int ovc_tts_encode_state_rows_tokens(ovc_ctx* c, const int64_t* dst_row, int N, int Tp, float* stats, int32_t* cum, float* g,
+                                     int64_t* y_lengths, void* stream) {
+  return tts_encode_state_rows(c, true, dst_row, N, Tp, stats, cum, g, y_lengths, stream);
+}
+
+static int tts_state_rows_from(ovc_ctx* c, bool g_tok, const float* stats, const int32_t* cum, const float* g,
+                               const int64_t* y_lengths, int B, int T, const int64_t* dst_row, int N, int Tp, float* d_stats,
+                               int32_t* d_cum, float* d_g, int64_t* d_y_lengths, void* stream) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
   if (!stats || !cum || !g || !y_lengths) return fail(OVC_ERR_INVALID, "null tensor argument");
   if (B < 1 || T < 1) return fail(OVC_ERR_INVALID, "B and T must be positive (got %d, %d)", B, T);
   ON_DEVICE(c);
-  return tts_state_rows(c, stats, cum, g, (const long long*)y_lengths, B, T, dst_row, N, Tp, d_stats, d_cum, d_g, d_y_lengths,
-                        (cudaStream_t)stream);
+  return tts_state_rows(c, stats, cum, g, g_tok, (const long long*)y_lengths, B, T, dst_row, N, Tp, d_stats, d_cum, d_g,
+                        d_y_lengths, (cudaStream_t)stream);
 }
 
-int ovc_tts_decode_windows(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths,
-                           int N, int T, const int64_t* row, const int64_t* frame0, const int64_t* len, int W, int Wmax,
-                           const uint64_t* seed, const int64_t* stream, const float* noise_scale, float* o, float* z_p,
-                           void* cuda_stream) {
+int ovc_tts_state_rows(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths, int B,
+                       int T, const int64_t* dst_row, int N, int Tp, float* d_stats, int32_t* d_cum, float* d_g,
+                       int64_t* d_y_lengths, void* stream) {
+  return tts_state_rows_from(c, false, stats, cum, g, y_lengths, B, T, dst_row, N, Tp, d_stats, d_cum, d_g, d_y_lengths, stream);
+}
+
+int ovc_tts_state_rows_tokens(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths,
+                              int B, int T, const int64_t* dst_row, int N, int Tp, float* d_stats, int32_t* d_cum, float* d_g,
+                              int64_t* d_y_lengths, void* stream) {
+  return tts_state_rows_from(c, true, stats, cum, g, y_lengths, B, T, dst_row, N, Tp, d_stats, d_cum, d_g, d_y_lengths, stream);
+}
+
+static int tts_decode_windows(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, bool g_tok,
+                              const int64_t* y_lengths, int N, int T, const int64_t* row, const int64_t* frame0,
+                              const int64_t* len, int W, int Wmax, const uint64_t* seed, const int64_t* stream,
+                              const float* noise_scale, float* o, float* z_p, void* cuda_stream) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized || !c->tts.ready) return fail(OVC_ERR_STATE, "no finalized TTS checkpoint");
   if (!stats || !cum || !g || !y_lengths || !row || !frame0 || !len || !seed || !stream || !noise_scale || !o)
@@ -2073,21 +2153,38 @@ int ovc_tts_decode_windows(ovc_ctx* c, const float* stats, const int32_t* cum, c
   if (N < 1 || T < 1 || W < 1 || Wmax < 1)
     return fail(OVC_ERR_INVALID, "N, T, W and Wmax must be positive (got %d, %d, %d, %d)", N, T, W, Wmax);
   if (W > 65535) return fail(OVC_ERR_INVALID, "W %d exceeds the grid limit", W);
+  if (g_tok) TRY(check_tts_per_frame_cond(c));
   if ((long long)Wmax * 256 * 64 > 2000000000LL) return fail(OVC_ERR_INVALID, "Wmax %d too large for 32-bit indexing", Wmax);
   ON_DEVICE(c);
   c->ev_used = c->prof ? c->ev_used : 0;
   cudaStream_t st = (cudaStream_t)cuda_stream;
-  TRY(ensure_ws(c, ws_layout(c, W, Wmax), W, Wmax, st));
+  TRY(ensure_ws(c, tts_windows_ws(c, W, Wmax, g_tok), W, Wmax, st));
   ItemParams it{};
   it.seed = (const unsigned long long*)seed; it.stream = (const long long*)stream; it.noise_scale = noise_scale;
   const TtsWindows win{(const long long*)row, (const long long*)frame0, (const long long*)len, N};
   std::vector<uintptr_t> key = {3, (uintptr_t)stats, (uintptr_t)cum, (uintptr_t)g, (uintptr_t)y_lengths, (uintptr_t)N,
                                 (uintptr_t)T, (uintptr_t)row, (uintptr_t)frame0, (uintptr_t)len, (uintptr_t)W, (uintptr_t)Wmax,
-                                (uintptr_t)o, (uintptr_t)z_p, option_bits(c)};
+                                (uintptr_t)o, (uintptr_t)z_p, option_bits(c), (uintptr_t)g_tok};
   append_item_key(key, it);
   return run_graphed(c, key, st, [&](cudaStream_t s) {
-    return run_tts_decode_windows(c, stats, cum, g, (const long long*)y_lengths, T, win, W, Wmax, it, o, z_p, s);
+    return run_tts_decode_windows(c, stats, cum, g, g_tok, (const long long*)y_lengths, T, win, W, Wmax, it, o, z_p, s);
   });
+}
+
+int ovc_tts_decode_windows(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths,
+                           int N, int T, const int64_t* row, const int64_t* frame0, const int64_t* len, int W, int Wmax,
+                           const uint64_t* seed, const int64_t* stream, const float* noise_scale, float* o, float* z_p,
+                           void* cuda_stream) {
+  return tts_decode_windows(c, stats, cum, g, false, y_lengths, N, T, row, frame0, len, W, Wmax, seed, stream, noise_scale, o,
+                            z_p, cuda_stream);
+}
+
+int ovc_tts_decode_windows_tokens(ovc_ctx* c, const float* stats, const int32_t* cum, const float* g, const int64_t* y_lengths,
+                                  int N, int T, const int64_t* row, const int64_t* frame0, const int64_t* len, int W, int Wmax,
+                                  const uint64_t* seed, const int64_t* stream, const float* noise_scale, float* o, float* z_p,
+                                  void* cuda_stream) {
+  return tts_decode_windows(c, stats, cum, g, true, y_lengths, N, T, row, frame0, len, W, Wmax, seed, stream, noise_scale, o,
+                            z_p, cuda_stream);
 }
 
 int ovc_philox_normals(uint64_t seed, int64_t stream, int64_t c0, int C, int64_t frame0, int T, float* out, void* cuda_stream) {

@@ -246,6 +246,45 @@ __global__ void tts_lin_kernel(const float* g, const float* W, const float* bias
   out[(size_t)b * rows + r] = acc;
 }
 
+// Per-token conditioning of the duration predictors (models.py:89-92, 139-141 with g [B, gin, T]):
+// out[b][t][r] = x[b][t][r] + (bias[r] + W[r][:] . g[b][:][t]) for t < lens[b]; in place safe (x == out).  Each sum is
+// the fmaf chain of tts_lin_kernel in the same order, then the add of tts_add_rowvec_kernel, so a token whose vector
+// equals the row vector gets bit-identical values.  A CTA takes 128 output rows of TTS_TOK_T tokens: g's columns are
+// staged in shared memory and each weight is read once per TTS_TOK_T tokens.  g [B][in_dim][T]; dynamic smem
+// in_dim * TTS_TOK_T floats.  grid (ceil(rows/128), ceil(T/TTS_TOK_T), B), 128 threads
+constexpr int TTS_TOK_T = 8;
+__global__ void __launch_bounds__(128) tts_cond_tok_kernel(const float* x, const float* __restrict__ g,
+                                                           const float* __restrict__ W, const float* __restrict__ bias,
+                                                           const long long* lens, int T, int in_dim, int rows, float* out) {
+  extern __shared__ float sg[];   // [in_dim][TTS_TOK_T]
+  const int r = blockIdx.x * blockDim.x + threadIdx.x, t0 = blockIdx.y * TTS_TOK_T, b = blockIdx.z;
+  const int nt = min(TTS_TOK_T, tts_len(lens, b, T) - t0);
+  if (nt <= 0) return;
+  for (int e = threadIdx.x; e < in_dim * TTS_TOK_T; e += blockDim.x) {
+    const int i = e / TTS_TOK_T, k = e % TTS_TOK_T;
+    sg[e] = k < nt ? g[((size_t)b * in_dim + i) * T + t0 + k] : 0.f;
+  }
+  __syncthreads();
+  if (r >= rows) return;
+  float acc[TTS_TOK_T];
+  const float b0 = bias[r];
+#pragma unroll
+  for (int k = 0; k < TTS_TOK_T; ++k) acc[k] = b0;
+  const float* wr = W + (size_t)r * in_dim;
+  for (int i = 0; i < in_dim; ++i) {
+    const float w = wr[i];
+#pragma unroll
+    for (int k = 0; k < TTS_TOK_T; ++k) acc[k] = fmaf(w, sg[i * TTS_TOK_T + k], acc[k]);
+  }
+#pragma unroll
+  for (int k = 0; k < TTS_TOK_T; ++k) {
+    if (k < nt) {
+      const size_t o = ((size_t)b * T + t0 + k) * rows + r;
+      out[o] = x[o] + acc[k];
+    }
+  }
+}
+
 // emb_g(sid)                                                                     models.py:470        grid (ceil(dim/128), B)
 __global__ void tts_speaker_kernel(const float* table, const long long* sid, int n_rows, int dim, float* out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
@@ -372,6 +411,26 @@ __global__ void tts_window_rows_kernel(const float* g, const long long* y_len, i
   }
 }
 
+// Per-token speaker vectors along the alignment path, as tts_expand_kernel expands m_p: g_out[b][i][y] = g[r][i][tok(f)]
+// for frames f = frame0[b] + y the expansion fills (inside the row, below len[b]), 0 elsewhere.  g [N][gin][T] (the
+// per-token encode's layout), g_out [B][gin][Ty].  One thread per frame finds its token once and writes every channel.
+// grid (ceil(Ty/128), B), 128 threads
+__global__ void tts_expand_g_kernel(const float* __restrict__ g, const int* __restrict__ cum, const long long* y_len, int T,
+                                    int gin, int Ty, float* __restrict__ g_out, TtsWindows win) {
+  const int y = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+  if (y >= Ty) return;
+  const long long r = win.row ? min(max(win.row[b], 0LL), (long long)win.N - 1) : (long long)b;
+  const long long f = win.frame0 ? win.frame0[b] + y : (long long)y;
+  float* dst = g_out + (size_t)b * gin * Ty + y;
+  if (f >= 0 && f < y_len[r] && (!win.len || y < win.len[b])) {
+    const int j = ovc_tts::frame_token(cum + (size_t)r * T, T, (int)f);
+    const float* src = g + (size_t)r * gin * T + j;
+    for (int i = 0; i < gin; ++i) dst[(size_t)i * Ty] = src[(size_t)i * T];
+  } else {
+    for (int i = 0; i < gin; ++i) dst[(size_t)i * Ty] = 0.f;
+  }
+}
+
 // Encoded rows -> rows of a state pool (ovc_tts_encode_state_rows / ovc_tts_state_rows): source row b (B rows of T tokens)
 // goes to pool row dst_row[b], clamped into [0, N), at token pitch Tp >= T.  Tokens T <= t < Tp get the padding a short
 // row gets inside an encode: cum keeps its last value (durations_row), stats are 0.  One item per element of the
@@ -397,6 +456,23 @@ __global__ void __launch_bounds__(256) tts_state_rows_kernel(const float* __rest
       } else {
         d_ylen[r] = y_len[b];
       }
+    }
+  }
+}
+
+// The per-token speaker vectors of encoded rows -> rows of a per-token state pool (ovc_tts_encode_state_rows_tokens /
+// ovc_tts_state_rows_tokens): g [B][gin][T] -> d_g[dst_row[b]][gin][Tp], dst_row clamped into [0, N); tokens
+// T <= t < Tp get 0, as the stats there.  The rest of each row is written by tts_state_rows_kernel.
+// grid (x: element blocks, y: rows), both strided; 256 threads
+__global__ void __launch_bounds__(256) tts_state_rows_g_kernel(const float* __restrict__ g, int B, int T, int gin,
+                                                               const long long* __restrict__ dst_row, int N, int Tp,
+                                                               float* __restrict__ d_g) {
+  const long long per_row = (long long)gin * Tp;
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    const long long r = min(max(dst_row[b], 0LL), (long long)N - 1);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < per_row; i += (long long)gridDim.x * blockDim.x) {
+      const int c = (int)(i / Tp), t = (int)(i - (long long)c * Tp);
+      d_g[r * per_row + i] = t < T ? g[((size_t)b * gin + c) * T + t] : 0.f;
     }
   }
 }

@@ -872,12 +872,15 @@ class StreamingSessions:
 
 
 class _CloneSession:
-    __slots__ = ("tts_keys", "conv_keys", "said", "unencoded", "plans", "length", "ended", "checked", "ss_id", "out_sr")
+    __slots__ = ("tts_keys", "conv_keys", "said", "unencoded", "plans", "length", "ended", "checked", "ss_id", "out_sr",
+                 "tokens", "tokens_encoded")
 
     def __init__(self, tts_keys: dict, conv_keys: dict, out_sr: Optional[int] = None):
         self.tts_keys, self.conv_keys, self.out_sr = tts_keys, conv_keys, out_sr
         self.said = 0                                     # sentences said so far: the next one is sentence `said`
         self.unencoded = 0                                # said sentences still waiting for the encode
+        self.tokens = 0                                   # tokens said so far: the next sentence starts at this position
+        self.tokens_encoded = 0                           # tokens of the sentences already encoded
         self.plans: deque = deque()                       # TTS windows to decode: (pool row, lo, hi, e0, e1, gap, last)
         self.length = 0                                   # samples of the encoded sentences and their gaps
         self.ended = False
@@ -994,11 +997,19 @@ class CloneSessions:
         (``NativeSynthesizer.check_tts_input``, the encode's own check); the session keeps what it had said before."""
         ids = self._sentences(sid, text, ids, language)
         flat = [t for q in ids for t in q]
+        keys = self.sessions[sid].tts_keys
         try:
-            self.tts.model.check_tts_input(torch.as_tensor(flat or [0], dtype=torch.int64),
-                                           torch.as_tensor([self.sessions[sid].tts_keys["speaker"]], dtype=torch.int64))
+            if keys["speaker"] is None:
+                self.tts.model.check_tts_input(torch.as_tensor(flat or [0], dtype=torch.int64), None, need_sid=False)
+            else:
+                self.tts.model.check_tts_input(torch.as_tensor(flat or [0], dtype=torch.int64),
+                                               torch.as_tensor([keys["speaker"]], dtype=torch.int64))
         except ValueError as e:
             raise ValueError(f"{self.label} {sid}: {e}") from None
+        e, n = keys["g"], self.sessions[sid].tokens + len(flat)
+        if torch.is_tensor(e) and e.dim() == 2 and n > e.shape[1]:
+            raise ValueError(f"{self.label} {sid}: its per-token speaker tensor has {e.shape[1]} columns, the session "
+                             f"would reach {n} tokens")
         self._queue(sid, ids)
 
     def _sentences(self, sid, text, ids, language) -> List[List[int]]:
@@ -1021,6 +1032,7 @@ class CloneSessions:
         self.pending += [(sid, q) for q in ids]
         s.said += len(ids)
         s.unencoded += len(ids)
+        s.tokens += sum(len(q) for q in ids)
 
     def end(self, sid: int) -> None:
         """No more text for session ``sid``: it closes once its audio is out."""
@@ -1065,14 +1077,18 @@ class CloneSessions:
     def _encode(self) -> None:
         from .api import TTS_HALO_FRAMES, TtsPool, plan_tts_windows
         tts = self.tts
-        seqs, spk = [q for _, q in self.pending], []
+        seqs, spk, spk_rows = [q for _, q in self.pending], [], []
         kw = {"seeds": [], "streams": [], "noise_scale": [], "noise_scale_w": [], "length_scale": [], "sdp_ratio": []}
         nth: Dict[int, int] = {}
-        for sid, _ in self.pending:
+        at: Dict[int, int] = {}                           # next token position of each session in this encode
+        for sid, q in self.pending:
             s = self.sessions[sid]
             j = s.said - s.unencoded + nth.get(sid, 0)    # the sentence's number in its session
             nth[sid] = nth.get(sid, 0) + 1
-            spk.append(s.tts_keys["speaker"])
+            o = at.get(sid, s.tokens_encoded)             # o_j: its first token's position in the session's stream
+            at[sid] = o + len(q)
+            spk.append(0 if s.tts_keys["speaker"] is None else s.tts_keys["speaker"])
+            spk_rows.append((s.tts_keys["speaker"], s.tts_keys["g"], o, len(q)))
             kw["seeds"].append(s.tts_keys["seed"])
             kw["streams"].append(j)
             tts._sentence_params(s.tts_keys, kw)
@@ -1083,6 +1099,9 @@ class CloneSessions:
         if self.pool is None:
             self.pool = TtsPool(tts.model.native, tts.model.device)
         x, lens = tts._pad_ids(seqs)
+        g = tts._speaker_rows(spk_rows, x.shape[1])
+        if g is not None:
+            kw["g"] = g
         state = tts.model.tts_encode(x, lens, sid=torch.as_tensor(spk, dtype=torch.int64), pool=self.pool, rows=rows, **kw)
         del self.free_rows[:len(take)]
         self.rows += len(new)
@@ -1099,6 +1118,7 @@ class CloneSessions:
                         for k, (lo, hi, e0, e1) in enumerate(wins)]
             s.length += self.hop * frames + gap
             s.unencoded -= 1
+            s.tokens_encoded += len(seqs[i])
         self.pending = []
 
     @torch.no_grad()
