@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 15 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 16 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
@@ -34,7 +34,8 @@ extern "C" {
                                * 13: ovc_resample_plan, ovc_resample_rings;
                                * 14: ovc_voice_conversion_frames, ovc_convert_waveform_frames, ovc_tone_track_expand;
                                * 15: ovc_tts_encode_g, ovc_tts_encode_state_tokens, ovc_tts_decode_windows_tokens,
-                               *     ovc_tts_encode_state_rows_tokens, ovc_tts_state_rows_tokens */
+                               *     ovc_tts_encode_state_rows_tokens, ovc_tts_state_rows_tokens;
+                               * 16: ovc_reference_encoder_stream, ovc_reference_encoder_stream_state_floats */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -284,6 +285,31 @@ OVC_API int ovc_reference_encoder(ovc_ctx* ctx, const float* spec, int N, int T,
  * ignores its mask, so its stride-2 convs and GRU read the padded frames. */
 OVC_API int ovc_reference_encoder_ragged(ovc_ctx* ctx, const float* spec, const int64_t* lengths,
                                          int N, int Tmax, float* out, void* stream);
+
+/* The reference encoder advanced with live streams, so a stream's source embedding can be learned from its own audio
+ * at constant cost per sample.  Each stream owns a state row of ovc_reference_encoder_stream_state_floats() floats
+ * (0 before ovc_finalize_weights or without ref_enc.* tensors): the spectrogram frames consumed so far (c0), the GRU
+ * hidden state and the <= 2 most recent rows of each conv input that later rows still read.  An all-zero row is a
+ * fresh stream.  Frame t is final at n samples when t * hop + (n_fft - pad) <= n (streaming.ready_frames).
+ *
+ * desc [B][4] int64 (device) = (state_row, ring_row, n_adv, n_snap) per item.  With n_snap > 0 the row first advances
+ * to the final frames of n_snap samples and out[b] ([B][gin]) gets the snapshot: bit for bit the embedding
+ * ovc_reference_encoder_ragged gives for the stream's first n_snap samples alone (n_snap >= hop and > pad).  The row
+ * then advances to the final frames of n_adv samples (never backwards).  The state is not otherwise changed by a
+ * snapshot.  Sample s of the stream is rings[ring_row * ring_cap + s % ring_cap]; the caller keeps samples
+ * [c0 * hop - pad, max(n_adv, n_snap)) there.  A call adds at most max_new_frames (1 .. 65536) final frames per row.
+ *
+ * Every descriptor is clamped on the device (rows into range, c0 into [0, 2^29], new frames to max_new_frames), so
+ * nothing outside rings, state and out is read or written whatever desc or a state row holds.  A snapshot that cannot
+ * be produced -- its final frames lie before the row's c0 or past c0 + max_new_frames, or n_snap is too short --
+ * writes NaN to out[b]; n_snap <= 0 leaves out[b] alone.  Two items naming one state row race.  Two launches whatever
+ * B (a ring STFT of each item's new and tail frames, then one CTA per item); the call only enqueues on `stream`, so it
+ * can be captured in a CUDA graph once a call with the same B and max_new_frames has sized the workspace outside
+ * capture (inside capture a larger workspace is OVC_ERR_STATE).  A checkpoint without ref_enc.* gives OVC_ERR_MISSING. */
+OVC_API size_t ovc_reference_encoder_stream_state_floats(const ovc_ctx* ctx);
+OVC_API int ovc_reference_encoder_stream(ovc_ctx* ctx, const float* rings, int ring_rows, int64_t ring_cap, float* state,
+                                         int state_rows, const int64_t* desc, int B, int max_new_frames, float* out,
+                                         void* stream);
 
 /* Sample-rate conversion on the device, for waveforms that do not arrive at the model's rate (the reference resamples
  * every input on the host: librosa.load(path, sr=hps.data.sampling_rate), openvoice/api.py:123,144).  The arithmetic is

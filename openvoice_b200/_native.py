@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 15
+ABI_VERSION = 16
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -26,7 +26,7 @@ EXPORTS = (
     "ovc_tts_encode_state_rows", "ovc_tts_state_rows", "ovc_resample_plan", "ovc_resample_rings",
     "ovc_voice_conversion_frames", "ovc_convert_waveform_frames", "ovc_tone_track_expand",
     "ovc_tts_encode_g", "ovc_tts_encode_state_tokens", "ovc_tts_decode_windows_tokens", "ovc_tts_encode_state_rows_tokens",
-    "ovc_tts_state_rows_tokens",
+    "ovc_tts_state_rows_tokens", "ovc_reference_encoder_stream", "ovc_reference_encoder_stream_state_floats",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample / ovc_spectrogram_ring length of a stream that has not ended
@@ -190,6 +190,10 @@ def load_library(path: Optional[str] = None):
     lib.ovc_resample_plan.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int32), C.c_void_p]
     lib.ovc_resample_rings.argtypes = ([C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64] + [C.c_void_p] * 5
                                        + [C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p])
+    lib.ovc_reference_encoder_stream_state_floats.restype = C.c_size_t
+    lib.ovc_reference_encoder_stream_state_floats.argtypes = [C.c_void_p]
+    lib.ovc_reference_encoder_stream.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p,
+                                                 C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     if lib.ovc_abi_version() != ABI_VERSION:
         raise OvcError(f"ABI mismatch: library {lib.ovc_abi_version()} vs binding {ABI_VERSION}")
     _lib = lib
@@ -489,6 +493,47 @@ class NativeConverter:
             rc = self.lib.ovc_reference_encoder_ragged(self.handle, C.c_void_p(spec.data_ptr()), C.c_void_p(lengths.data_ptr()),
                                                        N, T, C.c_void_p(out.data_ptr()), C.c_void_p(st.cuda_stream))
             _check(self.lib, rc, "ovc_reference_encoder_ragged")
+        return out
+
+    @property
+    def refenc_state_floats(self) -> int:
+        """Floats of one ``reference_encoder_stream`` state row (0 without ref_enc.* tensors)."""
+        return int(self.lib.ovc_reference_encoder_stream_state_floats(self.handle))
+
+    def reference_encoder_stream(self, rings, state, desc, max_new_frames: int, out=None, stream=None):
+        """Advance streams' reference encoders and take snapshots (include/ovc.h: ovc_reference_encoder_stream).
+        rings [R, cap] f32 cuda (sample s of row r at rings[r, s % cap]); state [S, refenc_state_floats] f32 cuda, one
+        row per stream, all zeros for a fresh one, updated in place; desc [B, 4] int64 cuda rows (state_row, ring_row,
+        n_adv, n_snap).  Returns out [B, gin]: row b is the embedding of the stream's first n_snap samples (NaN when it
+        cannot be produced; untouched when n_snap <= 0).  Asynchronous on `stream`; ValueError for bad shapes before any
+        launch."""
+        import torch
+        gin = self.hp.gin_channels
+        for name, t, dt in (("rings", rings, torch.float32), ("state", state, torch.float32), ("desc", desc, torch.int64)):
+            if not (t.is_cuda and t.dtype == dt and t.is_contiguous() and t.dim() == 2):
+                raise ValueError(f"reference_encoder_stream: {name} must be a contiguous 2-D {dt} cuda tensor")
+        F = self.refenc_state_floats
+        if F == 0:
+            raise ValueError("reference_encoder_stream: the checkpoint has no ref_enc.* tensors")
+        if state.shape[1] != F:
+            raise ValueError(f"reference_encoder_stream: state rows have {state.shape[1]} floats, expected {F}")
+        B = desc.shape[0]
+        if desc.shape[1] != 4 or B < 1:
+            raise ValueError(f"reference_encoder_stream: desc has shape {tuple(desc.shape)}, expected (B >= 1, 4)")
+        if rings.shape[1] < 1024 or rings.shape[0] < 1 or state.shape[0] < 1:
+            raise ValueError(f"reference_encoder_stream: rings {tuple(rings.shape)} / state {tuple(state.shape)} too small")
+        if not 1 <= int(max_new_frames) <= 65536:
+            raise ValueError(f"reference_encoder_stream: max_new_frames {max_new_frames} outside [1, 65536]")
+        if out is None:
+            out = torch.empty(B, gin, device=rings.device, dtype=torch.float32)
+        if not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == B * gin):
+            raise ValueError(f"reference_encoder_stream: out must be a contiguous float32 cuda tensor of {B} x {gin}")
+        st = stream if stream is not None else torch.cuda.current_stream(rings.device)
+        p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+        rc = self.lib.ovc_reference_encoder_stream(self.handle, p(rings), int(rings.shape[0]), int(rings.shape[1]), p(state),
+                                                   int(state.shape[0]), p(desc), B, int(max_new_frames), p(out),
+                                                   C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_reference_encoder_stream")
         return out
 
     def resample(self, x, in_lengths, sr_in: int, sr_out: int, out=None, out_pitch: Optional[int] = None,

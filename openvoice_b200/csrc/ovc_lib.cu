@@ -220,6 +220,8 @@ struct ovc_ctx {
   int re_gru_in = 0;           // columns of ref_enc.gru.weight_ih_l0
   float* d_re = nullptr;
   size_t re_floats = 0;
+  float* d_res = nullptr;      // ovc_reference_encoder_stream: spectrogram columns and layer rows of its items
+  size_t res_floats = 0;
 
   // ovc_resample: one fp64 polyphase bank per reduced (up, down) pair, built on first use and kept
   std::map<std::pair<int64_t, int64_t>, double*> rs_banks;
@@ -1543,6 +1545,7 @@ void ovc_destroy(ovc_ctx* c) {
       if (p) cudaFree(p);
   if (c->d_tcw) cudaFree(c->d_tcw);
   if (c->d_re) cudaFree(c->d_re);
+  if (c->d_res) cudaFree(c->d_res);
   for (auto& kv : c->rs_banks) cudaFree(kv.second);
   if (c->d_rs_plans) cudaFree(c->d_rs_plans);
   if (c->d_tw) cudaFree(c->d_tw);
@@ -1796,6 +1799,63 @@ int ovc_reference_encoder_ragged(ovc_ctx* c, const float* spec, const int64_t* l
                                  void* stream) {
   if (!lengths) return fail(OVC_ERR_INVALID, "null lengths in ovc_reference_encoder_ragged");
   return run_refenc(c, spec, (const long long*)lengths, N, Tmax, out, stream);
+}
+
+size_t ovc_reference_encoder_stream_state_floats(const ovc_ctx* c) {
+  if (!c || !c->finalized || !c->has_refenc) return 0;
+  return (size_t)ovc_re::geom(c->hp.spec_channels).floats;
+}
+
+int ovc_reference_encoder_stream(ovc_ctx* c, const float* rings, int ring_rows, int64_t ring_cap, float* state, int state_rows,
+                                 const int64_t* desc, int B, int max_new_frames, float* out, void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
+  if (!c->has_refenc) return fail(OVC_ERR_MISSING, "the checkpoint had no ref_enc.* tensors");
+  if (!rings || !state || !desc || !out) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (B < 1 || B > 65535 || ring_rows < 1 || state_rows < 1)
+    return fail(OVC_ERR_INVALID, "bad sizes B=%d ring_rows=%d state_rows=%d", B, ring_rows, state_rows);
+  if (max_new_frames < 1 || max_new_frames > ovc_re::MAX_NEW)
+    return fail(OVC_ERR_INVALID, "max_new_frames %d outside [1, %d]", max_new_frames, ovc_re::MAX_NEW);
+  if (ring_cap < STFT_N) return fail(OVC_ERR_INVALID, "ring_cap %lld is below one FFT frame (%d)", (long long)ring_cap, STFT_N);
+  if (c->hp.spec_channels != STFT_N / 2 + 1 || c->hp.hop_length != 256)
+    return fail(OVC_ERR_INVALID, "the STFT kernel is specialised for n_fft = win_length = 1024, hop 256");
+  const int F = c->hp.spec_channels, G = c->hp.gin_channels;
+  const ovc_re::Geom geo = ovc_re::geom(F);
+  if (ovc_re::filt(ovc_re::LAYERS) * geo.W[ovc_re::LAYERS] != c->re_gru_in)
+    return fail(OVC_ERR_INVALID, "ref_enc.gru.weight_ih_l0 takes %d inputs but spec_channels %d gives %d", c->re_gru_in, F,
+                ovc_re::filt(ovc_re::LAYERS) * geo.W[ovc_re::LAYERS]);
+  ON_DEVICE(c);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Tcols = max_new_frames + ovc_re::TAIL;
+  const size_t spec_floats = round_up((size_t)B * F * Tcols, 64);
+  const size_t item = (size_t)ovc_re::ws_floats(max_new_frames, F);
+  const size_t need = spec_floats + (size_t)B * item;
+  if (need > c->res_floats) {   // grows outside capture only: a captured call keeps the addresses it was captured with
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CK(cudaStreamIsCapturing(st, &cs));
+    if (cs != cudaStreamCaptureStatusNone)
+      return fail(OVC_ERR_STATE, "ovc_reference_encoder_stream: B=%d max_new_frames=%d needs a larger workspace; make one such "
+                  "call outside stream capture first", B, max_new_frames);
+    CK(cudaStreamSynchronize(st));
+    if (c->d_res) CK(cudaFree(c->d_res));
+    c->d_res = nullptr; c->res_floats = 0;
+    CK(cudaMalloc(&c->d_res, need * sizeof(float)));
+    c->res_floats = need;
+  }
+  float* spec = c->d_res;
+  dim3 grid((Tcols + STFT_FR - 1) / STFT_FR, B);
+  stft_refenc_kernel<<<grid, 256, 0, st>>>(rings, (long long)ring_cap, ring_rows, state, state_rows, (long long)geo.floats, desc,
+                                           max_new_frames, c->hp.hop_length, spec, Tcols, c->d_tw, c->d_win);
+  CK(cudaGetLastError());
+  RefencWeights P;
+  P.ln_g = c->d_w + c->re_lng; P.ln_b = c->d_w + c->re_lnb;
+  for (int i = 0; i < 6; ++i) { P.conv_w[i] = c->d_w + c->re_conv_w[i]; P.conv_b[i] = c->d_w + c->re_conv_b[i]; }
+  P.w_ih = c->d_w + c->re_wih; P.b_ih = c->d_w + c->re_bih; P.w_hh = c->d_w + c->re_whh; P.b_hh = c->d_w + c->re_bhh;
+  P.pw = c->d_w + c->re_pw; P.pb = c->d_w + c->re_pb;
+  refenc_stream_kernel<<<B, 256, 0, st>>>(P, spec, Tcols, state, state_rows, desc, ring_rows, max_new_frames, c->hp.hop_length, F, G,
+                                          spec + spec_floats, (long long)item, out);
+  CK(cudaGetLastError());
+  return OVC_OK;
 }
 
 static int resample_plan(int sr_in, int sr_out, ovc_rs::Plan* p) {

@@ -313,6 +313,19 @@ __global__ void __launch_bounds__(256) stft_mag_kernel(const float* __restrict__
 // ---------------------------------------------------------------------------------------------
 constexpr long long RING_OPEN = 0x7fffffffffffffffLL;
 
+// sample n of frame t of the stream in `ring` (cap samples), L samples long (RING_OPEN: not ended)
+__device__ __forceinline__ float ring_frame_sample(const float* __restrict__ ring, long long cap, long long L, long long t,
+                                                   int n, int hop) {
+  const long long pad = (STFT_N - hop) / 2;
+  long long idx = t * hop + n - pad;
+  if (idx < 0) idx = -idx;
+  if (L != RING_OPEN) {
+    if (idx >= L) idx = 2 * (L - 1) - idx;
+    idx = min(idx, L - 1);
+  }
+  return ring[max(idx, 0LL) % cap];
+}
+
 __global__ void __launch_bounds__(256) stft_ring_kernel(const float* __restrict__ rings, long long cap, int rows,
                                                         const long long* __restrict__ row, const long long* __restrict__ lo,
                                                         const long long* __restrict__ frames,
@@ -325,16 +338,7 @@ __global__ void __launch_bounds__(256) stft_ring_kernel(const float* __restrict_
   const int T = (int)max(0LL, min(frames[b], (long long)Tmax));
   const long long L = len[b] == RING_OPEN ? RING_OPEN : max(1LL, min(len[b], 1LL << 50));
   const float* ring = rings + r * cap;
-  const long long pad = (STFT_N - hop) / 2;
-  const auto load = [&](int t, int n) {
-    long long idx = (f0 + t) * hop + n - pad;
-    if (idx < 0) idx = -idx;
-    if (L != RING_OPEN) {
-      if (idx >= L) idx = 2 * (L - 1) - idx;
-      idx = min(idx, L - 1);
-    }
-    return ring[max(idx, 0LL) % cap];
-  };
+  const auto load = [&](int t, int n) { return ring_frame_sample(ring, cap, L, f0 + t, n, hop); };
   stft_block(load, T, t0, spec + (size_t)b * (STFT_N / 2 + 1) * Tmax, Tmax, Tmax, tw, win);
 }
 

@@ -70,6 +70,42 @@ def check_stream_length(n_in: int, hop: int, pad: int) -> None:
         raise ValueError("audio too short")
 
 
+class Enrollment:
+    """How a live stream learns its source embedding from its own audio.  Snapshot k >= 1 is the embedding of the
+    stream's first ``k * every_frames * hop`` model-rate samples (``extract_se`` of that prefix, bit for bit), for
+    ``k * every_frames <= until_frames``; each one retargets the stream's source over ``ramp_frames`` frames.  The
+    defaults are about 2 s and 10 s at 22.05 kHz.  ValueError for ``every_frames < 2``, ``until_frames < every_frames``
+    or ``ramp_frames < 0``."""
+
+    def __init__(self, every_frames: int = 172, until_frames: int = 861, ramp_frames: int = 16):
+        for name, v in (("every_frames", every_frames), ("until_frames", until_frames), ("ramp_frames", ramp_frames)):
+            if isinstance(v, bool) or int(v) != v:
+                raise ValueError(f"Enrollment: {name}={v!r} is not an integer")
+        self.every_frames, self.until_frames, self.ramp_frames = int(every_frames), int(until_frames), int(ramp_frames)
+        if self.every_frames < 2:
+            raise ValueError(f"Enrollment: every_frames must be >= 2, got {self.every_frames}")
+        if self.until_frames < self.every_frames:
+            raise ValueError(f"Enrollment: until_frames {self.until_frames} is below every_frames {self.every_frames}")
+        if self.ramp_frames < 0:
+            raise ValueError(f"Enrollment: ramp_frames must be >= 0, got {self.ramp_frames}")
+
+    def snapshot(self, n0: int, n1: int, hop: int) -> int:
+        """The snapshot a step taking a stream from n0 to n1 model-rate samples produces: the last k whose prefix
+        k * every_frames * hop lies in (n0, n1], or 0 for none."""
+        k = min(n1 // (self.every_frames * hop), self.until_frames // self.every_frames)
+        return k if k >= 1 and k * self.every_frames * hop > n0 else 0
+
+    def __repr__(self):
+        return f"Enrollment({self.every_frames}, {self.until_frames}, {self.ramp_frames})"
+
+
+def enroll_new_frames(n0: int, n1: int, hop: int, nfft: int) -> int:
+    """``max_new_frames`` of a ``reference_encoder_stream`` call taking a stream from n0 to n1 samples, rounded up to
+    64 so that steady steps reuse one workspace size."""
+    f = ready_frames(n1, hop, nfft, False) - ready_frames(n0, hop, nfft, False)
+    return max(64, -(-f // 64) * 64)
+
+
 class StreamingResampler:
     """Stateful ``ovc_resample`` (scipy.signal.resample_poly arithmetic) from ``sr_in`` to ``sr_out``.
 
@@ -165,14 +201,18 @@ def retarget_track(track, f: int, new, ramp_frames: int = 0):
 class StreamingConverter:
     def __init__(self, converter, src_se, tgt_se, tau: float = 0.3, window_frames: int = 256,
                  noise_fn: Optional[Callable[[int, int], torch.Tensor]] = None, seed: Optional[int] = None,
-                 input_sr: Optional[int] = None, output_sr: Optional[int] = None, request_seed: Optional[int] = None):
+                 input_sr: Optional[int] = None, output_sr: Optional[int] = None, request_seed: Optional[int] = None,
+                 enroll: Optional[Enrollment] = None):
         """``converter``: a ToneColorConverter.  ``noise_fn(t0, t1) -> [inter_channels, t1 - t0]`` supplies the noise of
         absolute frames [t0, t1) (tests pass slices of one tensor); default: a seeded device generator.
         ``input_sr`` / ``output_sr``: rates of the pushed and of the returned audio when they are not the model's
         (``StreamingResampler`` on each side; None: the model's rate).
         ``request_seed``: the request's own key, as ``ToneColorConverter.convert(seed=...)`` takes it: each window draws
         its noise in-kernel at its absolute frames, so the stream gives ``convert(seed=request_seed)`` and no noise is
-        kept.  It excludes ``noise_fn`` and ``seed`` (ValueError)."""
+        kept.  It excludes ``noise_fn`` and ``seed`` (ValueError).
+        ``enroll``: an ``Enrollment``: the stream learns its source embedding from its own audio (see
+        ``StreamingSessions.open``), with one reference-encoder state row and a device ring of its own.  ``src_se`` may
+        then be None: no window is converted before the first snapshot, which becomes the source from frame 0."""
         from .api import check_seeds
         if request_seed is not None:
             if noise_fn is not None or seed is not None:
@@ -196,8 +236,17 @@ class StreamingConverter:
         assert self.W >= 1
         self.tau = float(tau)
         self.dev = converter.device
-        self.src = converter._stack_se(src_se, 1)
+        if enroll is not None and not isinstance(enroll, Enrollment):
+            raise ValueError(f"enroll must be an Enrollment, got {enroll!r}")
+        if src_se is None and enroll is None:
+            raise ValueError("src_se is None: a stream without a source embedding needs enroll=Enrollment(...)")
+        self.enroll = enroll
+        self.src = None if src_se is None else converter._stack_se(src_se, 1)
         self.tgt = converter._stack_se(tgt_se, 1)
+        if enroll is not None:
+            nat = converter.model.native
+            self._est = torch.zeros(1, nat.refenc_state_floats, device=self.dev)
+            self._ering = torch.zeros(1, 4 * self.nfft, device=self.dev)
         self.tracks = {"src": None, "tgt": None}          # ToneTrack of a side once it has been retargeted
         if noise_fn is None and request_seed is None:
             gen = torch.Generator(device=self.dev)
@@ -271,8 +320,11 @@ class StreamingConverter:
         first frame no window has read yet (the frames ready so far), and is hard (``ramp_frames`` 0) or linear over
         ``ramp_frames`` frames (``retarget_track``).  Returns f.  The stream's output then equals ``convert`` on the whole
         clip with ``tone_track(side)`` as that side's embedding, bit for bit.  A window that overlaps no transition runs
-        exactly the per-item launch.  ValueError for an embedding that is not one per item."""
+        exactly the per-item launch.  ValueError for an embedding that is not one per item, and for ``src_se`` on an
+        enrolling stream without a prior that has no source yet (its first snapshot will be the source from frame 0)."""
         assert not self.closed, "the stream has been flushed"
+        if src_se is not None and self.src is None:
+            raise ValueError("retarget(src_se=...): the stream has no source before its first enrollment snapshot")
         f = self.f0 + int(self.spec.shape[2])
         for name, se in (("src", src_se), ("tgt", tgt_se)):
             if se is not None:
@@ -281,8 +333,11 @@ class StreamingConverter:
         return f
 
     def tone_track(self, name: str):
-        """The ``ToneTrack`` of side ``"src"`` or ``"tgt"`` over the whole stream so far."""
+        """The ``ToneTrack`` of side ``"src"`` or ``"tgt"`` over the whole stream so far.  ValueError for ``"src"`` of an
+        enrolling stream without a prior before its first snapshot."""
         from .api import ToneTrack
+        if name == "src" and self.src is None:
+            raise ValueError("the stream has no source embedding before its first enrollment snapshot")
         tr = self.tracks[name]
         return tr if tr is not None else ToneTrack([(0, (self.src if name == "src" else self.tgt)[0].cpu())])
 
@@ -327,18 +382,69 @@ class StreamingConverter:
         whole-clip spectrogram).  Total output = hop * (samples_in // hop) at the model's rate, as ``convert`` returns
         (then resampled to ``output_sr``)."""
         assert not self.closed
-        y = self._flush() if self.rs_in is None else np.concatenate([self._push(self.rs_in.flush()), self._flush()])
+        y = (self._flush() if self.rs_in is None else
+             np.concatenate([self._push(self.rs_in.flush(), ending=True), self._flush()]))
         return y if self.rs_out is None else np.concatenate([self.rs_out.push(y), self.rs_out.flush()])
 
-    def _push(self, x: np.ndarray) -> np.ndarray:
+    def _push(self, x: np.ndarray, ending: bool = False) -> np.ndarray:
+        """Append model-rate samples and convert the windows they complete.  A snapshot the samples produce retargets
+        the source after those windows, unless the stream is ``ending``: then it would take effect after the stream's
+        last window (as a session's closing step applies it), and is dropped."""
+        n0 = self.n_in
         self.audio = np.concatenate([self.audio, x])
         self.n_in += len(x)
+        snap = self._enroll_step(n0) if self.enroll is not None else None
         self._extend_spec(final=False)
         have = self.f0 + self.spec.shape[2]
-        outs = [self._convert_window(*w) for w in stream_windows(self.emitted, have, self.W, self.H)]
+        wins = stream_windows(self.emitted, have, self.W, self.H) if self.src is not None else []
+        outs = [self._convert_window(*w) for w in wins]
+        if snap is not None and not ending:
+            self.retarget(src_se=snap, ramp_frames=self.enroll.ramp_frames)
         return np.concatenate(outs) if outs else np.zeros(0, dtype=np.float32)
 
+    def _enroll_step(self, n0: int):
+        """Advance the stream's reference encoder over the pushed samples.  Returns the snapshot the push produces (to
+        retarget to once the push's windows are converted), or None; a stream without a source takes its first
+        snapshot as the source from frame 0."""
+        hop, pad = self.hop, self.pad
+        lo = max(0, ready_frames(n0, hop, self.nfft, False) * hop - pad)     # first sample the encoder still reads
+        at = n0
+        if self.n_in - lo > self._ering.shape[1]:         # grow: the samples [lo, n0) go to their new places too
+            self._ering = torch.zeros(1, 1 << (int((self.n_in - lo) * 1.25) - 1).bit_length(), device=self.dev)
+            at = lo
+        if self.n_in > at:
+            seg = torch.from_numpy(np.ascontiguousarray(self.audio[at - self.a0:])).to(self.dev)
+            pos = torch.from_numpy(np.arange(at, self.n_in) % self._ering.shape[1]).to(self.dev)
+            self._ering[0].index_copy_(0, pos, seg)
+        k = self.enroll.snapshot(n0, self.n_in, hop)
+        desc = torch.tensor([[0, 0, self.n_in, k * self.enroll.every_frames * hop]], dtype=torch.int64).to(self.dev)
+        out = self.conv.model.native.reference_encoder_stream(self._ering, self._est, desc,
+                                                              enroll_new_frames(n0, self.n_in, hop, self.nfft))
+        if not k:
+            return None
+        se = out.cpu()
+        if self.src is None:
+            self.src = se.to(self.dev)
+            return None
+        return se
+
+    @torch.no_grad()
+    def source_se(self):
+        """(embedding [1, gin, 1], n): ``extract_se`` of everything the stream has received (n model-rate samples),
+        bit for bit, from its encoder state in one call.  ValueError without ``enroll`` or for a stream still shorter
+        than one hop or than the STFT padding."""
+        if self.enroll is None:
+            raise ValueError("source_se needs a stream opened with enroll=Enrollment(...)")
+        n = self.n_in
+        if n < self.hop or n <= self.pad:
+            raise ValueError(f"source_se: the stream has {n} samples, needs at least {max(self.hop, self.pad + 1)}")
+        desc = torch.tensor([[0, 0, n, n]], dtype=torch.int64).to(self.dev)
+        se = self.conv.model.native.reference_encoder_stream(self._ering, self._est, desc, 1)
+        return se.cpu().reshape(1, -1, 1), n
+
     def _flush(self) -> np.ndarray:
+        if self.src is None:
+            raise ValueError("the stream ends before its first enrollment snapshot: it has no source embedding")
         self.closed = True
         check_stream_length(self.n_in, self.hop, self.pad)
         self._extend_spec(final=True)
@@ -354,7 +460,8 @@ SESSION_BATCH_FRAMES = 32768
 
 
 class _Session:
-    __slots__ = ("row", "seed", "tau", "n_in", "emitted", "in_sr", "out_sr", "raw_n", "out_n", "se", "tracks")
+    __slots__ = ("row", "seed", "tau", "n_in", "emitted", "in_sr", "out_sr", "raw_n", "out_n", "se", "tracks", "enroll",
+                 "has_src")
 
     def __init__(self, row: int, seed: int, tau: float, in_sr: Optional[int] = None, out_sr: Optional[int] = None):
         self.row, self.seed, self.tau = row, seed, tau
@@ -365,6 +472,8 @@ class _Session:
         self.out_n = 0                                    # samples returned at out_sr
         self.se = None                                    # [2, gin] host copy of the embedding table row
         self.tracks = [None, None]                        # ToneTrack of the source / target once retargeted
+        self.enroll = None                                # Enrollment of a session that learns its source
+        self.has_src = True                               # False until an enrolling session without a prior has one
 
 
 class StreamingSessions:
@@ -430,6 +539,7 @@ class StreamingSessions:
         self.cap = self.hop * (W + 2 * self.H + 8) + 4096   # samples per ring row; grows for larger pushes
         self.rings = torch.zeros(0, self.cap, device=self.dev)
         self.se = torch.zeros(2, 0, self.gin, device=self.dev)   # [src | tgt, row, gin]
+        self.est = None                                   # reference-encoder state rows of enrolling sessions
         self.next_id = 0
         self._bufs: dict = {}
         self._h2d_done = None
@@ -448,11 +558,19 @@ class StreamingSessions:
 
     # ------------------------------------------------------------------ sessions
     def open(self, src_se, tgt_se, tau: float = 0.3, seed: Optional[int] = None, input_sr: Optional[int] = None,
-             output_sr: Optional[int] = None) -> int:
+             output_sr: Optional[int] = None, enroll: Optional[Enrollment] = None) -> int:
         """Start a session converting from ``src_se`` to ``tgt_se`` (tone-colour embeddings of ``gin`` values each) and
         return its id.  ``seed``: the session's Philox key in [0, 2^64) (default: drawn from torch's generator).
         ``input_sr`` / ``output_sr``: rates of the pushed and of the returned audio, the model's or one declared with
-        ``rates`` (None: the model's); any other rate is refused."""
+        ``rates`` (None: the model's); any other rate is refused.
+
+        ``enroll``: an ``Enrollment``: the session learns its source embedding from its own model-rate audio.  Its
+        reference-encoder state row advances in every step that names it, in the step's one
+        ``ovc_reference_encoder_stream`` call.  With a prior ``src_se``, snapshot k (``extract_se`` of the first
+        ``k * every_frames * hop`` samples) takes effect exactly as ``retarget(sid, src_se=snapshot_k,
+        ramp_frames=ramp_frames)`` called right after the step whose push makes that prefix available; a step crossing
+        several boundaries applies only the last.  With ``src_se=None`` the session converts no window before its first
+        snapshot, which is the source from frame 0."""
         from .api import check_seeds
         sr = {}
         for name, rate in (("input_sr", input_sr), ("output_sr", output_sr)):
@@ -467,9 +585,15 @@ class StreamingSessions:
         if not math.isfinite(tau):
             raise ValueError(f"tau = {tau!r} is not a finite number")
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None else check_seeds([seed], 1, "seed")[0]
+        if enroll is not None and not isinstance(enroll, Enrollment):
+            raise ValueError(f"enroll must be an Enrollment, got {enroll!r}")
+        if src_se is None and enroll is None:
+            raise ValueError("src_se is None: a session without a source embedding needs enroll=Enrollment(...)")
+        if enroll is not None and self.native.refenc_state_floats == 0:
+            raise ValueError("enroll: the checkpoint has no reference encoder (ref_enc.* tensors)")
         ses = []
         for name, se in (("src_se", src_se), ("tgt_se", tgt_se)):
-            se = self._per_item_se(name, se)
+            se = torch.zeros(self.gin) if se is None else self._per_item_se(name, se)
             if se.numel() != self.gin:
                 raise ValueError(f"{name} has {se.numel()} values, the model's embeddings have {self.gin}")
             ses.append(se)
@@ -482,9 +606,35 @@ class StreamingSessions:
         self.se[:, row] = torch.stack(ses).to(self.dev)
         sid = self.next_id
         self.next_id += 1
-        self.sessions[sid] = _Session(row, seed, tau, sr["input_sr"], sr["output_sr"])
-        self.sessions[sid].se = torch.stack(ses)
+        s = self.sessions[sid] = _Session(row, seed, tau, sr["input_sr"], sr["output_sr"])
+        s.se = torch.stack(ses)
+        if enroll is not None:
+            s.enroll, s.has_src = enroll, src_se is not None
+            if self.est is None or self.est.shape[0] < self.rows:
+                self._grow_est()
+            self.est[row].zero_()
         return sid
+
+    def _grow_est(self):
+        est = torch.zeros(self.rows, self.native.refenc_state_floats, device=self.dev)
+        if self.est is not None:
+            est[: self.est.shape[0]] = self.est
+        self.est = est
+
+    @torch.no_grad()
+    def source_se(self, sid: int):
+        """(embedding [1, gin, 1], n): ``extract_se`` of everything session ``sid`` has received (n model-rate samples),
+        bit for bit, from its encoder state with one call and one sync.  ValueError for a session opened without
+        ``enroll`` or still shorter than one hop or than the STFT padding."""
+        s = self.sessions[self._check_ids([sid])[0]]
+        if s.enroll is None:
+            raise ValueError(f"session {sid} was opened without enroll")
+        n = s.n_in
+        if n < self.hop or n <= self.pad:
+            raise ValueError(f"session {sid} has {n} samples, source_se needs at least {max(self.hop, self.pad + 1)}")
+        desc = torch.tensor([[s.row, s.row, n, n]], dtype=torch.int64).to(self.dev)
+        se = self.native.reference_encoder_stream(self.rings, self.est, desc, 1)
+        return se.cpu().reshape(1, -1, 1), n
 
     def retarget(self, sid: int, src_se=None, tgt_se=None, ramp_frames: int = 0) -> int:
         """``StreamingConverter.retarget`` for session ``sid``: the change starts at the session's ready frames (the
@@ -492,8 +642,11 @@ class StreamingSessions:
         whole-clip schedule, and the session equals ``StreamingConverter`` with the same retargets bit for bit.  A step
         none of whose windows overlaps a transition runs exactly the launches it did before; one that has such windows
         adds one tone-track expansion per varying side (after a small upload of the keys) and the per-frame conditioning
-        of that side's launches.  ValueError for an embedding that is not ``gin`` values."""
+        of that side's launches.  ValueError for an embedding that is not ``gin`` values, and for ``src_se`` on an
+        enrolling session without a prior that has no source yet (its first snapshot will be the source from frame 0)."""
         s = self.sessions[self._check_ids([sid])[0]]
+        if src_se is not None and not s.has_src:
+            raise ValueError(f"retarget(src_se=...): session {sid} has no source before its first enrollment snapshot")
         f = ready_frames(s.n_in, self.hop, self.nfft, False)
         for k, se in enumerate((src_se, tgt_se)):
             if se is None:
@@ -516,16 +669,21 @@ class StreamingSessions:
         return torch.as_tensor(se, dtype=torch.float32).reshape(-1)
 
     def tone_track(self, sid: int, side: str):
-        """The ``ToneTrack`` of session ``sid``'s ``"src"`` or ``"tgt"`` embedding over its whole stream so far."""
+        """The ``ToneTrack`` of session ``sid``'s ``"src"`` or ``"tgt"`` embedding over its whole stream so far.
+        ValueError for ``"src"`` of an enrolling session without a prior before its first snapshot."""
         from .api import ToneTrack
         s = self.sessions[sid]
         k = ("src", "tgt").index(side)
+        if k == 0 and not s.has_src:
+            raise ValueError(f"session {sid} has no source embedding before its first enrollment snapshot")
         return s.tracks[k] if s.tracks[k] is not None else ToneTrack([(0, s.se[k].clone())])
 
-    def _window_tracks(self, ses, wins, b0: int, b1: int, Tmax: int, g):
+    def _window_tracks(self, ses, wins, b0: int, b1: int, Tmax: int, g, fresh=frozenset()):
         """Per side, the [b1 - b0, gin, Tmax] per-frame embeddings of launch windows b0 .. b1 - 1 when one of them
         overlaps a transition of that side (a track whose last key lies past the window's first frame), else the
-        gathered per-item rows g[side] (the launch is then exactly the per-item one)."""
+        gathered per-item rows g[side] (the launch is then exactly the per-item one).  ``fresh``: sessions whose source
+        is the first enrollment snapshot of this step, which only the device table holds: their constant windows take
+        the gathered row g[0] at each of their frames."""
         out = []
         for k in range(2):
             var = [ses[i][1].tracks[k] is not None and lo < ses[i][1].tracks[k].frames[-1]
@@ -538,6 +696,13 @@ class StreamingSessions:
             buf = self._buf(f"gpf{k}", (b1 - b0) * self.gin * Tmax, torch.float32).view(b1 - b0, self.gin, Tmax)
             out.append(expand_tone_keys(self.native, entries, [lo for _, lo, _, _, _ in wins[b0:b1]],
                                         [hi - lo for _, lo, hi, _, _ in wins[b0:b1]], Tmax, buf, ("src_se", "tgt_se")[k]))
+            fix = [j for j, (v, (i, _, _, _, _)) in enumerate(zip(var, wins[b0:b1])) if k == 0 and not v and i in fresh]
+            if fix:
+                ix = torch.tensor(fix, dtype=torch.int64).to(self.dev)
+                n = torch.tensor([wins[b0 + j][2] - wins[b0 + j][1] for j in fix], dtype=torch.int64).to(self.dev)
+                keep = (torch.arange(Tmax, device=self.dev)[None, :] < n[:, None])[:, None, :]
+                rows = g[k][b0:b1].index_select(0, ix)[:, :, None].expand(-1, -1, Tmax)
+                out[-1].index_copy_(0, ix, torch.where(keep, rows, torch.zeros((), device=self.dev)))
         return out
 
     @property
@@ -617,6 +782,7 @@ class StreamingSessions:
                     raise ValueError(f"session {sid}: run {(r, o, n)} is not inside src {tuple(src.shape)}")
         for sid in close:
             check_stream_length(self._model_len(self.sessions[sid], sum(n for _, _, n in xs[sid])), self.hop, self.pad)
+            self._check_has_src(sid, self._model_len(self.sessions[sid], sum(n for _, _, n in xs[sid])))
         out = self._step(xs, final=close, src=src)
         for sid in close:
             self.free_rows.append(self.sessions.pop(sid).row)
@@ -630,10 +796,19 @@ class StreamingSessions:
         ids = self._check_ids(ids)
         for sid in ids:
             check_stream_length(self._model_len(self.sessions[sid], 0), self.hop, self.pad)
+            self._check_has_src(sid, self._model_len(self.sessions[sid], 0))
         out = self._step({sid: np.zeros(0, dtype=np.float32) for sid in ids}, final=set(ids))
         for sid in ids:
             self.free_rows.append(self.sessions.pop(sid).row)
         return out
+
+    def _check_has_src(self, sid: int, n: int) -> None:
+        """ValueError for a session without a prior that would end (at n model-rate samples) before its first
+        snapshot, so it would have no source embedding to convert with."""
+        s = self.sessions[sid]
+        if not s.has_src and not s.enroll.snapshot(s.n_in, n, self.hop):
+            raise ValueError(f"session {sid} ends before its first enrollment snapshot: it has no source embedding "
+                             f"(discard it instead)")
 
     def discard(self, ids: Iterable[int]) -> None:
         """Drop the named sessions without converting what is left of them (a caller that has gone away) and free their
@@ -675,6 +850,8 @@ class StreamingSessions:
             self.raw = self._moved(self.raw, rows, self.raw.shape[1], [])
             self.orings = self._moved(self.orings, rows, self.orings.shape[1], [])
         self.rings, self.se, self.rows, self.cap = rings, se, rows, cap
+        if self.est is not None and self.est.shape[0] < rows:
+            self._grow_est()
 
     def _splice(self, source: torch.Tensor, seg: torch.Tensor, segs: List[Tuple[int, int, int, int, int]],
                 dst: torch.Tensor):
@@ -722,9 +899,18 @@ class StreamingSessions:
         if self.raw is not None and need > self.raw.shape[1]:
             live = [(s.row, self._raw_keep(s), s.raw_n) for s in self.sessions.values() if s.in_sr]
             self.raw = self._moved(self.raw, self.rows, -(-int(need * 1.25) // 1024) * 1024, live)
+        # enrolling sessions: (session index, snapshot k of the step or 0); first: the items (in enr) of sessions whose
+        # first snapshot becomes their source in this step
+        enr = [(i, s.enroll.snapshot(s.n_in, s.n_in + n, hop)) for i, ((_, s, _), n) in enumerate(zip(ses, gains))
+               if s.enroll is not None]
+        first = [b for b, (i, k) in enumerate(enr) if k and not ses[i][1].has_src]
+        no_src = {i for i, k in enr if not k and not ses[i][1].has_src}
+        nE, nF, gin = len(enr), len(first), self.gin
         # windows of every named session: (session index, lo, hi, e0, e1)
         wins = []
         for i, ((sid, s, _), n) in enumerate(zip(ses, gains)):
+            if i in no_src:                               # nothing to convert with yet
+                continue
             have = ready_frames(s.n_in + n, hop, self.nfft, sid in final)
             wins += [(i,) + w for w in stream_windows(s.emitted, have, self.W, H, sid in final)]
         # splice segments: each run to the ring row (raw ring row when the session resamples its input) of its session,
@@ -767,14 +953,16 @@ class StreamingSessions:
         # packed upload (int64 words): row, lo, frames, stream length, seed, stream (0), embedding rows (2B), tau (float32),
         # then the emitted frames' rows of the output, the splice segments (5 words each), the raw splice segments, the
         # input resampling items (6 words each, then their plans as int32), the output splice segments, the output
-        # resampling items and the pushed samples (float32)
+        # resampling items, the encoder descriptors (4 words each) with the first snapshots' items and embedding table
+        # rows, and the pushed samples (float32)
         nt = (B + 1) // 2
         o = 8 * B + nt + Nf
         o_r = o + 5 * nS
         o_i = o_r + 5 * nR
         o_o = o_i + 6 * nI + (nI + 1) // 2
         o_q = o_o + 5 * nO
-        o_s = o_q + 6 * nQ + (nQ + 1) // 2
+        o_e = o_q + 6 * nQ + (nQ + 1) // 2
+        o_s = o_e + 4 * nE + 2 * nF
         n_words = o_s + (Ns + 1) // 2
         if self._h2d_done is not None:
             self._h2d_done.synchronize()                  # the previous step's upload has left the pinned buffer
@@ -801,6 +989,12 @@ class StreamingSessions:
                 v = np.asarray(it, dtype=np.int64)
                 w[at:at + 6 * len(it)] = v[:, 1:].T.reshape(-1)
                 w[at + 6 * len(it):at + 6 * len(it) + (len(it) + 1) // 2].view(np.int32)[:len(it)] = v[:, 0]
+        if nE:
+            w[o_e:o_e + 4 * nE] = np.asarray([[ses[i][1].row, ses[i][1].row, ses[i][1].n_in + gains[i],
+                                               k * ses[i][1].enroll.every_frames * hop] for i, k in enr],
+                                             dtype=np.int64).reshape(-1)
+            w[o_e + 4 * nE:o_e + 4 * nE + nF] = first
+            w[o_e + 4 * nE + nF:o_s] = [ses[enr[b][0]][1].row for b in first]
         if Ns:
             w[o_s:].view(np.float32)[:Ns] = np.concatenate([x for _, _, x in ses])
         d = self._buf("up", n_words, torch.int64)
@@ -817,6 +1011,15 @@ class StreamingSessions:
         if nI:
             self._resample_rings(d, o_i, nI, self.raw, self.rings, max(it[4] for it in rin))
         res = {sid: np.zeros(0, dtype=np.float32) for sid, _, _ in ses}
+        snaps = [b for b, (_, k) in enumerate(enr) if k]
+        ybuf = self._buf("y", Nf * hop + No + (nE * gin if snaps else 0), torch.float32)
+        if nE:                                            # after the splice and the resampling: the samples are in
+            eout = ybuf[Nf * hop + No:Nf * hop + No + nE * gin].view(nE, gin) if snaps else \
+                self._buf("e", nE * gin, torch.float32).view(nE, gin)
+            M = max(enroll_new_frames(ses[i][1].n_in, ses[i][1].n_in + gains[i], hop, self.nfft) for i, _ in enr)
+            self.native.reference_encoder_stream(self.rings, self.est, d[o_e:o_e + 4 * nE].view(nE, 4), M, out=eout)
+            if nF:                                        # first snapshots are the sources of this step's windows
+                self.se[0].index_copy_(0, d[o_e + 4 * nE + nF:o_s], eout.index_select(0, d[o_e + 4 * nE:o_e + 4 * nE + nF]))
         if B:
             spec = self._buf("spec", B * self.S * Tmax, torch.float32).view(B, self.S, Tmax)
             self.native.spectrogram_ring(self.rings, d[0:B], d[B:2 * B], d[2 * B:3 * B], d[3 * B:4 * B], Tmax, out=spec)
@@ -829,18 +1032,18 @@ class StreamingSessions:
                 b1 = min(B, b0 + per)
                 items = {"seed": d[4 * B + b0:4 * B + b1], "stream": d[5 * B + b0:5 * B + b1],
                          "frame0": d[B + b0:B + b1], "tau": taus[b0:b1]}
-                gs, gt = self._window_tracks(ses, wins, b0, b1, Tmax, (g[:B], g[B:]))
+                gs, gt = self._window_tracks(ses, wins, b0, b1, Tmax, (g[:B], g[B:]), {enr[b][0] for b in first})
                 self.native.voice_conversion(spec[b0:b1], d[2 * B + b0:2 * B + b1], gs, gt,
                                              ragged=True, latents=False, items=items,
                                              out=obuf[b0 * Tmax * hop:b1 * Tmax * hop])
             fo = 8 * B + nt
-            ybuf = self._buf("y", Nf * hop + No, torch.float32)
             y = torch.index_select(obuf.view(B * Tmax, hop), 0, d[fo:fo + Nf], out=ybuf[:Nf * hop].view(Nf, hop))
             if nO:
                 self._splice(y.view(1, Nf * hop), d[o_o:o_o + 5 * nO].view(nO, 5), osegs, self.orings)
             if nQ:
                 self._resample_rings(d, o_q, nQ, self.orings, ybuf.view(1, -1), max(it[4] for it in rout))
-            host = self._buf("host", Nf * hop + No, torch.float32, pinned=True)
+        if B or snaps:
+            host = self._buf("host", ybuf.numel(), torch.float32, pinned=True)
             host.copy_(ybuf, non_blocking=True)
             if self.cuda:
                 torch.cuda.current_stream(self.dev).synchronize()
@@ -862,6 +1065,13 @@ class StreamingSessions:
             s.raw_n += counts[i] if s.in_sr is not None else 0
             s.out_n += qn[i]
             s.emitted = emitted[i]
+        for b in snaps:                                   # each snapshot takes effect after the step
+            sid, s, _ = ses[enr[b][0]]
+            se = torch.from_numpy(y[Nf * hop + No + b * gin:Nf * hop + No + (b + 1) * gin].copy())
+            if s.has_src:
+                self.retarget(sid, src_se=se, ramp_frames=s.enroll.ramp_frames)
+            else:
+                s.se[0], s.has_src = se, True
         return res
 
     def _resample_rings(self, d: torch.Tensor, at: int, n: int, src: torch.Tensor, dst: torch.Tensor, max_count: int):
