@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 16 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 17 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
@@ -35,7 +35,9 @@ extern "C" {
                                * 14: ovc_voice_conversion_frames, ovc_convert_waveform_frames, ovc_tone_track_expand;
                                * 15: ovc_tts_encode_g, ovc_tts_encode_state_tokens, ovc_tts_decode_windows_tokens,
                                *     ovc_tts_encode_state_rows_tokens, ovc_tts_state_rows_tokens;
-                               * 16: ovc_reference_encoder_stream, ovc_reference_encoder_stream_state_floats */
+                               * 16: ovc_reference_encoder_stream, ovc_reference_encoder_stream_state_floats;
+                               * 17: ovc_generate_frames, o_hat NULL on ovc_voice_conversion_frames (the latent half),
+                               *     OVC_SPLICE_SRC_WRAP */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -187,6 +189,11 @@ OVC_API int ovc_philox_normals(uint64_t seed, int64_t stream, int64_t c0, int C,
  *         wav and read back as float: libsndfile's default float -> PCM_16 write (scale by 32767, round to nearest)
  *         and its PCM_16 -> float read (divide by 32768), which is what librosa.load returns for such a file. */
 #define OVC_SPLICE_PCM16 1
+/*   flags OVC_SPLICE_SRC_WRAP: the source rows are rings as well: element i reads
+ *         src[src_row * src_pitch + (src_off + i) mod src_pitch] (src_off is reduced mod src_pitch on the device and the
+ *         count is no longer cut at the end of the source row).  This gathers runs that wrap around a ring row, such as a
+ *         live stream's latent frames, into a padded batch.  The flags combine. */
+#define OVC_SPLICE_SRC_WRAP 2
 OVC_API int ovc_splice(const float* src, int64_t src_rows, int64_t src_pitch, float* dst, int64_t dst_rows, int64_t dst_cap,
                        const int64_t* seg, int S, int flags, void* stream);
 
@@ -252,6 +259,24 @@ OVC_API int ovc_convert_waveform_frames(ovc_ctx* ctx, const float* wav, const in
                                         const float* g_src, const float* g_tgt, int se_frames, const float* noise,
                                         uint64_t seed, float tau, float* o_hat, int64_t* frames, void* stream,
                                         const ovc_item_params* items);
+
+/* The conversion in two halves, split at z_hat (the flow reverse's output, the generator's input).
+ *
+ * Latent half: ovc_voice_conversion_frames with o_hat == NULL runs the posterior encoder and both flow passes and
+ * writes whichever of z, z_p, z_hat are given (at least one output must be); the generator does not run.  Everything
+ * else (ragged, per-item parameters, se_frames, graph replay) is as with o_hat given, and the latents are the ones that
+ * call writes, bit for bit.
+ *
+ * Generator half: the HiFi-GAN generator on a caller's z_hat, each item at its own length (ragged).
+ *   z_hat    [B, inter, Tmax] fp32; frames past lengths[b] are not read
+ *   lengths  [B] int64 (device), 1 <= len <= Tmax
+ *   g_tgt    [B, gin] per item, or with se_frames = OVC_SE_FRAMES_TGT [B, gin, Tmax] per frame (the source side does not
+ *            reach the generator, so OVC_SE_FRAMES_SRC is refused)
+ *   o_hat    [B, hop*Tmax] out, zero past hop*len
+ * Given the z_hat an ovc_voice_conversion_frames call (ragged = 1) writes, with the same lengths and target, o_hat equals
+ * that call's o_hat bit for bit.  Same workspace as the voice conversion; replayed from a CUDA graph like it. */
+OVC_API int ovc_generate_frames(ovc_ctx* ctx, const float* z_hat, const int64_t* lengths, const float* g_tgt, int se_frames,
+                                int B, int Tmax, float* o_hat, void* stream);
 
 /* Per-frame embeddings from keyframe tracks ("tone tracks").  Keys are n_keys pairs (key_frame[k], key_se[k, 0:gin]);
  * track b is keys [key0[b], key0[b] + nkeys[b]) with non-decreasing frames.  out[b, c, t] = g_b(frame0[b] + t) for

@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 16
+ABI_VERSION = 17
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -27,10 +27,12 @@ EXPORTS = (
     "ovc_voice_conversion_frames", "ovc_convert_waveform_frames", "ovc_tone_track_expand",
     "ovc_tts_encode_g", "ovc_tts_encode_state_tokens", "ovc_tts_decode_windows_tokens", "ovc_tts_encode_state_rows_tokens",
     "ovc_tts_state_rows_tokens", "ovc_reference_encoder_stream", "ovc_reference_encoder_stream_state_floats",
+    "ovc_generate_frames",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample / ovc_spectrogram_ring length of a stream that has not ended
 SPLICE_PCM16 = 1            # ovc_splice flag: the 16-bit PCM round trip of every copied value
+SPLICE_SRC_WRAP = 2         # ovc_splice flag: source rows are rings, src_off + i wraps mod the source pitch
 SE_FRAMES_SRC, SE_FRAMES_TGT = 1, 2   # ovc_*_frames: the side's embedding is given per frame
 
 
@@ -194,6 +196,7 @@ def load_library(path: Optional[str] = None):
     lib.ovc_reference_encoder_stream_state_floats.argtypes = [C.c_void_p]
     lib.ovc_reference_encoder_stream.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p,
                                                  C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib.ovc_generate_frames.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     if lib.ovc_abi_version() != ABI_VERSION:
         raise OvcError(f"ABI mismatch: library {lib.ovc_abi_version()} vs binding {ABI_VERSION}")
     _lib = lib
@@ -362,6 +365,56 @@ class NativeConverter:
             C.c_void_p(st.cuda_stream), _items_ref(it))
         _check(self.lib, rc, "ovc_voice_conversion")
         return o, lat
+
+    def latent(self, spec, lengths, g_src, g_tgt, items: Optional[dict] = None, out=None, stream=None):
+        """The latent half of ``voice_conversion`` (ragged): posterior encoder, flow forward with g_src, flow reverse
+        with g_tgt, and no generator (``ovc_voice_conversion_frames`` with o_hat NULL).  Arguments as there; ``out``: a
+        caller-owned z_hat buffer of B * inter * T floats.  Returns z_hat [B, inter, T], bit for bit the z_hat
+        ``voice_conversion(..., ragged=True)`` returns.  Asynchronous on `stream`."""
+        import torch
+        assert spec.is_cuda and spec.dtype == torch.float32 and spec.is_contiguous()
+        assert lengths.is_cuda and lengths.dtype == torch.int64 and lengths.is_contiguous()
+        B, S, T = spec.shape
+        gs, fs = se_arg(g_src, B, self.hp.gin_channels, T, "g_src")
+        gt, ft = se_arg(g_tgt, B, self.hp.gin_channels, T, "g_tgt")
+        C_ = self.hp.inter_channels
+        if out is not None:
+            assert out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == B * C_ * T
+            z = out.view(B, C_, T)
+        else:
+            z = torch.empty(B, C_, T, device=spec.device, dtype=torch.float32)
+        st = stream if stream is not None else torch.cuda.current_stream(spec.device)
+        p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+        rc = self.lib.ovc_voice_conversion_frames(
+            self.handle, p(spec), p(lengths), p(gs), p(gt), (SE_FRAMES_SRC if fs else 0) | (SE_FRAMES_TGT if ft else 0),
+            None, C.c_uint64(0), C.c_float(0.3), B, T, 1, None, None, None, p(z), C.c_void_p(st.cuda_stream),
+            _items_ref(item_params(items, B)))
+        _check(self.lib, rc, "ovc_voice_conversion_frames (latent half)")
+        return z
+
+    def generate(self, z_hat, lengths, g_tgt, out=None, stream=None):
+        """The generator half (``ovc_generate_frames``): z_hat [B, inter, T] f32 cuda, lengths [B] i64 cuda (each item at
+        its own length), g_tgt [B, gin(,1)] per item or [B, gin, T] per frame.  ``out``: a caller-owned o_hat buffer of
+        B * hop * T floats.  Returns o_hat [B, 1, hop * T]; on ``latent``'s z_hat it equals ``voice_conversion(...,
+        ragged=True)``'s o_hat bit for bit.  Asynchronous on `stream`."""
+        import torch
+        assert z_hat.is_cuda and z_hat.dtype == torch.float32 and z_hat.is_contiguous()
+        assert lengths.is_cuda and lengths.dtype == torch.int64 and lengths.is_contiguous()
+        B, _, T = z_hat.shape
+        assert z_hat.shape[1] == self.hp.inter_channels
+        gt, ft = se_arg(g_tgt, B, self.hp.gin_channels, T, "g_tgt")
+        hop = self.hp.hop_length
+        if out is not None:
+            assert out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.numel() == B * hop * T
+            o = out.view(B, 1, hop * T)
+        else:
+            o = torch.empty(B, 1, hop * T, device=z_hat.device, dtype=torch.float32)
+        st = stream if stream is not None else torch.cuda.current_stream(z_hat.device)
+        p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+        rc = self.lib.ovc_generate_frames(self.handle, p(z_hat), p(lengths), p(gt), SE_FRAMES_TGT if ft else 0, B, T, p(o),
+                                          C.c_void_p(st.cuda_stream))
+        _check(self.lib, rc, "ovc_generate_frames")
+        return o
 
     def spectrogram(self, wav, wav_lengths, stream=None):
         """wav [B, Lmax] f32 cuda (zero padded), wav_lengths [B] i64 cuda (samples) ->
@@ -598,12 +651,13 @@ class NativeConverter:
         _check(self.lib, rc, "ovc_resample_rings")
         return out
 
-    def splice(self, src, seg, dst, pcm16: bool = False, stream=None):
+    def splice(self, src, seg, dst, pcm16: bool = False, stream=None, src_wrap: bool = False):
         """Copy sample runs between device buffers in one launch (include/ovc.h: ovc_splice).  src [rows, pitch] f32
         cuda, or None when every segment is a gap; seg [S, 5] int64 cuda, rows (src_row, src_off, count, dst_row,
         dst_off); dst [rows, cap] f32 cuda, written in place: segment s puts src[src_row, src_off + i] (0 when src_row
         < 0) at dst[dst_row, (dst_off + i) % cap], i < count.  ``pcm16``: every copied value takes the 16-bit PCM round
-        trip (``SPLICE_PCM16``).  Asynchronous on `stream`; returns ``dst``."""
+        trip (``SPLICE_PCM16``).  ``src_wrap``: the source rows are rings too, segment s reads
+        src[src_row, (src_off + i) % pitch] (``SPLICE_SRC_WRAP``).  Asynchronous on `stream`; returns ``dst``."""
         import torch
         assert dst.is_cuda and dst.dtype == torch.float32 and dst.is_contiguous() and dst.dim() == 2
         assert seg.is_cuda and seg.dtype == torch.int64 and seg.is_contiguous()
@@ -617,7 +671,8 @@ class NativeConverter:
         with torch.cuda.device(dst.device):
             rc = self.lib.ovc_splice(None if src is None else C.c_void_p(src.data_ptr()), rows, pitch,
                                      C.c_void_p(dst.data_ptr()), int(dst.shape[0]), int(dst.shape[1]),
-                                     C.c_void_p(seg.data_ptr()), int(seg.shape[0]), SPLICE_PCM16 if pcm16 else 0,
+                                     C.c_void_p(seg.data_ptr()), int(seg.shape[0]),
+                                     (SPLICE_PCM16 if pcm16 else 0) | (SPLICE_SRC_WRAP if src_wrap else 0),
                                      C.c_void_p(st.cuda_stream))
         _check(self.lib, rc, "ovc_splice")
         return dst

@@ -1490,8 +1490,38 @@ static int run_vc(ovc_ctx* c, const float* spec, int spec_pitch, const long long
   TRY(copy_latent(zp_out));
   TRY(run_flow(r, W, ws, true, cr[2]));
   TRY(copy_latent(zh_out));
+  if (!o_hat) return OVC_OK;   // the latent half alone (ovc_voice_conversion_frames with o_hat NULL)
 
   return run_dec(r, W, ws, cr[3], lens, o_hat);
+}
+
+// The generator half of run_vc: z_hat [B][192][Tmax] from the caller (zero from each length on, as the flow leaves it
+// masked) through the same conditioning and run_dec, so a latent-half call followed by this one is run_vc bit for bit.
+// Only the target side is read: the per-item launch computes every column (the source columns read zeros and go
+// unread), a per-frame target only the generator's section of its per-frame columns.
+static int run_gen(ovc_ctx* c, const float* z_hat, const long long* lens, const float* g_tgt, int se_frames, int B, int Tmax,
+                   float* o_hat, cudaStream_t st) {
+  const WsLayout W = ws_layout(c, B, Tmax, cond_pf_cols(c, se_frames));
+  TRY(ensure_ws(c, W, B, Tmax, st));
+  float* ws = c->d_ws;
+  Run r{c, st, B, Tmax, W.P, lens, lens, (double)B * Tmax};
+  c->launches = 0;
+  const int o = c->precision >= 1;
+  const bool tgt_pf = se_frames & OVC_SE_FRAMES_TGT;
+  TRY(launch_cond(c, st, B, 1, nullptr, c->cond_rows_out, cond_side(c, nullptr, false, Tmax),
+                  cond_side(c, tgt_pf ? nullptr : g_tgt, false, Tmax), ws + W.cond, c->cond_rows_out, 0));
+  const int pf = tgt_pf ? c->cond_pf_off[o][OVC_SE_FRAMES_TGT - 1][3] : -1;   // -1: zero_g, the generator reads no g
+  const int n_dec = 512;   // the generator's section: dec.cond rows (ovc_finalize_weights)
+  if (pf >= 0)
+    TRY(launch_cond(c, st, B, Tmax, c->d_cond_cols[o][OVC_SE_FRAMES_TGT - 1] + pf, n_dec, cond_side(c, nullptr, true, Tmax),
+                    cond_side(c, g_tgt, true, Tmax), ws + W.cond_pf, (long long)Tmax * n_dec, n_dec));
+  const CondRef cr = pf < 0 ? CondRef{ws + W.cond + c->cond_off_dec, c->cond_rows_out, 0}
+                            : CondRef{ws + W.cond_pf, (long long)Tmax * n_dec, n_dec};
+  dim3 grid((W.P + 255) / 256, 192, B);
+  latent_in_kernel<<<grid, 256, 0, st>>>(z_hat, Tmax, ws + W.z, W.P, 192, lens);
+  CK(cudaGetLastError());
+  c->launches++;
+  return run_dec(r, W, ws, cr, lens, o_hat);
 }
 
 #include "ovc_tts_run.inc"    // run_tts_encode() / run_tts_decode(): SynthesizerTrn.infer on the device
@@ -1607,7 +1637,8 @@ int ovc_voice_conversion_frames(ovc_ctx* c, const float* spec, const int64_t* le
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (se_frames & ~(OVC_SE_FRAMES_SRC | OVC_SE_FRAMES_TGT)) return fail(OVC_ERR_INVALID, "unknown se_frames bits 0x%x", se_frames);
   if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
-  if (!spec || !lengths || !g_src || !g_tgt || !o_hat) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (!spec || !lengths || !g_src || !g_tgt) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (!o_hat && !z && !z_p && !z_hat) return fail(OVC_ERR_INVALID, "no output: o_hat, z, z_p and z_hat are all NULL");
   if (B < 1 || Tmax < 1) return fail(OVC_ERR_INVALID, "B and Tmax must be positive (got %d, %d)", B, Tmax);
   if ((long long)Tmax * 256 * 64 > 2000000000LL) return fail(OVC_ERR_INVALID, "Tmax %d too large for 32-bit indexing", Tmax);
   if (B > 65535) return fail(OVC_ERR_INVALID, "B %d exceeds the grid limit", B);
@@ -1624,6 +1655,27 @@ int ovc_voice_conversion_frames(ovc_ctx* c, const float* spec, const int64_t* le
   return run_graphed(c, key, st, [&](cudaStream_t s) {
     return run_vc(c, spec, Tmax, (const long long*)lengths, g_src, g_tgt, se_frames, noise, seed, tau, B, Tmax, ragged, o_hat, z,
                   z_p, z_hat, s);
+  });
+}
+
+int ovc_generate_frames(ovc_ctx* c, const float* z_hat, const int64_t* lengths, const float* g_tgt, int se_frames, int B,
+                        int Tmax, float* o_hat, void* stream) {
+  if (!c) return fail(OVC_ERR_INVALID, "null context");
+  if (se_frames & ~OVC_SE_FRAMES_TGT)
+    return fail(OVC_ERR_INVALID, "ovc_generate_frames: se_frames 0x%x (the generator reads the target side only)", se_frames);
+  if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
+  if (!z_hat || !lengths || !g_tgt || !o_hat) return fail(OVC_ERR_INVALID, "null tensor argument");
+  if (B < 1 || Tmax < 1) return fail(OVC_ERR_INVALID, "B and Tmax must be positive (got %d, %d)", B, Tmax);
+  if ((long long)Tmax * 256 * 64 > 2000000000LL) return fail(OVC_ERR_INVALID, "Tmax %d too large for 32-bit indexing", Tmax);
+  if (B > 65535) return fail(OVC_ERR_INVALID, "B %d exceeds the grid limit", B);
+  ON_DEVICE(c);
+  c->ev_used = c->prof ? c->ev_used : 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  TRY(ensure_ws(c, ws_layout(c, B, Tmax, cond_pf_cols(c, se_frames)), B, Tmax, st));
+  const std::vector<uintptr_t> key = {4, (uintptr_t)z_hat, (uintptr_t)lengths, (uintptr_t)g_tgt, (uintptr_t)o_hat, (uintptr_t)B,
+                                      (uintptr_t)Tmax, option_bits(c), (uintptr_t)se_frames};
+  return run_graphed(c, key, st, [&](cudaStream_t s) {
+    return run_gen(c, z_hat, (const long long*)lengths, g_tgt, se_frames, B, Tmax, o_hat, s);
   });
 }
 
@@ -2255,7 +2307,7 @@ int ovc_philox_normals(uint64_t seed, int64_t stream, int64_t c0, int C, int64_t
   return OVC_OK;
 }
 
-static_assert(OVC_SPLICE_PCM16 == ovc_sp::PCM16, "ovc_splice flag");
+static_assert(OVC_SPLICE_PCM16 == ovc_sp::PCM16 && OVC_SPLICE_SRC_WRAP == ovc_sp::SRC_WRAP, "ovc_splice flags");
 
 int ovc_splice(const float* src, int64_t src_rows, int64_t src_pitch, float* dst, int64_t dst_rows, int64_t dst_cap,
                const int64_t* seg, int S, int flags, void* stream) {
@@ -2264,7 +2316,7 @@ int ovc_splice(const float* src, int64_t src_rows, int64_t src_pitch, float* dst
     return fail(OVC_ERR_INVALID, "ovc_splice: bad destination (rows %lld, cap %lld)", (long long)dst_rows, (long long)dst_cap);
   if (src_rows < 0 || (src_rows > 0 && (!src || src_pitch < 1)))
     return fail(OVC_ERR_INVALID, "ovc_splice: bad source (rows %lld, pitch %lld)", (long long)src_rows, (long long)src_pitch);
-  if (flags & ~OVC_SPLICE_PCM16) return fail(OVC_ERR_INVALID, "ovc_splice: unknown flags %d", flags);
+  if (flags & ~(OVC_SPLICE_PCM16 | OVC_SPLICE_SRC_WRAP)) return fail(OVC_ERR_INVALID, "ovc_splice: unknown flags %d", flags);
   if (S == 0) return OVC_OK;
   const int gy = S < 65535 ? S : 65535;
   const int gx = std::max(1, std::min(1024, 2048 / gy));

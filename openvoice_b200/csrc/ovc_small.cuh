@@ -216,6 +216,17 @@ __global__ void __launch_bounds__(256) copy_latent_kernel(const float* __restric
   dst[((size_t)b * C + c) * tmax + t] = v;
 }
 
+// latent copy-in, the inverse: caller [B][C][tmax] -> internal [B][C][pitch] (pitch >= tmax), zero from the length on,
+// so the generator reads a caller's z_hat exactly as it reads the one the flow left in the workspace
+__global__ void __launch_bounds__(256) latent_in_kernel(const float* __restrict__ src, int tmax, float* __restrict__ dst,
+                                                        int pitch, int C, const long long* lens) {
+  const int b = blockIdx.z, c = blockIdx.y;
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= pitch) return;
+  const int len = (int)max(0LL, min((long long)tmax, lens[b]));
+  dst[((size_t)b * C + c) * pitch + t] = t < len ? src[((size_t)b * C + c) * tmax + t] : 0.f;
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // stft_mag_kernel: the linear-spectrogram front end of convert (mel_processing.py:40-75):

@@ -3,7 +3,8 @@
 //
 //   dst[dst_row * dst_cap + (dst_off + i) mod dst_cap] = f(src[src_row * src_pitch + src_off + i])   (0 if src_row < 0)
 //
-// with f the identity, or with PCM16 the int16 round trip of pcm16() below.  load_seg clamps every descriptor value, so
+// with f the identity, or with PCM16 the int16 round trip of pcm16() below.  With SRC_WRAP the source is a ring too: the
+// element read is src[src_row * src_pitch + (src_off + i) mod src_pitch].  load_seg clamps every descriptor value, so
 // no element is read or written outside src [src_rows][src_pitch] or dst [dst_rows][dst_cap] whatever the table holds.
 // The functions are OVC_HD so that the kernel and tests/hostcheck/splice_host.cpp evaluate the same expressions.
 #pragma once
@@ -20,7 +21,8 @@
 
 namespace ovc_sp {
 
-constexpr int PCM16 = 1;   // OVC_SPLICE_PCM16
+constexpr int PCM16 = 1;      // OVC_SPLICE_PCM16
+constexpr int SRC_WRAP = 2;   // OVC_SPLICE_SRC_WRAP
 
 struct Seg {
   int64_t src_row, src_off, count, dst_row, dst_off;
@@ -31,8 +33,10 @@ OVC_HD int64_t clamp64(int64_t v, int64_t lo, int64_t hi) { return v < lo ? lo :
 // Segment s, clamped: dst_row into [0, dst_rows), dst_off reduced mod dst_cap into [0, dst_cap), count into
 // [0, dst_cap] (a segment never writes a ring slot twice).  A source row < 0 (or a call without source rows) is a gap
 // of zeros; any other source row is clamped into [0, src_rows), src_off into [0, src_pitch], and count to the samples
-// left in the source row after src_off.
-OVC_HD Seg load_seg(const int64_t* seg, int64_t s, int64_t src_rows, int64_t src_pitch, int64_t dst_rows, int64_t dst_cap) {
+// left in the source row after src_off -- or, with SRC_WRAP, src_off is reduced mod src_pitch into [0, src_pitch) and the
+// count is not limited by the source (its reads wrap).
+OVC_HD Seg load_seg(const int64_t* seg, int64_t s, int64_t src_rows, int64_t src_pitch, int64_t dst_rows, int64_t dst_cap,
+                    int flags = 0) {
   const int64_t* v = seg + 5 * s;
   Seg g;
   g.dst_row = clamp64(v[3], 0, dst_rows - 1);
@@ -44,8 +48,13 @@ OVC_HD Seg load_seg(const int64_t* seg, int64_t s, int64_t src_rows, int64_t src
     g.src_off = 0;
   } else {
     g.src_row = v[0] < src_rows ? v[0] : src_rows - 1;
-    g.src_off = clamp64(v[1], 0, src_pitch);
-    if (g.count > src_pitch - g.src_off) g.count = src_pitch - g.src_off;
+    if (flags & SRC_WRAP) {
+      g.src_off = v[1] % src_pitch;
+      if (g.src_off < 0) g.src_off += src_pitch;
+    } else {
+      g.src_off = clamp64(v[1], 0, src_pitch);
+      if (g.count > src_pitch - g.src_off) g.count = src_pitch - g.src_off;
+    }
   }
   return g;
 }
@@ -73,7 +82,8 @@ OVC_HD float pcm16(float x) {
 
 OVC_HD float value(const Seg& g, const float* src, int64_t src_pitch, int64_t i, int flags) {
   if (g.src_row < 0) return 0.0f;
-  const float x = src[g.src_row * src_pitch + g.src_off + i];
+  const int64_t j = (flags & SRC_WRAP) ? (g.src_off + i) % src_pitch : g.src_off + i;
+  const float x = src[g.src_row * src_pitch + j];
   return (flags & PCM16) ? pcm16(x) : x;
 }
 
@@ -83,7 +93,7 @@ __global__ void __launch_bounds__(256) splice_kernel(const float* __restrict__ s
                                                      const int64_t* __restrict__ seg, int S, float* __restrict__ dst,
                                                      int64_t dst_rows, int64_t dst_cap, int flags) {
   for (int s = blockIdx.y; s < S; s += gridDim.y) {
-    const Seg g = load_seg(seg, s, src_rows, src_pitch, dst_rows, dst_cap);
+    const Seg g = load_seg(seg, s, src_rows, src_pitch, dst_rows, dst_cap, flags);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < g.count; i += (int64_t)gridDim.x * blockDim.x)
       dst[dst_index(g, i, dst_cap)] = value(g, src, src_pitch, i, flags);
   }

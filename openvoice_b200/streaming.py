@@ -461,7 +461,7 @@ SESSION_BATCH_FRAMES = 32768
 
 class _Session:
     __slots__ = ("row", "seed", "tau", "n_in", "emitted", "in_sr", "out_sr", "raw_n", "out_n", "se", "tracks", "enroll",
-                 "has_src")
+                 "has_src", "lat")
 
     def __init__(self, row: int, seed: int, tau: float, in_sr: Optional[int] = None, out_sr: Optional[int] = None):
         self.row, self.seed, self.tau = row, seed, tau
@@ -474,6 +474,7 @@ class _Session:
         self.tracks = [None, None]                        # ToneTrack of the source / target once retargeted
         self.enroll = None                                # Enrollment of a session that learns its source
         self.has_src = True                               # False until an enrolling session without a prior has one
+        self.lat = 0                                      # StagedSessions: frames whose final latents are in its ring
 
 
 class StreamingSessions:
@@ -678,14 +679,14 @@ class StreamingSessions:
             raise ValueError(f"session {sid} has no source embedding before its first enrollment snapshot")
         return s.tracks[k] if s.tracks[k] is not None else ToneTrack([(0, s.se[k].clone())])
 
-    def _window_tracks(self, ses, wins, b0: int, b1: int, Tmax: int, g, fresh=frozenset()):
+    def _window_tracks(self, ses, wins, b0: int, b1: int, Tmax: int, g, fresh=frozenset(), sides=(0, 1)):
         """Per side, the [b1 - b0, gin, Tmax] per-frame embeddings of launch windows b0 .. b1 - 1 when one of them
         overlaps a transition of that side (a track whose last key lies past the window's first frame), else the
         gathered per-item rows g[side] (the launch is then exactly the per-item one).  ``fresh``: sessions whose source
         is the first enrollment snapshot of this step, which only the device table holds: their constant windows take
-        the gathered row g[0] at each of their frames."""
+        the gathered row g[0] at each of their frames.  ``sides``: the sides to return (default both)."""
         out = []
-        for k in range(2):
+        for k in sides:
             var = [ses[i][1].tracks[k] is not None and lo < ses[i][1].tracks[k].frames[-1]
                    for i, lo, _, _, _ in wins[b0:b1]]
             if not any(var):
@@ -853,15 +854,18 @@ class StreamingSessions:
         if self.est is not None and self.est.shape[0] < rows:
             self._grow_est()
 
-    def _splice(self, source: torch.Tensor, seg: torch.Tensor, segs: List[Tuple[int, int, int, int, int]],
-                dst: torch.Tensor):
-        """``ovc_splice`` of ``segs`` (on the device as ``seg``) from ``source`` into the ring array ``dst``."""
+    def _splice(self, source: torch.Tensor, seg: torch.Tensor, segs: Optional[List[Tuple[int, int, int, int, int]]],
+                dst: torch.Tensor, src_wrap: bool = False):
+        """``ovc_splice`` of ``segs`` (on the device as ``seg``; None: only there) from ``source`` into the ring array
+        ``dst``; ``src_wrap``: the source rows are rings too (``SPLICE_SRC_WRAP``)."""
         if self.cuda:
-            self.native.splice(source, seg, dst)
+            self.native.splice(source, seg, dst, src_wrap=src_wrap)
         else:   # only the CPU stand-in converters of the host tests get here: the same writes as one index_copy_
-            cap = dst.shape[1]
+            segs = seg.tolist() if segs is None else segs
+            cap, pitch = dst.shape[1], source.shape[1]
             at = np.concatenate([r * cap + np.arange(a, a + n) % cap for _, _, n, r, a in segs])
-            val = torch.cat([source[row, off:off + n] if row >= 0 else torch.zeros(n) for row, off, n, _, _ in segs])
+            val = torch.cat([torch.zeros(n) if row < 0 else source[row, (off + torch.arange(n)) % pitch] if src_wrap
+                             else source[row, off:off + n] for row, off, n, _, _ in segs])
             dst.view(-1).index_copy_(0, torch.from_numpy(at), val)
 
     # ------------------------------------------------------------------ one step
@@ -869,7 +873,7 @@ class StreamingSessions:
         """One step over the sessions of ``xs``: xs[sid] is the session's new host samples, or with ``src`` its runs
         (src_row, src_off, count) of that device array, at the session's input rate; the sessions in ``final`` end after
         them."""
-        hop, H, sr = self.hop, self.H, self.sr
+        hop, sr = self.hop, self.sr
         ses = [(sid, self.sessions[sid], xs[sid]) for sid in xs]
         if src is None:                                   # host samples: the upload's sample block is the one source row
             counts = [len(x) for _, _, x in ses]
@@ -906,13 +910,8 @@ class StreamingSessions:
         first = [b for b, (i, k) in enumerate(enr) if k and not ses[i][1].has_src]
         no_src = {i for i, k in enr if not k and not ses[i][1].has_src}
         nE, nF, gin = len(enr), len(first), self.gin
-        # windows of every named session: (session index, lo, hi, e0, e1)
-        wins = []
-        for i, ((sid, s, _), n) in enumerate(zip(ses, gains)):
-            if i in no_src:                               # nothing to convert with yet
-                continue
-            have = ready_frames(s.n_in + n, hop, self.nfft, sid in final)
-            wins += [(i,) + w for w in stream_windows(s.emitted, have, self.W, H, sid in final)]
+        # the windows whose frames the step emits, (session index, lo, hi, e0, e1), and how they are converted
+        wins, plan = self._plan(ses, gains, final, no_src)
         # splice segments: each run to the ring row (raw ring row when the session resamples its input) of its session,
         # at the session's next sample positions
         segs, rsegs = [], []
@@ -923,7 +922,6 @@ class StreamingSessions:
                     dst.append((row, off, n, s.row, at))
                     at += n
         B, nS, nR, Ns = len(wins), len(segs), len(rsegs), (sum(counts) if src is None else 0)
-        Tmax = -(-max([hi - lo for _, lo, hi, _, _ in wins], default=1) // 16) * 16
         Nf = sum(e1 - e0 for _, _, _, e0, e1 in wins)
         # output side: the emitted frames of output-resampling sessions go to their output ring rows (osegs: splice
         # from the gathered frames) and their new output-rate samples are packed after the frames (rout, qn)
@@ -950,13 +948,11 @@ class StreamingSessions:
                 live = [(s.row, self._out_keep(s), s.emitted * hop) for s in self.sessions.values() if s.out_sr]
                 self.orings = self._moved(self.orings, self.rows, -(-int(need * 1.25) // 1024) * 1024, live)
         nO, nI, nQ = len(osegs), len(rin), len(rout)
-        # packed upload (int64 words): row, lo, frames, stream length, seed, stream (0), embedding rows (2B), tau (float32),
-        # then the emitted frames' rows of the output, the splice segments (5 words each), the raw splice segments, the
-        # input resampling items (6 words each, then their plans as int32), the output splice segments, the output
-        # resampling items, the encoder descriptors (4 words each) with the first snapshots' items and embedding table
-        # rows, and the pushed samples (float32)
-        nt = (B + 1) // 2
-        o = 8 * B + nt + Nf
+        # packed upload (int64 words): the conversion's tables (``_pack``), the splice segments (5 words each), the raw
+        # splice segments, the input resampling items (6 words each, then their plans as int32), the output splice
+        # segments, the output resampling items, the encoder descriptors (4 words each) with the first snapshots' items
+        # and embedding table rows, and the pushed samples (float32)
+        o = self._plan_words(plan)
         o_r = o + 5 * nS
         o_i = o_r + 5 * nR
         o_o = o_i + 6 * nI + (nI + 1) // 2
@@ -968,19 +964,7 @@ class StreamingSessions:
             self._h2d_done.synchronize()                  # the previous step's upload has left the pinned buffer
         pin = self._buf("pin", n_words, torch.int64, pinned=True)
         w = pin.numpy()
-        if B:
-            ii = np.asarray([i for i, _, _, _, _ in wins])
-            rows = np.asarray([s.row for _, s, _ in ses], dtype=np.int64)[ii]
-            lo = np.asarray([v[1] for v in wins], dtype=np.int64)
-            w[0:B], w[B:2 * B], w[2 * B:3 * B] = rows, lo, [hi - l for _, l, hi, _, _ in wins]
-            w[3 * B:4 * B] = [ses[i][1].n_in + gains[i] if ses[i][0] in final else STREAM_OPEN for i in ii]
-            from .api import seed_array
-            w[4 * B:5 * B] = seed_array([ses[i][1].seed for i in ii])
-            w[5 * B:6 * B] = 0
-            w[6 * B:7 * B], w[7 * B:8 * B] = rows, rows + self.rows
-            w[8 * B:8 * B + nt].view(np.float32)[:B] = [ses[i][1].tau for i in ii]
-            w[8 * B + nt:o] = np.concatenate([b * Tmax + np.arange(e0 - l, e1 - l)
-                                              for b, (_, l, _, e0, e1) in enumerate(wins)])
+        self._pack(w, plan, ses, gains, final)
         for at, sg in ((o, segs), (o_r, rsegs), (o_o, osegs)):
             if sg:
                 w[at:at + 5 * len(sg)] = np.asarray(sg, dtype=np.int64).reshape(-1)
@@ -1020,24 +1004,8 @@ class StreamingSessions:
             self.native.reference_encoder_stream(self.rings, self.est, d[o_e:o_e + 4 * nE].view(nE, 4), M, out=eout)
             if nF:                                        # first snapshots are the sources of this step's windows
                 self.se[0].index_copy_(0, d[o_e + 4 * nE + nF:o_s], eout.index_select(0, d[o_e + 4 * nE:o_e + 4 * nE + nF]))
+        y = self._convert(d, plan, ses, {enr[b][0] for b in first}, ybuf[:Nf * hop].view(Nf, hop))
         if B:
-            spec = self._buf("spec", B * self.S * Tmax, torch.float32).view(B, self.S, Tmax)
-            self.native.spectrogram_ring(self.rings, d[0:B], d[B:2 * B], d[2 * B:3 * B], d[3 * B:4 * B], Tmax, out=spec)
-            g = torch.index_select(self.se.view(-1, self.gin), 0, d[6 * B:8 * B],
-                                   out=self._buf("g", 2 * B * self.gin, torch.float32).view(2 * B, self.gin))
-            obuf = self._buf("o", B * Tmax * hop, torch.float32)
-            per = max(1, SESSION_BATCH_FRAMES // Tmax)
-            taus = d[8 * B:8 * B + nt].view(torch.float32)[:B]
-            for b0 in range(0, B, per):
-                b1 = min(B, b0 + per)
-                items = {"seed": d[4 * B + b0:4 * B + b1], "stream": d[5 * B + b0:5 * B + b1],
-                         "frame0": d[B + b0:B + b1], "tau": taus[b0:b1]}
-                gs, gt = self._window_tracks(ses, wins, b0, b1, Tmax, (g[:B], g[B:]), {enr[b][0] for b in first})
-                self.native.voice_conversion(spec[b0:b1], d[2 * B + b0:2 * B + b1], gs, gt,
-                                             ragged=True, latents=False, items=items,
-                                             out=obuf[b0 * Tmax * hop:b1 * Tmax * hop])
-            fo = 8 * B + nt
-            y = torch.index_select(obuf.view(B * Tmax, hop), 0, d[fo:fo + Nf], out=ybuf[:Nf * hop].view(Nf, hop))
             if nO:
                 self._splice(y.view(1, Nf * hop), d[o_o:o_o + 5 * nO].view(nO, 5), osegs, self.orings)
             if nQ:
@@ -1074,11 +1042,244 @@ class StreamingSessions:
                 s.se[0], s.has_src = se, True
         return res
 
+    # ------------------------------------------------------------------ the conversion part of a step
+    def _plan(self, ses, gains: List[int], final: Set[int], skip: Set[int]):
+        """(windows, plan) of a step whose sessions ``ses`` gain ``gains`` model-rate samples: the windows (session
+        index, lo, hi, e0, e1) whose frames [e0, e1) the step emits, and what ``_pack`` and ``_convert`` take -- here the
+        same windows, each converted whole with both halos.  Sessions in ``skip`` have nothing to convert with yet."""
+        wins = []
+        for i, ((sid, s, _), n) in enumerate(zip(ses, gains)):
+            if i in skip:
+                continue
+            have = ready_frames(s.n_in + n, self.hop, self.nfft, sid in final)
+            wins += [(i,) + w for w in stream_windows(s.emitted, have, self.W, self.H, sid in final)]
+        return wins, wins
+
+    @staticmethod
+    def _tmax(wins) -> int:
+        """Padded window length of a launch: the longest window rounded up to 16 frames (steady steps repeat it)."""
+        return -(-max([hi - lo for _, lo, hi, _, _ in wins], default=1) // 16) * 16
+
+    def _plan_words(self, wins) -> int:
+        B = len(wins)
+        return 8 * B + (B + 1) // 2 + sum(e1 - e0 for _, _, _, e0, e1 in wins)
+
+    def _pack(self, w: np.ndarray, wins, ses, gains: List[int], final: Set[int]) -> None:
+        """The conversion's tables at the front of the step's upload ``w``: row, lo, frames, stream length, seed,
+        stream (0), embedding rows (2B), tau (float32), then the emitted frames' rows of the output."""
+        B = len(wins)
+        if not B:
+            return
+        nt, Tmax = (B + 1) // 2, self._tmax(wins)
+        ii = np.asarray([i for i, _, _, _, _ in wins])
+        rows = np.asarray([s.row for _, s, _ in ses], dtype=np.int64)[ii]
+        lo = np.asarray([v[1] for v in wins], dtype=np.int64)
+        w[0:B], w[B:2 * B], w[2 * B:3 * B] = rows, lo, [hi - l for _, l, hi, _, _ in wins]
+        w[3 * B:4 * B] = [ses[i][1].n_in + gains[i] if ses[i][0] in final else STREAM_OPEN for i in ii]
+        from .api import seed_array
+        w[4 * B:5 * B] = seed_array([ses[i][1].seed for i in ii])
+        w[5 * B:6 * B] = 0
+        w[6 * B:7 * B], w[7 * B:8 * B] = rows, rows + self.rows
+        w[8 * B:8 * B + nt].view(np.float32)[:B] = [ses[i][1].tau for i in ii]
+        w[8 * B + nt:self._plan_words(wins)] = np.concatenate([b * Tmax + np.arange(e0 - l, e1 - l)
+                                                                for b, (_, l, _, e0, e1) in enumerate(wins)])
+
+    def _convert(self, d: torch.Tensor, wins, ses, fresh: Set[int], y: torch.Tensor) -> Optional[torch.Tensor]:
+        """Spectrogram -> voice conversion -> emitted frames of the step's windows, from the tables ``_pack`` put at the
+        front of the uploaded ``d``: the emitted frames go into ``y`` [Nf, hop], which is returned (None without
+        windows).  ``fresh``: sessions whose source is the first enrollment snapshot of this step."""
+        B = len(wins)
+        if not B:
+            return None
+        hop, nt, Tmax, Nf = self.hop, (B + 1) // 2, self._tmax(wins), y.shape[0]
+        spec = self._buf("spec", B * self.S * Tmax, torch.float32).view(B, self.S, Tmax)
+        self.native.spectrogram_ring(self.rings, d[0:B], d[B:2 * B], d[2 * B:3 * B], d[3 * B:4 * B], Tmax, out=spec)
+        g = torch.index_select(self.se.view(-1, self.gin), 0, d[6 * B:8 * B],
+                               out=self._buf("g", 2 * B * self.gin, torch.float32).view(2 * B, self.gin))
+        obuf = self._buf("o", B * Tmax * hop, torch.float32)
+        per = max(1, SESSION_BATCH_FRAMES // Tmax)
+        taus = d[8 * B:8 * B + nt].view(torch.float32)[:B]
+        for b0 in range(0, B, per):
+            b1 = min(B, b0 + per)
+            items = {"seed": d[4 * B + b0:4 * B + b1], "stream": d[5 * B + b0:5 * B + b1],
+                     "frame0": d[B + b0:B + b1], "tau": taus[b0:b1]}
+            gs, gt = self._window_tracks(ses, wins, b0, b1, Tmax, (g[:B], g[B:]), fresh)
+            self.native.voice_conversion(spec[b0:b1], d[2 * B + b0:2 * B + b1], gs, gt,
+                                         ragged=True, latents=False, items=items,
+                                         out=obuf[b0 * Tmax * hop:b1 * Tmax * hop])
+        fo = 8 * B + nt
+        return torch.index_select(obuf.view(B * Tmax, hop), 0, d[fo:fo + Nf], out=y)
+
     def _resample_rings(self, d: torch.Tensor, at: int, n: int, src: torch.Tensor, dst: torch.Tensor, max_count: int):
         """One ``ovc_resample_rings`` over the n items packed at word ``at`` of the step's upload ``d``."""
         v = [d[at + k * n:at + (k + 1) * n] for k in range(6)]
         plan = d[at + 6 * n:at + 6 * n + (n + 1) // 2].view(torch.int32)[:n]
         self.native.resample_rings(plan, src, v[0], v[1], v[2], v[3], dst, v[4], v[5], max_count)
+
+
+# Halo of each stage of StagedSessions (frames on each side whose context a frame's value depends on).  The latent stack
+# (posterior encoder, flow forward, flow reverse) sees +-96: the encoder's WN has 16 layers of kernel 5 at dilation 1
+# (16 x 2 = 32), and each flow direction 4 couplings of 4 such layers (4 x 4 x 2 = 32); its other convs are 1x1.  The
+# generator sees +-14: conv_pre (k 7: 3 frames), then per upsampling stage the ResBlock dilations (k 3/7/11 at 1, 3, 5)
+# and the transposed conv, expressed in frames of the stage's input -- the figure the TTS window decode relies on.
+LATENT_HALO_FRAMES = 96
+GEN_HALO_FRAMES = 14
+
+
+class StagedSessions(StreamingSessions):
+    """``StreamingSessions`` converting in two stages, so the generator -- about 93 % of the converter's work -- no
+    longer recomputes the whole converter's 2 x 128 halo frames.  Each session keeps its final latents (z_hat, the flow
+    reverse's output) in a device ring of ``[inter_channels, cap]`` rows:
+
+    * stage A (latent): windows of U = min(window_frames, 16) frames with ``LATENT_HALO_FRAMES`` (96) on each side
+      (``stream_windows`` over the ready spectrogram frames); one ``ovc_spectrogram_ring`` over all of them, ragged
+      latent-half calls (``NativeConverter.latent``) of up to ``SESSION_BATCH_FRAMES`` padded frames each, and one
+      ``ovc_splice`` of their interiors into the latent rings;
+    * stage B (generator): windows of ``window_frames`` frames with ``GEN_HALO_FRAMES`` (14) on each side over the final
+      latent frames; one source-wrapping ``ovc_splice`` gathers them from the rings into a padded batch, ragged generator
+      calls (``NativeConverter.generate``) convert it, and the emitted frames go out as in ``StreamingSessions``.
+
+    Stage A runs before stage B in the same step, so a push that completes both emits in that step.  A window's geometry
+    depends on absolute frames only and every item is converted at its own length, so a session's audio depends on its
+    own stream alone -- not on its chunking nor on the sessions beside it -- and is within the streaming bound of
+    ``convert`` on the whole clip (the tile geometry differs from ``StreamingConverter``'s, so it is not bit-identical to
+    it).  The largest look-ahead, at the first frame of a stage-B window starting at e0, is U * ceil((e0 + W + 14) / U) +
+    96 - e0 frames: W + 112 for every W that U divides (all W <= 16 and every multiple of 16), against W + 128 for
+    ``StreamingSessions``.
+
+    Everything else -- ``open`` (rates, enrollment), ``push``, ``push_device``, ``close``, ``discard``, ``retarget``,
+    ``tone_track``, ``source_se``, ``state_samples`` -- is ``StreamingSessions``'.  The audio ring keeps the next stage-A
+    window and the STFT support (plus the largest push), the latent ring the next stage-B window and the stage-A unit
+    ahead of it; both are grow-only."""
+
+    def __init__(self, converter, window_frames: int = 256, rates: Iterable[int] = ()):
+        super().__init__(converter, window_frames, rates)
+        self.U = min(self.W, 16)
+        self.C = int(converter.hps.model.inter_channels)
+        self.cap = self.hop * (self.U + 2 * LATENT_HALO_FRAMES + 8) + 4096
+        self.rings = torch.zeros(0, self.cap, device=self.dev)
+        self.lcap = self.U + self.W + 2 * GEN_HALO_FRAMES + 16          # latent frames per ring row; grows
+        self.lrings = torch.zeros(0, self.lcap, device=self.dev)        # [rows * C, lcap]: session row r at r*C + c
+        # channel c's splice segment of a latent window: the window's channel-0 segment plus (c, 0, 0, c, 0)
+        coff = torch.zeros(1, self.C, 5, dtype=torch.int64)
+        coff[0, :, 0] = coff[0, :, 3] = torch.arange(self.C)
+        self._coff = coff.to(self.dev)
+
+    def _keep_from(self, s: _Session) -> int:
+        """First sample of the session's next stage-A window."""
+        return max(0, (s.lat - LATENT_HALO_FRAMES) * self.hop - self.pad)
+
+    def _grow(self, rows: int, cap: int, live: List[Tuple[int, int, int]]):
+        if rows != self.rows:
+            self.lrings = self._moved(self.lrings, rows * self.C, self.lcap, [])
+        super()._grow(rows, cap, live)
+
+    def _plan(self, ses, gains: List[int], final: Set[int], skip: Set[int]):
+        """Stage-A windows over the ready spectrogram frames, then stage-B windows over the latent frames stage A leaves
+        final (ended: all of them once the session is closed).  Grows the latent rings when a session's step would write
+        past what it still reads: from its next stage-B window's left halo to its new latent end."""
+        winsA, winsB, lat = [], [], {}
+        for i, ((sid, s, _), n) in enumerate(zip(ses, gains)):
+            if i in skip:
+                continue
+            end = sid in final
+            have = ready_frames(s.n_in + n, self.hop, self.nfft, end)
+            wa = stream_windows(s.lat, have, self.U, LATENT_HALO_FRAMES, end)
+            lat[i] = wa[-1][3] if wa else s.lat
+            winsA += [(i,) + w for w in wa]
+            winsB += [(i,) + w for w in stream_windows(s.emitted, lat[i], self.W, GEN_HALO_FRAMES, end and lat[i] == have)]
+        need = max([v - max(0, ses[i][1].emitted - GEN_HALO_FRAMES) for i, v in lat.items()], default=0)
+        if need > self.lcap:
+            cap = -(-int(need * 1.25) // 16) * 16
+            live = [(s.row * self.C + c, max(0, s.emitted - GEN_HALO_FRAMES), s.lat)
+                    for s in self.sessions.values() if s.lat > max(0, s.emitted - GEN_HALO_FRAMES) for c in range(self.C)]
+            self.lrings = (self._moved(self.lrings, self.rows * self.C, cap, live) if live
+                           else torch.zeros(self.rows * self.C, cap, device=self.dev))
+            self.lcap = cap
+        return winsB, (winsA, winsB, lat)
+
+    def _plan_words(self, plan) -> int:
+        winsA, winsB, _ = plan
+        BA, BB = len(winsA), len(winsB)
+        return 13 * BA + (BA + 1) // 2 + 7 * BB + sum(e1 - e0 for _, _, _, e0, e1 in winsB)
+
+    def _pack(self, w: np.ndarray, plan, ses, gains: List[int], final: Set[int]) -> None:
+        """Stage A: row, lo, frames, stream length, seed, stream (0), embedding rows (2 BA), tau (float32), the channel-0
+        scatter segments of the interiors (5 words each).  Stage B: the channel-0 gather segments (5 words each), frames,
+        target embedding rows, the emitted frames' rows of the output."""
+        from .api import seed_array
+        winsA, winsB, _ = plan
+        BA, BB, C = len(winsA), len(winsB), self.C
+        if BA:
+            ii = [i for i, _, _, _, _ in winsA]
+            rows = np.asarray([ses[i][1].row for i in ii], dtype=np.int64)
+            w[0:BA], w[BA:2 * BA] = rows, [lo for _, lo, _, _, _ in winsA]
+            w[2 * BA:3 * BA] = [hi - lo for _, lo, hi, _, _ in winsA]
+            w[3 * BA:4 * BA] = [ses[i][1].n_in + gains[i] if ses[i][0] in final else STREAM_OPEN for i in ii]
+            w[4 * BA:5 * BA] = seed_array([ses[i][1].seed for i in ii])
+            w[5 * BA:6 * BA] = 0
+            w[6 * BA:7 * BA], w[7 * BA:8 * BA] = rows, rows + self.rows
+            w[8 * BA:8 * BA + (BA + 1) // 2].view(np.float32)[:BA] = [ses[i][1].tau for i in ii]
+            o = 8 * BA + (BA + 1) // 2
+            w[o:o + 5 * BA] = np.asarray([(a * C, e0 - lo, e1 - e0, ses[i][1].row * C, e0)
+                                          for a, (i, lo, _, e0, e1) in enumerate(winsA)], dtype=np.int64).reshape(-1)
+        if BB:
+            o, Tmax = 13 * BA + (BA + 1) // 2, self._tmax(winsB)
+            rows = np.asarray([ses[i][1].row for i, _, _, _, _ in winsB], dtype=np.int64)
+            w[o:o + 5 * BB] = np.asarray([(r * C, lo, hi - lo, b * C, 0) for b, (r, (_, lo, hi, _, _))
+                                          in enumerate(zip(rows, winsB))], dtype=np.int64).reshape(-1)
+            w[o + 5 * BB:o + 6 * BB] = [hi - lo for _, lo, hi, _, _ in winsB]
+            w[o + 6 * BB:o + 7 * BB] = rows + self.rows
+            w[o + 7 * BB:self._plan_words(plan)] = np.concatenate([b * Tmax + np.arange(e0 - lo, e1 - lo)
+                                                                    for b, (_, lo, _, e0, e1) in enumerate(winsB)])
+
+    def _segs(self, base: torch.Tensor, n: int, name: str) -> torch.Tensor:
+        """The [n * C, 5] per-channel splice segments of n latent windows from their channel-0 segments ``base``."""
+        out = self._buf(name, n * self.C * 5, torch.int64).view(n, self.C, 5)
+        torch.add(base.view(n, 1, 5), self._coff, out=out)
+        return out.view(n * self.C, 5)
+
+    def _convert(self, d: torch.Tensor, plan, ses, fresh: Set[int], y: torch.Tensor) -> Optional[torch.Tensor]:
+        """Stage A, then stage B, from the tables ``_pack`` put at the front of ``d``; advances each session's latent
+        end.  Returns ``y`` [Nf, hop] holding the emitted frames, or None when stage B has no window."""
+        winsA, winsB, lat = plan
+        BA, BB, C, hop, gin = len(winsA), len(winsB), self.C, self.hop, self.gin
+        if BA:
+            nt, Tmax = (BA + 1) // 2, self._tmax(winsA)
+            spec = self._buf("spec", BA * self.S * Tmax, torch.float32).view(BA, self.S, Tmax)
+            self.native.spectrogram_ring(self.rings, d[0:BA], d[BA:2 * BA], d[2 * BA:3 * BA], d[3 * BA:4 * BA], Tmax,
+                                         out=spec)
+            g = torch.index_select(self.se.view(-1, gin), 0, d[6 * BA:8 * BA],
+                                   out=self._buf("g", 2 * BA * gin, torch.float32).view(2 * BA, gin))
+            z = self._buf("za", BA * C * Tmax, torch.float32).view(BA, C, Tmax)
+            per = max(1, SESSION_BATCH_FRAMES // Tmax)
+            taus = d[8 * BA:8 * BA + nt].view(torch.float32)[:BA]
+            for b0 in range(0, BA, per):
+                b1 = min(BA, b0 + per)
+                items = {"seed": d[4 * BA + b0:4 * BA + b1], "stream": d[5 * BA + b0:5 * BA + b1],
+                         "frame0": d[BA + b0:BA + b1], "tau": taus[b0:b1]}
+                gs, gt = self._window_tracks(ses, winsA, b0, b1, Tmax, (g[:BA], g[BA:]), fresh)
+                self.native.latent(spec[b0:b1], d[2 * BA + b0:2 * BA + b1], gs, gt, items=items, out=z[b0:b1])
+            o = 8 * BA + nt
+            self._splice(z.view(BA * C, Tmax), self._segs(d[o:o + 5 * BA], BA, "sega"), None, self.lrings)
+        for i, v in lat.items():
+            ses[i][1].lat = v
+        if not BB:
+            return None
+        o, Tmax, Nf = 13 * BA + (BA + 1) // 2, self._tmax(winsB), y.shape[0]
+        z = self._buf("zb", BB * C * Tmax, torch.float32).view(BB, C, Tmax)
+        self._splice(self.lrings, self._segs(d[o:o + 5 * BB], BB, "segb"), None, z.view(BB * C, Tmax), src_wrap=True)
+        g = torch.index_select(self.se.view(-1, gin), 0, d[o + 6 * BB:o + 7 * BB],
+                               out=self._buf("gb", BB * gin, torch.float32).view(BB, gin))
+        obuf = self._buf("o", BB * Tmax * hop, torch.float32)
+        per = max(1, SESSION_BATCH_FRAMES // Tmax)
+        for b0 in range(0, BB, per):
+            b1 = min(BB, b0 + per)
+            gt = self._window_tracks(ses, winsB, b0, b1, Tmax, (None, g), fresh, sides=(1,))[0]
+            self.native.generate(z[b0:b1], d[o + 5 * BB + b0:o + 5 * BB + b1], gt,
+                                 out=obuf[b0 * Tmax * hop:b1 * Tmax * hop])
+        fo = o + 7 * BB
+        return torch.index_select(obuf.view(BB * Tmax, hop), 0, d[fo:fo + Nf], out=y)
 
 
 class _CloneSession:
