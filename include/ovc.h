@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define OVC_ABI_VERSION 17 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
+#define OVC_ABI_VERSION 18 /* 2: ovc_graph_replays, OVC_OPT_PDL .. OVC_OPT_PAIR; 3: option keys 1, 4 and 6 (kernel variant,
                                * activation TMA, tune bits) removed; 4: ovc_reference_encoder_ragged;
                                * 5: ovc_resample, ovc_resample_span; 6: ovc_item_params, the *_items entry points,
                                * ovc_philox_normals; 7: ovc_tts_encode_state, ovc_tts_decode_windows;
@@ -37,7 +37,8 @@ extern "C" {
                                *     ovc_tts_encode_state_rows_tokens, ovc_tts_state_rows_tokens;
                                * 16: ovc_reference_encoder_stream, ovc_reference_encoder_stream_state_floats;
                                * 17: ovc_generate_frames, o_hat NULL on ovc_voice_conversion_frames (the latent half),
-                               *     OVC_SPLICE_SRC_WRAP */
+                               *     OVC_SPLICE_SRC_WRAP;
+                               * 18: ovc_tts_fit, ovc_tts_encode_fit */
 
 #if defined(__GNUC__)
 #define OVC_API __attribute__((visibility("default")))
@@ -422,6 +423,30 @@ OVC_API int ovc_tts_encode_items(ovc_ctx* ctx, const int64_t* tokens, const int6
 OVC_API int ovc_tts_decode_items(ovc_ctx* ctx, const float* noise, uint64_t seed, float noise_scale, int B, int Ymax,
                                  int max_len, int ragged, float* o, float* z, float* z_p, void* stream,
                                  const ovc_item_params* items);
+
+/* Duration fit: the encode with each fit group's length scale solved on the device, so that a run of rows (the
+ * sentences of one request, say) lasts a given number of frames.  Group g is rows [row0[g], row1[g]) with a target of
+ * target_frames[g] = F* frames.  Its frames at scale s are F(s) = sum over its rows of max(1, sum_t ceilf(expf(logw[t]) * s)),
+ * the y_lengths the encode gives at length_scale = s, and its scale s* is the smallest float s in [scale_lo, scale_hi] with
+ * F(s) >= F*, or scale_hi if there is none.  Every row of the group is then encoded at length_scale = s*, bit for bit as an
+ * encode given s* as that row's per-item length_scale.  Rows outside every group keep the call's (or their per-item)
+ * length_scale.  length_scale [B] receives every row's scale.  Device arrays are clamped on the device: row ranges into
+ * [0, B), each to start at or after the previous group's end (groups never share a row), targets to at least 1.
+ * The call only enqueues work. */
+typedef struct ovc_tts_fit {
+  const int64_t* row0;            /* [G], device: the group's first row */
+  const int64_t* row1;            /* [G], device: one past its last row */
+  const int64_t* target_frames;   /* [G], device */
+  int G;                          /* 1 <= G <= B */
+  float scale_lo, scale_hi;       /* 0 < scale_lo <= scale_hi, finite */
+  float* length_scale;            /* [B], device out */
+} ovc_tts_fit;
+/* ovc_tts_encode_items / ovc_tts_encode_g with fit groups (`fit` a host pointer); exactly one of sid and g is given
+ * (g_tokens as in ovc_tts_encode_g).  The ovc_tts_encode_state* calls and ovc_tts_decode work after it unchanged. */
+OVC_API int ovc_tts_encode_fit(ovc_ctx* ctx, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid,
+                               const float* g, int g_tokens, const float* noise_w, uint64_t seed, float noise_scale_w,
+                               float length_scale, float sdp_ratio, int B, int T, int64_t* y_lengths, float* w_ceil,
+                               float* logw, void* stream, const ovc_item_params* items, const ovc_tts_fit* fit);
 
 /* Streaming decode: the decode half in time windows, from encode state the caller owns.
  *

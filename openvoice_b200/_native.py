@@ -13,7 +13,7 @@ from typing import Dict, Iterable, Optional, Tuple
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libovc_b200.so")
 
-ABI_VERSION = 17
+ABI_VERSION = 18
 EXPORTS = (
     "ovc_abi_version", "ovc_last_error", "ovc_create", "ovc_destroy", "ovc_load_tensor",
     "ovc_finalize_weights", "ovc_workspace_floats", "ovc_voice_conversion", "ovc_last_launch_count",
@@ -27,7 +27,7 @@ EXPORTS = (
     "ovc_voice_conversion_frames", "ovc_convert_waveform_frames", "ovc_tone_track_expand",
     "ovc_tts_encode_g", "ovc_tts_encode_state_tokens", "ovc_tts_decode_windows_tokens", "ovc_tts_encode_state_rows_tokens",
     "ovc_tts_state_rows_tokens", "ovc_reference_encoder_stream", "ovc_reference_encoder_stream_state_floats",
-    "ovc_generate_frames",
+    "ovc_generate_frames", "ovc_tts_encode_fit",
 )
 
 STREAM_OPEN = 2 ** 63 - 1   # ovc_resample / ovc_spectrogram_ring length of a stream that has not ended
@@ -68,6 +68,14 @@ class ItemParams(C.Structure):
         ("seed", C.c_void_p), ("stream", C.c_void_p), ("frame0", C.c_void_p), ("tau", C.c_void_p),
         ("noise_scale", C.c_void_p), ("noise_scale_w", C.c_void_p), ("length_scale", C.c_void_p),
         ("sdp_ratio", C.c_void_p),
+    ]
+
+
+class TtsFit(C.Structure):
+    """struct ovc_tts_fit of include/ovc.h: fit groups of ovc_tts_encode_fit (device arrays)."""
+    _fields_ = [
+        ("row0", C.c_void_p), ("row1", C.c_void_p), ("target_frames", C.c_void_p), ("G", C.c_int),
+        ("scale_lo", C.c_float), ("scale_hi", C.c_float), ("length_scale", C.c_void_p),
     ]
 
 
@@ -197,6 +205,8 @@ def load_library(path: Optional[str] = None):
     lib.ovc_reference_encoder_stream.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p,
                                                  C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     lib.ovc_generate_frames.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+    lib.ovc_tts_encode_fit.argtypes = (lib.ovc_tts_encode.argtypes[:4] + [C.c_void_p, C.c_int]
+                                       + lib.ovc_tts_encode.argtypes[4:] + [P, C.POINTER(TtsFit)])
     if lib.ovc_abi_version() != ABI_VERSION:
         raise OvcError(f"ABI mismatch: library {lib.ovc_abi_version()} vs binding {ABI_VERSION}")
     _lib = lib
@@ -686,12 +696,14 @@ class NativeConverter:
 
     def tts_encode(self, tokens, x_lengths, sid, noise_w=None, seed: int = 0, noise_scale_w: float = 1.0,
                    length_scale: float = 1.0, sdp_ratio: float = 0.2, stream=None, items: Optional[dict] = None,
-                   g=None):
+                   g=None, fit=None):
         """tokens [B,T] i64 cuda, x_lengths [B] i64 cuda, sid [B] i64 cuda, noise_w [B,2,T] or None (Philox).
         Returns (y_lengths [B] i64, w_ceil [B,T], logw [B,T]), all on the device; asynchronous on `stream`.
         ``items``: per-item ``{"seed", "stream", "noise_scale_w", "length_scale", "sdp_ratio"}`` (``item_params``).
         ``g``: speaker vectors instead of ``sid`` (which is then ignored), f32 cuda [B, gin] or per token [B, gin, T]
-        (include/ovc.h: ovc_tts_encode_g)."""
+        (include/ovc.h: ovc_tts_encode_g).
+        ``fit``: ``(row0, row1, target_frames, scale_lo, scale_hi)``, the first three [G] i64 cuda tensors (include/ovc.h:
+        ovc_tts_encode_fit); the return then ends with each row's length scale, [B] f32 on the device."""
         import torch
         for t in (tokens, x_lengths) + ((sid,) if g is None else ()):
             assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()
@@ -711,6 +723,16 @@ class NativeConverter:
         it = item_params(items, B)
         rest = (p(noise_w), C.c_uint64(seed & (2 ** 64 - 1)), C.c_float(noise_scale_w), C.c_float(length_scale),
                 C.c_float(sdp_ratio), B, T, p(y_lengths), p(w_ceil), p(logw), C.c_void_p(st.cuda_stream), _items_ref(it))
+        if fit is not None:
+            row0, row1, target, lo, hi = fit
+            for t in (row0, row1, target):
+                assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous() and t.shape == row0.shape
+            scale = torch.empty(B, device=tokens.device, dtype=torch.float32)
+            f = TtsFit(p(row0), p(row1), p(target), int(row0.numel()), lo, hi, p(scale))
+            rc = self.lib.ovc_tts_encode_fit(self.handle, p(tokens), p(x_lengths), p(sid) if g is None else None, p(g),
+                                             1 if g is not None and g.dim() == 3 else 0, *rest, C.byref(f))
+            _check(self.lib, rc, "ovc_tts_encode_fit")
+            return y_lengths, w_ceil, logw, scale
         if g is None:
             rc = self.lib.ovc_tts_encode_items(self.handle, p(tokens), p(x_lengths), p(sid), *rest)
         else:

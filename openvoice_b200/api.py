@@ -245,6 +245,9 @@ def plan_se_chunks(frames: Sequence[int], budget: int = SE_CHUNK_FRAMES) -> List
 # forward flow here, so this is about half of HALO_FRAMES.
 TTS_HALO_FRAMES = 64
 
+# Range of the length scale a duration fit may choose (include/ovc.h: ovc_tts_fit): speed 4x down to 0.25x.
+FIT_SCALE_RANGE = (0.25, 4.0)
+
 
 def plan_tts_windows(frames: int, first_window: int, window: int, halo: int) -> List[Tuple[int, int, int, int]]:
     """Windows of one sentence of ``frames`` decoded frames: (lo, hi, e0, e1) with decoded span [lo, hi) and interior
@@ -301,6 +304,29 @@ class TtsState(NamedTuple):
     dec_keys: List[int]
     dec_streams: List[int]
     dec_noise_scale: List[float]
+    length_scale: Optional[List[float]] = None     # each row's length scale, after an encode with fit groups
+
+
+def fit_groups(fit, B: int, device) -> Optional[tuple]:
+    """The ``fit`` argument of ``NativeSynthesizer.tts_encode`` / ``infer_ragged`` as ``_native`` takes it: groups
+    ``[(row0, row1, target_frames), ...]`` of rows [row0, row1) in increasing order that do not overlap, each with a
+    target of at least 1 frame.  None or [] -> None (an encode without fit groups).  ValueError for anything else."""
+    if not fit:
+        return None
+    fit = [tuple(int(v) for v in f) for f in fit]
+    end = 0
+    for i, f in enumerate(fit):
+        if len(f) != 3:
+            raise ValueError(f"fit group {i}: expected (row0, row1, target_frames), got {f}")
+        r0, r1, target = f
+        if not end <= r0 < r1 <= B:
+            raise ValueError(f"fit group {i}: rows [{r0}, {r1}) must be non-empty, inside [0, {B}) and after the "
+                             f"previous group's rows")
+        if target < 1:
+            raise ValueError(f"fit group {i}: target of {target} frames (at least 1)")
+        end = r1
+    cols = [torch.tensor(c, dtype=torch.int64, device=device) for c in zip(*fit)]
+    return (*cols, *FIT_SCALE_RANGE)
 
 
 class TtsPool:
@@ -537,13 +563,14 @@ class NativeSynthesizer:
     @torch.no_grad()
     def infer_ragged(self, x, x_lengths, sid=None, noise_scale=1, length_scale=1, noise_scale_w=1.0, sdp_ratio=0.2,
                      seed: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
-                     streams: Optional[Sequence[int]] = None, g=None) -> Tuple[torch.Tensor, List[int]]:
+                     streams: Optional[Sequence[int]] = None, g=None, fit=None) -> Tuple[torch.Tensor, List[int]]:
         """The audio of ``infer(..., ragged=True, latents=False)`` (same arguments and draws) left on the device, with
         each row's decoded frames on the host: (o [B, hop * max(frames)], frames).  Row b's samples are
-        o[b, : hop * frames[b]], zeros after.  One host sync (y_lengths), as in ``infer``."""
+        o[b, : hop * frames[b]], zeros after.  One host sync (y_lengths), as in ``infer``.  ``fit`` as in
+        ``tts_encode``."""
         a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams, g)
-        y_lengths, _, _ = self.native.tts_encode(a["x"], a["x_lengths"], a["sid"], seed=a["seed"], items=a["enc_items"],
-                                                 g=a["g"], **a["enc_scalars"])
+        y_lengths = self.native.tts_encode(a["x"], a["x_lengths"], a["sid"], seed=a["seed"], items=a["enc_items"],
+                                           g=a["g"], fit=fit_groups(fit, a["B"], self.device), **a["enc_scalars"])[0]
         frames = [int(v) for v in y_lengths.cpu()]             # the sync
         o, _ = self.native.tts_decode(a["B"], max(frames), self.device, seed=a["seed"] + 1,
                                       noise_scale=float(a["noise_scale"]), ragged=True, latents=False,
@@ -636,7 +663,7 @@ class NativeSynthesizer:
     def tts_encode(self, x, x_lengths, sid=None, noise_scale=1, length_scale=1, noise_scale_w=1.0, sdp_ratio=0.2,
                    seed: Optional[int] = None, seeds: Optional[Sequence[int]] = None,
                    streams: Optional[Sequence[int]] = None, pool: Optional["TtsPool"] = None,
-                   rows: Optional[Sequence[int]] = None, g=None) -> "TtsState":
+                   rows: Optional[Sequence[int]] = None, g=None, fit=None) -> "TtsState":
         """The encode half of ``infer`` (same arguments and draws), returning state the caller owns: a later
         ``tts_encode`` or ``infer`` does not change it.  ``tts_decode_windows`` decodes any frames of its rows, each
         row with the decode key, stream and noise scale ``infer`` would give it.  One host sync (y_lengths), as in
@@ -649,7 +676,13 @@ class NativeSynthesizer:
         ``g`` as in ``infer``.  With per-token vectors the state's g is [B, gin, T] (include/ovc.h:
         ovc_tts_encode_state_tokens), and a pool turns per-token (``TtsPool.to_per_token``).  Into a per-token pool,
         rows with one vector (or a speaker id) are encoded with it in every token column, which gives the same
-        values."""
+        values.
+
+        ``fit``: ``[(row0, row1, target_frames), ...]``, runs of rows whose frames are fitted to a target (include/ovc.h:
+        ovc_tts_encode_fit): every row of a group is encoded at the smallest length scale s in ``FIT_SCALE_RANGE``
+        whose group frames sum_r max(1, sum_t ceil(exp(logw_r[t]) * s)) reach the target (the range's top when none
+        does), exactly as an encode given s as the row's ``length_scale``.  Rows outside every group keep their
+        ``length_scale``.  The state's ``length_scale`` then lists each row's scale."""
         a = self._tts_args(x, x_lengths, sid, noise_scale, length_scale, noise_scale_w, sdp_ratio, seed, seeds, streams, g)
         x = a["x"]
         B, T = x.shape
@@ -667,15 +700,18 @@ class NativeSynthesizer:
             if len(rows) != B or min(rows) < 0:
                 raise ValueError(f"tts_encode: {len(rows)} pool rows for {B} encoded rows (each >= 0)")
             pool.fit(max(rows) + 1, T)
-        y_lengths, _, _ = self.native.tts_encode(x, a["x_lengths"], a["sid"], seed=a["seed"], items=a["enc_items"],
-                                                 g=a["g"], **a["enc_scalars"])
+        groups = fit_groups(fit, B, self.device)
+        enc = self.native.tts_encode(x, a["x_lengths"], a["sid"], seed=a["seed"], items=a["enc_items"], g=a["g"],
+                                     fit=groups, **a["enc_scalars"])
+        y_lengths = enc[0]
         if pool is None:
             stats, cum, g = self.native.tts_encode_state(B, T, self.device, per_token=per_token)
         else:
             stats, cum, g, _ = self.native.tts_state_rows(rows, pool.stats, pool.cum, pool.g, pool.y_lengths)
         frames = [int(v) for v in y_lengths.cpu()]             # the sync
+        scales = enc[3].cpu().tolist() if groups is not None else None
         return TtsState(stats, cum, g, y_lengths if pool is None else pool.y_lengths, frames, a["dec_keys"],
-                        a["dec_streams"], a["dec_noise_scale"])
+                        a["dec_streams"], a["dec_noise_scale"], scales)
 
     @torch.no_grad()
     def tts_decode_windows(self, state: "TtsState", windows: Sequence[Tuple[int, int, int]], w_max: Optional[int] = None,
@@ -868,7 +904,12 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
         drawn from torch's global generator), ``noise_scale`` (0.667), ``noise_scale_w`` (0.6), ``sdp_ratio`` (0.2).
         Sentence j of request r draws at (seed_r, stream j) with request r's parameters, so each returned array equals
         ``audio_numpy_concat(tts_from_ids(ids, speaker, speed=..., seed=seed_r, ...), sr, speed)`` bit for bit: the
-        sentences joined with 50 ms / speed gaps, as ``tts`` does.  Returns one array per request."""
+        sentences joined with 50 ms / speed gaps, as ``tts`` does.  Returns one array per request.
+
+        ``duration`` (seconds) fits the request to that length: its sentences are one fit group (``fit_target``) whose
+        length scale the encode solves on the device, and ``speed`` then only sets the gaps.  The array has at least
+        round(duration * sr) samples, and less than one hop more unless two tokens change length at the same scale or
+        the scale reaches an end of ``FIT_SCALE_RANGE``."""
         reqs = list(requests)
         seqs, sid, owner, speeds, kw = self._request_sentences(reqs)
         sr = self.hps.data.sampling_rate
@@ -885,12 +926,15 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
         sentence and the speaker ids are placeholders."""
         seqs, sid, seeds, streams, owner, rows = [], [], [], [], [], []
         par = {"noise_scale": [], "noise_scale_w": [], "length_scale": [], "sdp_ratio": []}
-        speeds = []
+        speeds, fit = [], []
         for r, q in enumerate(reqs):
             ids = [list(q_ids) for q_ids in (q["ids"] if "ids" in q else self._sentences(q["text"], q.get("language", "English")))]
             k = self._request_keys(q, f"request {r}")
             self._check_speaker_tokens(k["g"], [len(q_ids) for q_ids in ids], f"request {r}")
             speeds.append(k["speed"])
+            if k["duration"] is not None and ids:
+                target = self.fit_target(k["duration"], len(ids), k["speed"], True, f"request {r}")
+                fit.append((len(seqs), len(seqs) + len(ids), target))
             o = 0
             for j, q_ids in enumerate(ids):
                 seqs.append(q_ids)
@@ -902,6 +946,8 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
                 owner.append(r)
                 self._sentence_params(k, par)
         kw = dict(seeds=seeds, streams=streams, **par)
+        if fit:
+            kw["fit"] = fit
         g = self._speaker_rows(rows, max((len(q) for q in seqs), default=1))
         if g is not None:
             kw["g"] = g
@@ -922,10 +968,34 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
         speed = float(q.get("speed", 1.0))
         if not (math.isfinite(speed) and speed > 0):
             raise ValueError(f"{who}: speed {speed!r} must be a positive number")
+        duration = self._check_duration(q.get("duration"), who)
         seed = q.get("seed")
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if seed is None else check_seeds([seed], 1, "seed")[0]
         return dict(speaker=spk, g=g, speed=speed, seed=seed, noise_scale=float(q.get("noise_scale", 0.667)),
-                    noise_scale_w=float(q.get("noise_scale_w", 0.6)), sdp_ratio=float(q.get("sdp_ratio", 0.2)))
+                    noise_scale_w=float(q.get("noise_scale_w", 0.6)), sdp_ratio=float(q.get("sdp_ratio", 0.2)),
+                    duration=duration)
+
+    @staticmethod
+    def _check_duration(duration, who: str) -> Optional[float]:
+        if duration is None:
+            return None
+        duration = float(duration)
+        if not (math.isfinite(duration) and duration > 0):
+            raise ValueError(f"{who}: duration {duration!r} must be a positive number of seconds")
+        return duration
+
+    def fit_target(self, duration: float, n: int, speed: float, gaps: bool, who: str) -> int:
+        """Frames F* that ``n`` sentences must fill to last ``duration`` seconds: ceil((N* - gaps) / hop), N* =
+        round(duration * sr) samples and gaps = n * int(sr * 0.05 / speed), the silences ``audio_numpy_concat`` appends
+        (0 without ``gaps``).  ValueError naming ``who`` when that leaves less than one frame per sentence."""
+        sr, hop = int(self.hps.data.sampling_rate), int(self.hps.data.hop_length)
+        total = int(round(duration * sr))
+        silence = n * int((sr * 0.05) / speed) if gaps else 0
+        target = -(-(total - silence) // hop)
+        if target < n:
+            raise ValueError(f"{who}: duration {duration} s is too short for {n} sentence(s): it needs more than "
+                             f"{(silence + (n - 1) * hop) / sr:.4f} s (the gaps and one {hop}-sample frame per sentence)")
+        return target
 
     @staticmethod
     def _sentence_params(k: dict, par: dict) -> None:
@@ -952,7 +1022,8 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
         of every unfinished request and yields one chunk per such request, in request order.  A request's sentences are
         decoded in order: the first sentence in windows of ``first_window_frames`` then ``window_frames`` frames, the
         others in windows of ``window_frames``, each decoded with ``TTS_HALO_FRAMES`` frames of context on both sides
-        (``plan_tts_windows``); a sentence's last chunk ends with its 50 ms / speed of silence.  A request's chunks
+        (``plan_tts_windows``); a sentence's last chunk ends with its 50 ms / speed of silence.  A ``duration`` key fits
+        the request as in ``tts_batch``.  A request's chunks
         concatenate to ``tts_batch``'s array for it (same length, same gaps) within fp32 reordering (2e-6 of its rms),
         whatever requests it is batched with.  Malformed requests (an empty one, a speed <= 0, a bad seed) or window
         sizes < 1 raise ValueError here, before anything is launched."""
@@ -989,13 +1060,14 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
                 yield r, np.concatenate([chunk, np.zeros(gap, np.float32)]) if gap else chunk.copy()
 
     def tts_stream(self, text=None, speaker=None, language="English", speed=1.0, seed: Optional[int] = None, ids=None,
-                   window_frames: int = 256, first_window_frames: int = 32) -> Iterator[np.ndarray]:
+                   window_frames: int = 256, first_window_frames: int = 32,
+                   duration: Optional[float] = None) -> Iterator[np.ndarray]:
         """``tts`` as a stream of float32 chunks (``tts_stream_batch`` with one request): the first chunk is
         ``first_window_frames`` frames of audio, available once the encode and one small decode have run.  ``ids``
         (token-id lists, one per sentence) replaces ``text``.  The chunks concatenate to ``tts(text, None, speaker,
         language, speed, seed)`` within 2e-6 of its rms, with the same length and the same silences.  Feeding them to
-        ``streaming.StreamingConverter.push`` gives cloned-voice streaming."""
-        q = dict(speaker=speaker, speed=speed, seed=seed)
+        ``streaming.StreamingConverter.push`` gives cloned-voice streaming.  ``duration`` as in ``tts``."""
+        q = dict(speaker=speaker, speed=speed, seed=seed, duration=duration)
         q.update({"ids": ids} if ids is not None else {"text": text, "language": language})
         gen = self.tts_stream_batch([q], window_frames=window_frames, first_window_frames=first_window_frames)
         return (chunk for _, chunk in gen)
@@ -1010,13 +1082,19 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
 
     @torch.no_grad()
     def tts_from_ids(self, sequences, speaker, speed=1.0, noise_scale=0.667, noise_scale_w=0.6, sdp_ratio=0.2,
-                     seed: Optional[int] = None) -> List[np.ndarray]:
+                     seed: Optional[int] = None, duration: Optional[float] = None) -> List[np.ndarray]:
         """All sentences in ONE batched infer() (the reference loops over them at batch 1, api.py:79-91); every
         sentence gets what its own batch-1 call would give (ragged decode).  ``seed``: the call's key (sentence j
         draws at stream j); default: one drawn from torch's global generator.  ``speaker``: a style name or id, a
         speaker vector ([gin] or [1, gin, 1], e.g. a blend of ``style`` rows), a ``ToneTrack`` keyed in token positions
         of the whole call (sentence j's tokens at [o_j, o_j + n_j)) or a [1, gin, N] per-token tensor with N the
-        call's token count; ValueError for anything else."""
+        call's token count; ValueError for anything else.  ``duration`` (seconds of speech: the sentences are returned
+        without gaps) fits all the sentences as one group, as ``tts_batch`` does, and replaces ``speed``."""
+        return self._from_ids(sequences, speaker, speed, noise_scale, noise_scale_w, sdp_ratio, seed, duration, False)
+
+    def _from_ids(self, sequences, speaker, speed, noise_scale, noise_scale_w, sdp_ratio, seed, duration, gaps):
+        """``tts_from_ids``; a ``duration`` counts the gaps ``audio_numpy_concat`` adds when ``gaps`` is set."""
+        duration = self._check_duration(duration, "duration")
         sequences = [list(q) for q in sequences]
         speaker_id, entry = self._speaker(speaker, "speaker")
         self._check_speaker_tokens(entry, [len(q) for q in sequences], "speaker")
@@ -1026,14 +1104,19 @@ class BaseSpeakerTTS(OpenVoiceBaseClass):
         offs = np.cumsum([0] + [len(q) for q in sequences]).tolist()
         g = self._speaker_rows([(speaker_id, entry, offs[j], len(q)) for j, q in enumerate(sequences)],
                                max(len(q) for q in sequences))
+        extra = {} if g is None else {"g": g}
+        if duration is not None:
+            extra["fit"] = [(0, n, self.fit_target(duration, n, speed, gaps, "duration"))]
         return self._infer_sentences(sequences, [0 if speaker_id is None else speaker_id] * n, noise_scale=noise_scale,
                                      noise_scale_w=noise_scale_w, length_scale=1.0 / speed, sdp_ratio=sdp_ratio, seed=seed,
-                                     **({} if g is None else {"g": g}))
+                                     **extra)
 
-    def tts(self, text, output_path, speaker, language="English", speed=1.0, seed: Optional[int] = None):
-        """openvoice/api.py:73-98.  ``seed``: the request's key (``tts_from_ids``); same seed, same audio."""
+    def tts(self, text, output_path, speaker, language="English", speed=1.0, seed: Optional[int] = None,
+            duration: Optional[float] = None):
+        """openvoice/api.py:73-98.  ``seed``: the request's key (``tts_from_ids``); same seed, same audio.
+        ``duration`` (seconds, gaps included) fits the utterance as ``tts_batch`` does; ``speed`` then sets the gaps."""
         sequences = self._sentences(text, language)
-        audio_list = self.tts_from_ids(sequences, speaker, speed=speed, seed=seed)
+        audio_list = self._from_ids(sequences, speaker, speed, 0.667, 0.6, 0.2, seed, duration, True)
         audio = self.audio_numpy_concat(audio_list, sr=self.hps.data.sampling_rate, speed=speed)
         if output_path is None:
             return audio
@@ -1280,7 +1363,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
         ``convert(...)`` gives, without the audio leaving the GPU in between.  A request is a ``tts.tts_batch`` request
         dict plus ``src_se`` and ``tgt_se`` (required; [1, gin, 1] embeddings), ``tau`` (0.3), ``convert_seed`` (the
         conversion's key; default: drawn from torch's generator, as ``seed`` is) and ``message`` (watermark payload,
-        applied on the host as ``convert_batch`` applies it).
+        applied on the host as ``convert_batch`` applies it).  A ``duration`` key fits the TTS half as ``tts_batch``
+        does; the converted audio keeps ``convert``'s length, hop * floor(L / hop) for an utterance of L samples.
 
         One ragged TTS encode + decode of every sentence (one host sync, for the frame counts), then per chunk of
         ``max_batch`` requests (sorted by length, as ``convert_batch`` chunks) one ``ovc_splice`` that builds the
@@ -1332,7 +1416,8 @@ class ToneColorConverter(OpenVoiceBaseClass):
         ``CloneSessions.step``, one batched launch sequence over every unfinished request: ONE ``tts_decode_windows``
         call decodes, per request, the next TTS windows (``plan_tts_windows``: ``first_window_frames`` then
         ``window_frames`` frames) until its converter can emit a window or its text is done; ONE ``ovc_splice`` writes
-        the windows' interiors and the sentences' 50 ms / speed gaps into the converter's rings; then one ring
+        the windows' interiors and the sentences' 50 ms / speed gaps into the converter's rings (a ``duration`` key is
+        ``CloneSessions.say(duration=)``); then one ring
         spectrogram and ragged conversion of every ready window, and one download.  A request is closed in the step
         that writes its last gap.  Every step yields one non-empty chunk per unfinished request, in
         request order; a request's chunks concatenate to its ``clone_batch`` array (same length; the TTS windows equal
@@ -1344,12 +1429,13 @@ class ToneColorConverter(OpenVoiceBaseClass):
         (seqs, _, owner, speeds, kw), _, _, taus, seeds, _ = self._clone_requests(tts, reqs)
         if not reqs:
             return iter(())
+        targets = {row0: target for row0, _, target in kw.get("fit", [])}
         for r, q in enumerate(reqs):                     # session r is request r, with the keys drawn above
             mine = [i for i, o in enumerate(owner) if o == r]
             keys = {k: q[k] for k in CloneSessions.OPEN_KEYS if k in q}
             keys.update(seed=kw["seeds"][mine[0]], convert_seed=seeds[r], tau=taus[r], speed=speeds[r])
             sid = cs.open(**keys)
-            cs._queue(sid, [seqs[i] for i in mine])       # checked by the encode below, for the whole call
+            cs._queue(sid, [seqs[i] for i in mine], targets.get(mine[0]))   # checked by the encode below
             cs.end(sid)
         cs.encode_pending()
         return self._clone_stream(cs)

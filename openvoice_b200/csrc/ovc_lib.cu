@@ -2098,7 +2098,7 @@ static int check_tts_per_frame_cond(const ovc_ctx* c) {
 static int tts_encode_any(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid, const float* g,
                           int g_tokens, const float* noise_w, uint64_t seed, float noise_scale_w, float length_scale,
                           float sdp_ratio, int B, int T, int64_t* y_lengths, float* w_ceil, float* logw, void* stream,
-                          const ovc_item_params* items) {
+                          const ovc_item_params* items, const ovc_tts_fit* fit = nullptr) {
   if (!c) return fail(OVC_ERR_INVALID, "null context");
   if (!c->finalized) return fail(OVC_ERR_STATE, "ovc_finalize_weights has not been called");
   if (!c->tts.ready) return fail(OVC_ERR_STATE, "the checkpoint has no TTS members (enc_p / dp / sdp / emb_g): not a V1 base speaker");
@@ -2108,11 +2108,20 @@ static int tts_encode_any(ovc_ctx* c, const int64_t* tokens, const int64_t* x_le
   if (B < 1 || T < 1) return fail(OVC_ERR_INVALID, "B and T must be positive (got %d, %d)", B, T);
   if (B > 65535 || (long long)T * T > 2000000000LL / 256) return fail(OVC_ERR_INVALID, "B %d / T %d exceed the grid limits", B, T);
   if (!(length_scale > 0.f)) return fail(OVC_ERR_INVALID, "length_scale must be positive");
+  TtsFit tf{};
+  if (fit) {
+    if (fit->G < 1 || fit->G > B) return fail(OVC_ERR_INVALID, "fit: G = %d groups for B = %d rows (1 <= G <= B)", fit->G, B);
+    if (!fit->row0 || !fit->row1 || !fit->target_frames || !fit->length_scale) return fail(OVC_ERR_INVALID, "fit: null array");
+    if (!(fit->scale_lo > 0.f && fit->scale_lo <= fit->scale_hi && std::isfinite(fit->scale_hi)))
+      return fail(OVC_ERR_INVALID, "fit: scale range [%g, %g] must satisfy 0 < lo <= hi < inf", fit->scale_lo, fit->scale_hi);
+    tf = TtsFit{(const long long*)fit->row0, (const long long*)fit->row1, (const long long*)fit->target_frames, fit->G,
+                fit->scale_lo, fit->scale_hi, fit->length_scale};
+  }
   ON_DEVICE(c);
   c->ev_used = c->prof ? c->ev_used : 0;
   return run_tts_encode(c, (const long long*)tokens, (const long long*)x_lengths, (const long long*)sid, g, g_tokens, noise_w,
                         seed, noise_scale_w, length_scale, sdp_ratio, B, T, (long long*)y_lengths, w_ceil, logw,
-                        item_params(items), (cudaStream_t)stream);
+                        item_params(items), (cudaStream_t)stream, fit ? &tf : nullptr);
 }
 
 int ovc_tts_encode_items(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid, const float* noise_w,
@@ -2129,6 +2138,16 @@ int ovc_tts_encode_g(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths
   if (!g) return fail(OVC_ERR_INVALID, "null tensor argument");
   return tts_encode_any(c, tokens, x_lengths, nullptr, g, g_tokens, noise_w, seed, noise_scale_w, length_scale, sdp_ratio, B,
                         T, y_lengths, w_ceil, logw, stream, items);
+}
+
+int ovc_tts_encode_fit(ovc_ctx* c, const int64_t* tokens, const int64_t* x_lengths, const int64_t* sid, const float* g,
+                       int g_tokens, const float* noise_w, uint64_t seed, float noise_scale_w, float length_scale,
+                       float sdp_ratio, int B, int T, int64_t* y_lengths, float* w_ceil, float* logw, void* stream,
+                       const ovc_item_params* items, const ovc_tts_fit* fit) {
+  if (!sid == !g) return fail(OVC_ERR_INVALID, "ovc_tts_encode_fit takes exactly one of sid and g");
+  if (!fit) return fail(OVC_ERR_INVALID, "null fit");
+  return tts_encode_any(c, tokens, x_lengths, sid, g, sid ? 0 : g_tokens, noise_w, seed, noise_scale_w, length_scale,
+                        sdp_ratio, B, T, y_lengths, w_ceil, logw, stream, items, fit);
 }
 
 int ovc_tts_decode(ovc_ctx* c, const float* noise, uint64_t seed, float noise_scale, int B, int Ymax, int max_len, int ragged,

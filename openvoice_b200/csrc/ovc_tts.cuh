@@ -363,6 +363,67 @@ __global__ void tts_durations_kernel(const float* logw_sdp, const float* logw_dp
                                     cum + o);
 }
 
+// Fit groups of ovc_tts_encode_fit (include/ovc.h: ovc_tts_fit), all device arrays
+struct TtsFit {
+  const long long* row0;     // [G] first row of group g
+  const long long* row1;     // [G] one past its last row
+  const long long* target;   // [G] frames
+  int G;
+  float lo, hi;              // the scale range
+  float* scale;              // [B] out: every row's length scale
+};
+
+// CTA g fits group g (ovc_tts::fit_* on the logw tts_durations_kernel wrote) and writes its scale to the group's rows;
+// it also writes the unfitted rows between the previous group and this one (and the last CTA those after every
+// group) with the scale they have without a fit.  Row ranges are clamped into [0, B), each to start at or after the
+// previous group's end, so no two groups share a row; targets below 1 count as 1.  Warp w sums rows r0 + w, r0 + w + 8,
+// ... with its lanes striding over the row's tokens, so a row may be longer than the CTA.  grid (G), 256 threads
+constexpr int TTS_FIT_THREADS = 256;
+__global__ void __launch_bounds__(TTS_FIT_THREADS) tts_fit_kernel(const float* __restrict__ logw, const long long* lens, int B,
+                                                                  int T, TtsFit fit, float length_scale,
+                                                                  const float* it_length_scale) {
+  __shared__ long long s_part[TTS_FIT_THREADS / 32];
+  __shared__ long long s_total;
+  const int g = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  long long prev_end = 0, r0 = 0, r1 = 0;
+  for (int k = 0; k <= g; ++k) {
+    prev_end = r1;
+    r0 = min(max(fit.row0[k], prev_end), (long long)B);
+    r1 = min(max(fit.row1[k], r0), (long long)B);
+  }
+  for (long long b = prev_end + threadIdx.x; b < r0; b += blockDim.x)
+    fit.scale[b] = it_length_scale ? it_length_scale[b] : length_scale;
+  if (g == fit.G - 1)
+    for (long long b = r1 + threadIdx.x; b < B; b += blockDim.x) fit.scale[b] = it_length_scale ? it_length_scale[b] : length_scale;
+  const long long target = max(fit.target[g], 1LL);
+  ovc_tts::FitSearch f = ovc_tts::fit_begin(fit.lo, fit.hi);
+  while (!ovc_tts::fit_done(f)) {                    // f is the same in every thread: the loop is CTA-uniform
+    const float s = ovc_tts::fit_probe(f);
+    long long acc = 0;
+    for (long long r = r0 + warp; r < r1; r += TTS_FIT_THREADS / 32) {
+      const int len = tts_len(lens, (int)r, T);
+      const float* lw = logw + r * T;
+      long long n = 0;
+      for (int t = lane; t < len; t += 32) n += ovc_tts::token_frames_int(expf(lw[t]), s);
+#pragma unroll
+      for (int m = 16; m > 0; m >>= 1) n += __shfl_xor_sync(0xffffffffu, n, m);
+      acc += n < 1 ? 1 : n;
+    }
+    if (lane == 0) s_part[warp] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      long long tot = 0;
+      for (int w = 0; w < TTS_FIT_THREADS / 32; ++w) tot += s_part[w];
+      s_total = tot;
+    }
+    __syncthreads();
+    ovc_tts::fit_step(f, s_total >= target);
+    __syncthreads();                                 // s_part / s_total are rewritten by the next step
+  }
+  const float s = ovc_tts::fit_result(f);
+  for (long long b = r0 + threadIdx.x; b < r1; b += blockDim.x) fit.scale[b] = s;
+}
+
 // Windows of ovc_tts_decode_windows: output row w expands encoded row row[w] at absolute frames frame0[w] + t,
 // t < len[w].  Every pointer NULL: output row b is encoded row b from frame 0 (the whole decode).
 struct TtsWindows {

@@ -12,6 +12,7 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+#include <string.h>
 
 #if defined(__CUDACC__)
 #define OVC_HD __host__ __device__ __forceinline__
@@ -189,6 +190,9 @@ OVC_HD float convflow_tail(const float* h_row, const float* pw, const float* pb,
   return rq_spline_inverse(x1, p, sqrtf((float)C), bound);
 }
 
+// ---- one token's frames at length scale s, from e = expf(logw)                models.py:477-478
+OVC_HD float token_frames(float e, float s) { return ceilf(e * s); }
+
 // ---- durations of one utterance (serial over tokens)                          models.py:474-481
 // logw = sdp * ratio + dp * (1 - ratio);  w = exp(logw) * mask * length_scale;  w_ceil = ceil(w);
 // cum[t] = inclusive prefix sum (commons.generate_path, commons.py:135);  returns y_length = max(1, sum)
@@ -200,7 +204,7 @@ OVC_HD long long durations_row(const float* logw_sdp, const float* logw_dp, floa
     float lw = 0.f, wc = 0.f;
     if (t < len) {
       lw = logw_sdp[t] * ratio + logw_dp[t] * (1.f - ratio);
-      wc = ceilf(expf(lw) * length_scale);
+      wc = token_frames(expf(lw), length_scale);
     }
     logw[t] = lw;
     w_ceil[t] = wc;
@@ -210,6 +214,50 @@ OVC_HD long long durations_row(const float* logw_sdp, const float* logw_dp, floa
   }
   const long long n = (long long)total;
   return n < 1 ? 1 : n;
+}
+
+// ---- duration fit (ovc_tts_encode_fit)
+// A fit group is a run of rows [r0, r1) with a target of F* frames.  Its frames at scale s are
+// F(s) = sum_r max(1, sum_{t < len_r} token_frames(expf(logw_r[t]), s)), durations_row's y_lengths at length_scale = s.
+// The fitted scale is the smallest fp32 s in [lo, hi] with F(s) >= F*, or hi when there is none.  F is monotone
+// non-decreasing in s (fp32 rounding of a product with a positive factor is monotone, and so is ceilf), and the bit
+// patterns of positive floats are ordered as their values, so a bisection over the patterns in [lo, hi] finds s in
+// about 25 steps.  Frames add up in integers, so the order of the sum cannot change it.
+OVC_HD long long token_frames_int(float e, float s) {
+  const float wc = token_frames(e, s);
+  return wc < 1073741824.f ? (long long)wc : 1073741824LL;   // a NaN or a count past 2^30 saturates instead of overflowing
+}
+
+OVC_HD uint32_t fit_bits(float s) { uint32_t u; memcpy(&u, &s, sizeof u); return u; }
+OVC_HD float fit_float(uint32_t u) { float s; memcpy(&s, &u, sizeof s); return s; }
+
+struct FitSearch { uint32_t lo, hi; };   // the answer's bit pattern lies in [lo, hi]
+OVC_HD FitSearch fit_begin(float scale_lo, float scale_hi) { return FitSearch{fit_bits(scale_lo), fit_bits(scale_hi)}; }
+OVC_HD bool fit_done(const FitSearch& f) { return f.lo >= f.hi; }
+OVC_HD float fit_probe(const FitSearch& f) { return fit_float(f.lo + (f.hi - f.lo) / 2); }
+OVC_HD void fit_step(FitSearch& f, bool reached) {   // reached: F(fit_probe(f)) >= F*
+  const uint32_t mid = f.lo + (f.hi - f.lo) / 2;
+  if (reached) f.hi = mid; else f.lo = mid + 1;
+}
+OVC_HD float fit_result(const FitSearch& f) { return fit_float(f.lo); }
+
+// F(s) of rows [r0, r1) of e = expf(logw) [rows][T], lens clamped into [0, T] (serial: the host statement of the rule)
+OVC_HD long long fit_group_frames(const float* e, const long long* lens, int T, long long r0, long long r1, float s) {
+  long long F = 0;
+  for (long long r = r0; r < r1; ++r) {
+    const int len = lens[r] < 0 ? 0 : (lens[r] > T ? T : (int)lens[r]);
+    long long n = 0;
+    for (int t = 0; t < len; ++t) n += token_frames_int(e[r * T + t], s);
+    F += n < 1 ? 1 : n;
+  }
+  return F;
+}
+
+OVC_HD float fit_scale(const float* e, const long long* lens, int T, long long r0, long long r1, long long target,
+                       float scale_lo, float scale_hi) {
+  FitSearch f = fit_begin(scale_lo, scale_hi);
+  while (!fit_done(f)) fit_step(f, fit_group_frames(e, lens, T, r0, r1, fit_probe(f)) >= target);
+  return fit_result(f);
 }
 
 // ---- frame -> token: first token whose cumulative duration exceeds y          commons.py:136-141

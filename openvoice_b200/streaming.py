@@ -1352,6 +1352,10 @@ class CloneSessions:
         self.sessions: Dict[int, _CloneSession] = {}
         self.next_id = 0
         self.pending: List[Tuple[int, List[int]]] = []   # (session, token ids) said since the last encode, in order
+        # beside each pending sentence: None, or (say number, target frames), shared by the sentences of one
+        # say(duration=), which the encode fits as one group
+        self.pending_fit: List[Optional[Tuple[int, int]]] = []
+        self.says = 0
         self.ss: Optional[StreamingSessions] = None       # the converter side, made with the first audio
         if self.output_rates:                             # ... or here, where its filter banks may wait for the device
             self.ss = StreamingSessions(converter, window_frames=W, rates=self.output_rates)
@@ -1401,12 +1405,22 @@ class CloneSessions:
         return s
 
     def say(self, sid: int, text: Optional[str] = None, ids: Optional[Sequence[Sequence[int]]] = None,
-            language: str = "English") -> None:
+            language: str = "English", duration: Optional[float] = None) -> None:
         """Queue sentences for session ``sid``: ``ids`` (token-id lists, one per sentence) or ``text`` through the TTS
         model's front end.  They are encoded in the next ``step``.  ValueError for an unknown or ended session, no
         sentences, a token id outside the vocabulary or a session speaker outside the checkpoint's speakers
-        (``NativeSynthesizer.check_tts_input``, the encode's own check); the session keeps what it had said before."""
+        (``NativeSynthesizer.check_tts_input``, the encode's own check); the session keeps what it had said before.
+
+        ``duration`` (seconds) fits these sentences and their 50 ms / speed gaps to that length, as a ``tts_batch``
+        request with ``duration`` is fitted (``BaseSpeakerTTS.fit_target``): they form one fit group of the step's
+        encode, which fits the groups of every session at once.  ValueError for a duration that is not positive and
+        finite or too short for the gaps and one frame per sentence."""
         ids = self._sentences(sid, text, ids, language)
+        target = None
+        if duration is not None:
+            who = f"{self.label} {sid}"
+            target = self.tts.fit_target(self.tts._check_duration(duration, who), len(ids),
+                                         self.sessions[sid].tts_keys["speed"], True, who)
         flat = [t for q in ids for t in q]
         keys = self.sessions[sid].tts_keys
         try:
@@ -1421,7 +1435,7 @@ class CloneSessions:
         if torch.is_tensor(e) and e.dim() == 2 and n > e.shape[1]:
             raise ValueError(f"{self.label} {sid}: its per-token speaker tensor has {e.shape[1]} columns, the session "
                              f"would reach {n} tokens")
-        self._queue(sid, ids)
+        self._queue(sid, ids, target)
 
     def _sentences(self, sid, text, ids, language) -> List[List[int]]:
         s = self._session(sid)
@@ -1436,11 +1450,15 @@ class CloneSessions:
             raise ValueError(f"{self.label} {sid}: no sentences to say")
         return ids
 
-    def _queue(self, sid: int, ids: List[List[int]]) -> None:
-        """``say`` after its checks.  ``clone_stream_batch`` queues here: its eager encode checks every sentence of the
-        call before the generator is returned, so a bad request fails the whole call and no step ever runs."""
+    def _queue(self, sid: int, ids: List[List[int]], target: Optional[int] = None) -> None:
+        """``say`` after its checks (``target``: the frames to fit the sentences to, or None).  ``clone_stream_batch``
+        queues here: its eager encode checks every sentence of the call before the generator is returned, so a bad
+        request fails the whole call and no step ever runs."""
         s = self.sessions[sid]
+        fit = None if target is None else (self.says, int(target))
+        self.says += 1
         self.pending += [(sid, q) for q in ids]
+        self.pending_fit += [fit] * len(ids)
         s.said += len(ids)
         s.unencoded += len(ids)
         s.tokens += sum(len(q) for q in ids)
@@ -1455,7 +1473,8 @@ class CloneSessions:
     def cancel(self, sid: int) -> None:
         """Drop session ``sid`` now: its queued text, pool rows and converter row are freed; it returns nothing more."""
         s = self._session(sid)
-        self.pending = [(o, q) for o, q in self.pending if o != sid]
+        keep = [i for i, (o, _) in enumerate(self.pending) if o != sid]
+        self.pending, self.pending_fit = [self.pending[i] for i in keep], [self.pending_fit[i] for i in keep]
         self.free_rows += sorted({p[0] for p in s.plans})
         if s.ss_id is not None:
             self.ss.discard([s.ss_id])
@@ -1492,6 +1511,15 @@ class CloneSessions:
         kw = {"seeds": [], "streams": [], "noise_scale": [], "noise_scale_w": [], "length_scale": [], "sdp_ratio": []}
         nth: Dict[int, int] = {}
         at: Dict[int, int] = {}                           # next token position of each session in this encode
+        fit: List[List[int]] = []                         # [row0, row1, target] of each say(duration=) in the encode
+        for i, f in enumerate(self.pending_fit):
+            if f is not None:
+                if fit and fit[-1][1] == i and self.pending_fit[i - 1] == f:
+                    fit[-1][1] = i + 1
+                else:
+                    fit.append([i, i + 1, f[1]])
+        if fit:
+            kw["fit"] = fit
         for sid, q in self.pending:
             s = self.sessions[sid]
             j = s.said - s.unencoded + nth.get(sid, 0)    # the sentence's number in its session
@@ -1530,7 +1558,7 @@ class CloneSessions:
             s.length += self.hop * frames + gap
             s.unencoded -= 1
             s.tokens_encoded += len(seqs[i])
-        self.pending = []
+        self.pending, self.pending_fit = [], []
 
     @torch.no_grad()
     def step(self) -> Dict[int, np.ndarray]:
